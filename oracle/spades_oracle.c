@@ -194,6 +194,27 @@ const uint64_t *orc_kset_keys(const kset_t *s) { return s->keys; }
 const uint32_t *orc_kset_counts(const kset_t *s) { return s->counts; }
 const int64_t *orc_kset_bsz(const kset_t *s) { return s->bsz; }
 
+/* a k-mer set from caller arrays (copied): n records of nwords(K) words in bucket-major order, counts (NULL: no
+ * multiplicities), B bucket sizes adding up to n. Lets a check build the MPHF of any bucket layout, e.g. the buckets
+ * one rank of a distributed count owns. */
+kset_t *orc_kset_from_arrays(const uint64_t *keys, const uint32_t *counts, const int64_t *bsz, int64_t n, int K, int B) {
+    int nw = nwords(K);
+    int64_t tot = 0;
+    for (int b = 0; b < B; ++b) tot += bsz[b];
+    if (tot != n || n < 0 || B < 1) return NULL;
+    kset_t *s = (kset_t *)calloc(1, sizeof(kset_t));
+    s->K = K; s->nw = nw; s->B = B; s->n = n;
+    s->bsz = (int64_t *)malloc((size_t)B * 8);
+    memcpy(s->bsz, bsz, (size_t)B * 8);
+    s->keys = (uint64_t *)malloc((size_t)(n ? n : 1) * nw * 8);
+    memcpy(s->keys, keys, (size_t)n * nw * 8);
+    if (counts) {
+        s->counts = (uint32_t *)malloc((size_t)(n ? n : 1) * 4);
+        memcpy(s->counts, counts, (size_t)n * 4);
+    }
+    return s;
+}
+
 typedef struct { uint64_t *rec; int64_t n, cap; int rw; } recvec_t;   /* records: [bucket, w0..w(nw-1)] */
 static void rv_push(recvec_t *v, uint64_t b, const uint64_t *w, int nw) {
     if (v->n == v->cap) { v->cap = v->cap ? v->cap * 2 : 1024; v->rec = (uint64_t *)realloc(v->rec, (size_t)v->cap * v->rw * 8); }

@@ -9,10 +9,19 @@ _CTX = None
 
 
 def ctx():
+    """the session's shared context on device 0 (default arena: most of the free device memory), created on first use"""
     global _CTX
     if _CTX is None:
         _CTX = Context(0)
     return _CTX
+
+
+def release():
+    """close the shared context and give its arena back to the device; the next ctx() creates a new one"""
+    global _CTX
+    if _CTX is not None:
+        _CTX.close()
+        _CTX = None
 
 
 def gpu_graph_artifacts(reads, k, B, keep_loops=True, early_tc=0, early_at=False):

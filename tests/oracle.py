@@ -25,6 +25,7 @@ def lib():
         L.orc_rc.restype = None; L.orc_rc.argtypes = [vp, i32, vp]
         L.orc_count.restype = vp; L.orc_count.argtypes = [vp, vp, vp, i64, i32, i32, i32]
         L.orc_kmers_from_kpomers.restype = vp; L.orc_kmers_from_kpomers.argtypes = [vp, i32]
+        L.orc_kset_from_arrays.restype = vp; L.orc_kset_from_arrays.argtypes = [vp, vp, vp, i64, i32, i32]
         for f in ("orc_kset_keys", "orc_kset_counts", "orc_kset_bsz"):
             getattr(L, f).restype = vp; getattr(L, f).argtypes = [vp]
         L.orc_kset_n.restype = i64; L.orc_kset_n.argtypes = [vp]
@@ -87,6 +88,21 @@ class KSet:
 def count(words, offs, lens, K, B, mode):
     words = np.ascontiguousarray(words, np.uint64); offs = np.ascontiguousarray(offs, np.uint64); lens = np.ascontiguousarray(lens, np.uint32)
     h = lib().orc_count(_p(words), _p(offs), _p(lens), len(lens), K, B, mode)
+    return KSet(h, K, B)
+
+
+def kset_from_arrays(keys, counts, bsz, K):
+    """KSet over given records: keys u64 [n, nwords(K)] in bucket-major order, counts u32 [n] or None, bsz i64 [B]"""
+    B = len(bsz)
+    nw = (K + 31) // 32
+    keys = np.ascontiguousarray(keys, np.uint64).reshape(-1, nw)
+    bsz = np.ascontiguousarray(bsz, np.int64)
+    cnt = None if counts is None else np.ascontiguousarray(counts, np.uint32)
+    if cnt is not None and len(cnt) != len(keys):
+        raise ValueError("counts and keys differ in length")
+    h = lib().orc_kset_from_arrays(_p(keys), _p(cnt) if cnt is not None else None, _p(bsz), len(keys), K, B)
+    if not h:
+        raise ValueError("bucket sizes add up to %d, not to the %d records given" % (int(bsz.sum()), len(keys)))
     return KSet(h, K, B)
 
 

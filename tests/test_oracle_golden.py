@@ -176,6 +176,34 @@ def test_rtseq_known_answers():
         assert bool(L.orc_is_minimal(w.ctypes.data_as(C.c_void_p), K)) == (s <= revcomp(s))
 
 
+@pytest.mark.parametrize("K,B,mode", [(22, 7, 0), (32, 16, 1), (33, 40, 0), (78, 5, 0), (128, 11, 0)])
+def test_kset_from_arrays_round_trip(K, B, mode):
+    """A KSet rebuilt from a count's own arrays is the same set: same records, counts and bucket sizes, and an MPHF that
+    serializes to the same bytes. With some buckets emptied (what one rank of a distributed count owns) every other bucket
+    keeps its keys and its slots."""
+    from spades_b200.packing import synthetic_reads
+    words, offs, lens = pack_reads(synthetic_reads(300, 150, 2000, 0.01, seed=K))
+    ks = O.count(words, offs, lens, K, B, mode)
+    assert ks.n > 0 and (ks.counts is None) == (mode == 1)
+    rb = O.kset_from_arrays(ks.keys, ks.counts, ks.bsz, K)
+    assert rb.n == ks.n and rb.nw == ks.nw and np.array_equal(rb.keys, ks.keys) and np.array_equal(rb.bsz, ks.bsz)
+    assert (rb.counts is None and ks.counts is None) or np.array_equal(rb.counts, ks.counts)
+    assert O.Mphf(rb).serialize() == O.Mphf(ks).serialize()
+    # keep every other bucket
+    start = np.concatenate(([0], np.cumsum(ks.bsz)))
+    keep = np.arange(B) % 2 == 0
+    sel = np.concatenate([np.arange(start[b], start[b + 1]) for b in range(B) if keep[b]] + [np.zeros(0, np.int64)]).astype(np.int64)
+    part = O.kset_from_arrays(ks.keys[sel], None if ks.counts is None else ks.counts[sel], np.where(keep, ks.bsz, 0), K)
+    assert part.n == len(sel)
+    m_all, m_part = O.Mphf(ks), O.Mphf(part)
+    pstart = np.concatenate(([0], np.cumsum(part.bsz)))
+    for b in np.flatnonzero(keep)[:3]:
+        for i in range(start[b], min(start[b + 1], start[b] + 20)):
+            assert m_part.lookup(ks.keys[i]) - pstart[b] == m_all.lookup(ks.keys[i]) - start[b]
+    with pytest.raises(ValueError):
+        O.kset_from_arrays(ks.keys[:-1], None, ks.bsz, K)
+
+
 def test_empty_and_short_inputs():
     # reads shorter than K are skipped (kmer_splitters.hpp:30-31); empty input gives empty buckets
     words, offs, lens = pack_reads(["ACGT", "AC"])
