@@ -1615,8 +1615,13 @@ static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, int B, bool
     // the source once, and passes are planned from exact per-bucket record counts.
     const int rA = levelA_key_bits(est_records, B, total_bits, sort_target<NW>(), tuning().pa_max);
     const int SR = std::max(1, kLevelAMaxParts >> rA);      // buckets per histogram super-range
+    // every pass becomes one chunk of the set, and a set holds at most kMaxChunks of them: each super-range may use an equal
+    // share of the chunks still free. There are at most 128 super-ranges (B <= 2^20 with SR = 8192 when rA = 0, a single one
+    // when rA > 0), so every share is at least one pass.
+    const int n_ranges = (B + SR - 1) / SR;
     int64_t first = 0;
     for (int s_lo = 0; s_lo < B; s_lo += SR) {
+        const int share = (kMaxChunks - (int)out->chunks.size()) / (n_ranges - s_lo / SR);
         LevelAJob<NW, Src> job;
         job.ctx = ctx; job.srcs = srcs; job.K = K; job.B = B; job.rA = rA; job.G = ctx->num_sms * levelA_ctas_per_sm();
         job.s_lo = s_lo; job.s_hi = std::min(B, s_lo + SR);
@@ -1624,13 +1629,14 @@ static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, int B, bool
         if constexpr (kIsReads) job.roll = !srcs.empty() && !srcs[0].both;
         levelA_count(job, est_records, tm, tr);
         // bucket-group passes: simulate the greedy "as many whole buckets as fit" plan to learn how many passes are needed, then
-        // aim for equally sized passes (a tiny last pass still costs a full scan of the source)
+        // aim for equally sized passes (a tiny last pass still costs a full scan of the source), at most `share` of them
         auto current_limit = [&]() {
             return ctx->hbm_budget ? (ctx->hbm_budget > ctx->allocated ? ctx->hbm_budget - ctx->allocated : 0) : (size_t)(ctx->free_bytes() * 0.90);
         };
         uint64_t total_records = 0;
         for (int b = job.s_lo; b < job.s_hi; ++b) total_records += job.bucket_records(b);
         uint64_t pass_target = total_records;
+        bool capped = false;
         {
             double lim_sim = (double)current_limit();
             int npass_sim = 0, b = job.s_lo;
@@ -1644,19 +1650,26 @@ static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, int B, bool
                 lim_sim -= (double)I * (W + 4) * 0.5;            // this pass's output stays resident
                 ++npass_sim;
             }
-            pass_target = total_records / (uint64_t)npass_sim + total_records / 64 + 1;
+            capped = npass_sim > share;
+            pass_target = total_records / (uint64_t)std::min(npass_sim, share) + total_records / 64 + 1;
         }
-        int b_lo = job.s_lo;
+        int b_lo = job.s_lo, npass = 0;
         while (b_lo < job.s_hi) {
-            // ---- plan this pass: whole buckets that fit next to what is already resident (X + Y + its own output)
+            // ---- plan this pass: whole buckets that fit next to what is already resident (X + Y + its own output). When the
+            // budget would need more passes than the range's share of chunks (or this is the share's last pass), the pass takes
+            // at least an even split of the buckets left, above the budget if need be: the budget is a planning target (blocks
+            // beyond the arena come from the driver), a device that really lacks the memory fails with SGPU_ENOMEM.
+            const int left = share - npass;
+            const int min_b = (capped || left == 1) ? div_up(job.s_hi - b_lo, left) : 1;
             const size_t lim = current_limit();
             int b_hi = b_lo;
             uint64_t I = 0;
             while (b_hi < job.s_hi) {
                 const uint64_t ib = job.bucket_records(b_hi);
-                if (b_hi > b_lo && (pass_bytes_needed(I + ib, W) > (double)lim || I + ib > pass_target)) break;
+                if (b_hi - b_lo >= min_b && (pass_bytes_needed(I + ib, W) > (double)lim || I + ib > pass_target)) break;
                 I += ib; ++b_hi;
             }
+            ++npass;
             const uint32_t p_lo = (uint32_t)(b_lo - job.s_lo) << rA;
             const uint32_t PA = (uint32_t)(b_hi - b_lo) << rA;
             DArr<uint64_t> part_total(ctx, PA + 1), part_start(ctx, PA + 1);

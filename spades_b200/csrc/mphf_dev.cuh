@@ -4,7 +4,6 @@
 
 namespace sg {
 
-static const int kMaxChunks = 128;
 struct KeyTable {
     int nchunks;
     int64_t first[kMaxChunks + 1];

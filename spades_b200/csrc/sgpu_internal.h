@@ -234,6 +234,9 @@ struct Chunk {
     int b_lo = 0, b_hi = 0;  // buckets [b_lo, b_hi)
     int64_t first = 0;       // index of its first record in final_kmers order
 };
+// chunks one set may hold: the MPHF build and the graph kernels pass the chunk table by value in their parameter block
+// (KeyTable, mphf_dev.cuh), so the count's planner never makes more passes than this
+static const int kMaxChunks = 128;
 struct KSet {
     Ctx *ctx = nullptr;
     int K = 0, nw = 0, B = 0;

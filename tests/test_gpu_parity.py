@@ -10,11 +10,12 @@ from spades_b200.packing import pack_reads, revcomp, synthetic_reads
 pytestmark = pytest.mark.gpu
 
 
-def _oracle_art(reads, k, B):
-    r = O.full_graph(reads, k, B)
+def _oracle_art(reads, k, B, **clippers):
+    """the oracle's artefacts of the whole path (clippers: early_tc / early_at of O.full_graph); `oracle` keeps its sets and MPHFs"""
+    r = O.full_graph(reads, k, B, **clippers)
     return dict(kpomers=r["kp"].keys, kp_bsz=r["kp"].bsz, kmers=r["km"].keys, kmer_index=r["mk"].serialize(),
                 kpomer_index=r["mkp"].serialize(), masks=r["masks"], cov=r["cov"], hist=r["hist"].astype(np.int64),
-                unitigs=r["unitigs"].seqs, gfa=r["gfa"], kp_counts=r["kp"].counts)
+                unitigs=r["unitigs"].seqs, gfa=r["gfa"], kp_counts=r["kp"].counts, oracle=r)
 
 
 def _compare(a, b, B):
