@@ -76,6 +76,14 @@ typedef struct sgpu_times {
     uint64_t launches;    /* kernels launched by this context so far */
     uint64_t peak_bytes;  /* peak device memory held by this context */
     uint64_t cached_bytes;/* freed device blocks kept by the context's caching allocator (reusable) */
+    /* which paths of the count ran (last sgpu_count / sgpu_kmers_from_kpomers / sgpu_dist_begin .. sgpu_dist_end) */
+    uint64_t level_a_key_bits;      /* rA: key bits folded into a level-A partition id */
+    uint64_t level_a_scatters;      /* level-A scatter launches (one per source, pass and partition sub-range) */
+    uint64_t refine_rounds_max;     /* most refinement rounds any pass ran, the gather round included */
+    uint64_t refine_splits_round0;  /* segments the first refinement round (the gather) added beyond the partitions */
+    uint64_t refine_splits_later;   /* segments the later refinement rounds added */
+    uint64_t sort_lsd_fallbacks;    /* local-sort segments that took the exact LSD fallback */
+    uint64_t sort_oversize_equal;   /* segments longer than the local-sort capacity whose records are all equal */
 } sgpu_times;
 
 int sgpu_create(const sgpu_config *cfg, sgpu_ctx **out);

@@ -42,7 +42,10 @@ class SgpuGraphOptions(C.Structure):
 class SgpuTimes(C.Structure):
     _fields_ = [("extract_count_ms", C.c_float), ("extract_scatter_ms", C.c_float), ("refine_ms", C.c_float),
                 ("local_sort_ms", C.c_float), ("compact_ms", C.c_float), ("mphf_ms", C.c_float), ("exchange_ms", C.c_float),
-                ("instances", C.c_uint64), ("passes", C.c_uint64), ("launches", C.c_uint64), ("peak_bytes", C.c_uint64), ("cached_bytes", C.c_uint64)]
+                ("instances", C.c_uint64), ("passes", C.c_uint64), ("launches", C.c_uint64), ("peak_bytes", C.c_uint64), ("cached_bytes", C.c_uint64),
+                ("level_a_key_bits", C.c_uint64), ("level_a_scatters", C.c_uint64), ("refine_rounds_max", C.c_uint64),
+                ("refine_splits_round0", C.c_uint64), ("refine_splits_later", C.c_uint64), ("sort_lsd_fallbacks", C.c_uint64),
+                ("sort_oversize_equal", C.c_uint64)]
 
 
 _lib = None

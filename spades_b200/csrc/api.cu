@@ -81,6 +81,9 @@ int sgpu_get_times(const sgpu_ctx *ctx, sgpu_times *out) {
     out->extract_count_ms = t.extract_count; out->extract_scatter_ms = t.extract_scatter; out->refine_ms = t.refine;
     out->local_sort_ms = t.local_sort; out->compact_ms = t.compact; out->mphf_ms = t.mphf; out->exchange_ms = t.exchange;
     out->instances = t.instances; out->passes = t.passes; out->launches = ctx->c.launches; out->peak_bytes = ctx->c.peak; out->cached_bytes = ctx->c.pool_cached;
+    out->level_a_key_bits = t.level_a_key_bits; out->level_a_scatters = t.level_a_scatters;
+    out->refine_rounds_max = t.refine_rounds_max; out->refine_splits_round0 = t.refine_splits_round0; out->refine_splits_later = t.refine_splits_later;
+    out->sort_lsd_fallbacks = t.sort_lsd_fallbacks; out->sort_oversize_equal = t.sort_oversize_equal;
     return SGPU_OK;
 }
 

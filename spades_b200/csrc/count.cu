@@ -1010,7 +1010,10 @@ __global__ void __launch_bounds__(kSThreads) local_sort3_k(const Seg *__restrict
         uint32_t *gcnt = reinterpret_cast<uint32_t *>(gpartner);
         if (s.len == 0) { if (threadIdx.x == 0) ndist[si] = 0; __syncthreads(); continue; }
         if (s.len > (uint64_t)CAP) {
-            if (threadIdx.x == 0) { gcnt[0] = (uint32_t)s.len; ndist[si] = 1; if (s.bits < (uint32_t)total_bits) atomicAdd(&stats[0], 1ull); }
+            if (threadIdx.x == 0) {
+                gcnt[0] = (uint32_t)s.len; ndist[si] = 1;
+                atomicAdd(&stats[s.bits < (uint32_t)total_bits ? 0 : 2], 1ull);     // [0] is an internal error, [2] an equal-key segment
+            }
             __syncthreads();
             continue;
         }
@@ -1327,6 +1330,7 @@ static void sort_pass(Ctx *ctx, int K, DArr<uint64_t> &X, DArr<uint64_t> &Y, con
     rp.rmax = tuning().rmax;
     DArr<unsigned long long> wcounter(ctx, 4);
     tm.start();
+    uint64_t rounds = 0;
     for (int round = 0; round < 300; ++round) {
         DArr<uint32_t> nchild(ctx, nsegs + 1), isw(ctx, nsegs + 1);
         DArr<uint64_t> cbase(ctx, nsegs + 1), wpos(ctx, nsegs + 1);
@@ -1366,9 +1370,12 @@ static void sort_pass(Ctx *ctx, int K, DArr<uint64_t> &X, DArr<uint64_t> &Y, con
         ctx->launches++;
         SG_CUDA(cudaGetLastError());
         tr.mark("refine round");
+        (round == 0 ? ctx->times.refine_splits_round0 : ctx->times.refine_splits_later) += tot[0] - nsegs;
+        ++rounds;
         segs = std::move(nsegs_arr);
         nsegs = tot[0];
     }
+    ctx->times.refine_rounds_max = std::max(ctx->times.refine_rounds_max, rounds);
     ctx->times.refine += tm.stop();
     // ---- local sort
     DArr<uint32_t> ndist(ctx, nsegs + 1);
@@ -1403,6 +1410,8 @@ static void sort_pass(Ctx *ctx, int K, DArr<uint64_t> &X, DArr<uint64_t> &Y, con
     ctx->times.local_sort += tm.stop();
     tr.mark("local sort");
     SG_CHECK(h_stats[0] == 0, 6, "internal: oversize segment with unfixed key bits reached the local sort");
+    ctx->times.sort_lsd_fallbacks += h_stats[1];
+    ctx->times.sort_oversize_equal += h_stats[2];
     // ---- compaction into the dense chunk
     Chunk ch;
     ch.n = (int64_t)D; ch.b_lo = (int)b_lo; ch.b_hi = b_hi; ch.first = first;
@@ -1572,7 +1581,7 @@ static void levelA_scatter(LevelAJob<NW, Src> &job, int b_lo, int b_hi, uint64_t
                         levelA_scatter_roll_k<NW, true><<<G, kRollThreads, smem_sub, st>>>(src, pa_sub, base.p, X, job.tile_off[si].p, job.ids[si].p, p_lo + q_lo, PA, q_lo, (uint64_t)job.ids[si].n);
                     else
                         levelA_scatter_roll_k<NW, false><<<G, kRollThreads, smem, st>>>(src, pa, base.p, X, nullptr, nullptr, 0u, PA, 0u, 0ull);
-                    ctx->launches++;
+                    ctx->launches++; ctx->times.level_a_scatters++;
                 }
             }
             }
@@ -1585,7 +1594,7 @@ static void levelA_scatter(LevelAJob<NW, Src> &job, int b_lo, int b_hi, uint64_t
             if (src.n == 0) continue;
             levelA_scatter_k<NW, Src><<<G, kAThreads, smem, st>>>(src, pa, base.p, X, job.use_ids ? job.tile_off[si].p : nullptr,
                                                                  job.use_ids ? job.ids[si].p : nullptr, p_lo);
-            ctx->launches++;
+            ctx->launches++; ctx->times.level_a_scatters++;
         }
     }
     SG_CUDA(cudaGetLastError());
@@ -1614,6 +1623,7 @@ static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, int B, bool
     // source serves every bucket-group pass (the groups are contiguous partition ranges), so a multi-pass job hashes
     // the source once, and passes are planned from exact per-bucket record counts.
     const int rA = levelA_key_bits(est_records, B, total_bits, sort_target<NW>(), tuning().pa_max);
+    ctx->times.level_a_key_bits = (uint64_t)rA;
     const int SR = std::max(1, kLevelAMaxParts >> rA);      // buckets per histogram super-range
     // every pass becomes one chunk of the set, and a set holds at most kMaxChunks of them: each super-range may use an equal
     // share of the chunks still free. There are at most 128 super-ranges (B <= 2^20 with SR = 8192 when rA = 0, a single one
@@ -2129,6 +2139,7 @@ DistState *dist_begin(Ctx *ctx, int K, int B, int mode, int world, int rank) {
     int rA = 0;
     while (rA < 8 && ((uint64_t)B << (rA + 1)) <= (uint64_t)kLevelAMaxParts && rA + 1 <= 2 * K) ++rA;
     d->plan.world = world; d->plan.rank = rank; d->plan.B = B; d->plan.rA = rA; d->plan.PA_all = (uint32_t)B << rA;
+    ctx->times.level_a_key_bits = (uint64_t)rA;
     try { d->begin(); } catch (...) { delete d; throw; }
     return d;
 }

@@ -69,6 +69,10 @@ struct PhaseTimes {   // device milliseconds measured with CUDA events on ctx->s
     uint64_t launches = 0;
     uint64_t instances = 0;       // records written by the partition kernel
     uint64_t passes = 0;
+    // paths taken (sgpu_times)
+    uint64_t level_a_key_bits = 0, level_a_scatters = 0;
+    uint64_t refine_rounds_max = 0, refine_splits_round0 = 0, refine_splits_later = 0;
+    uint64_t sort_lsd_fallbacks = 0, sort_oversize_equal = 0;
 };
 
 struct Ctx {
