@@ -5,10 +5,16 @@
 //   -s S        streams per CTA                       (open 128-byte lines per CTA; 2 CTAs of 512 threads per SM)
 //   -w 16|32    bytes per store                       (32 = two records of a stream written back to back by one thread)
 //   -l cta|part layout: CTA-major (a CTA's streams are adjacent: its stores stay inside total/G bytes) or partition-major
-//               (stream p of every CTA adjacent: a CTA's stores spread over the whole buffer -> TLB reach)
+//               (stream p of every CTA adjacent: a CTA's stores spread over the whole buffer)
 //   -g GB       total bytes written
 // Prints GB/s for each configuration so that "streams per CTA", "store width" and "layout" can be separated. Build + run:
 //   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o scatter_bench scatter_bench.cu && ./scatter_bench
+//
+// Page-locality mode (-c MB): every CTA writes C MB of 16-byte records into S streams (-S, default 640), CTA-major, either into
+// one region of C MB (today's level-A staging: the stores of a CTA hit all of its region's pages for the whole launch) or in
+// consecutive slices of R MB each (-r, repeatable): the cursors restart in a fresh sub-region of R MB at every slice, so only the
+// current slice's pages take stores. Same bytes, same streams per slice, same instructions; only the live footprint differs.
+//   ./scatter_bench -c 57 -S 640 -r 57 -r 16 -r 4 -r 2
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -42,6 +48,48 @@ __global__ void __launch_bounds__(512, 2) scatter_k(uint64_t *out, const uint64_
     }
 }
 
+// CTA g writes nslice slices of recs_per_slice records; slice s owns the sub-region [(g * nslice + s) * S * per_stream, +S * per_stream)
+__global__ void __launch_bounds__(512, 2) slice_k(uint64_t *out, int S, uint32_t per_stream, uint32_t recs_per_slice, int nslice) {
+    extern __shared__ uint32_t cur[];
+    for (int sl = 0; sl < nslice; ++sl) {
+        for (int i = threadIdx.x; i < S; i += blockDim.x) cur[i] = 0;
+        __syncthreads();
+        const uint64_t region = ((uint64_t)blockIdx.x * nslice + sl) * S * per_stream;
+        for (uint32_t i = threadIdx.x; i < recs_per_slice; i += blockDim.x) {
+            const uint32_t h = mix(i * 2654435761u + (blockIdx.x * nslice + sl) * 40503u);
+            const uint32_t s = h % (uint32_t)S;
+            const uint32_t slot = atomicAdd(&cur[s], 1u);
+            if (slot >= per_stream) continue;
+            uint64_t *dst = out + (region + (uint64_t)s * per_stream + slot) * 2;
+            asm volatile("st.global.L1::no_allocate.v2.u64 [%0], {%1, %2};" ::"l"(dst), "l"((uint64_t)h), "l"(~(uint64_t)h) : "memory");
+        }
+        __syncthreads();
+    }
+}
+
+// GB/s of record bytes, best of `reps`, for C MB per CTA written in slices of R MB
+static float run_slices(double cta_mb, double slice_mb, int S, int G, uint64_t *d_out, size_t out_bytes, int reps) {
+    int nslice = (int)(cta_mb / slice_mb + 0.5);
+    if (nslice < 1) nslice = 1;
+    const uint64_t per_cta = (uint64_t)(cta_mb * 1e6 / 16);
+    const uint32_t per_slice = (uint32_t)(per_cta / nslice);
+    const uint32_t per_stream = (uint32_t)((uint64_t)per_slice * 5 / 4 / S + 8) & ~1u;
+    if ((uint64_t)per_stream * S * nslice * G * 16 > out_bytes) { fprintf(stderr, "buffer too small\n"); exit(1); }
+    cudaEvent_t e0, e1;
+    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+    float best = 1e30f;
+    for (int rep = 0; rep < reps; ++rep) {
+        CK(cudaEventRecord(e0));
+        slice_k<<<G, 512, S * 4>>>(d_out, S, per_stream, per_slice, nslice);
+        CK(cudaEventRecord(e1));
+        CK(cudaEventSynchronize(e1));
+        float ms; CK(cudaEventElapsedTime(&ms, e0, e1));
+        if (ms < best) best = ms;
+    }
+    CK(cudaGetLastError());
+    return (float)((double)per_slice * nslice * G * 16 / 1e9 / (best / 1e3));
+}
+
 static float run(int width, int S, bool cta_major, double gb, int G, uint64_t *d_out, size_t out_bytes) {
     const uint64_t total_rec = (uint64_t)(gb * 1e9 / 16);
     const uint32_t per_cta = (uint32_t)(total_rec / G);
@@ -71,10 +119,34 @@ static float run(int width, int S, bool cta_major, double gb, int G, uint64_t *d
 }
 
 int main(int argc, char **argv) {
-    double gb = 8.0;
-    for (int i = 1; i + 1 < argc; i += 2) if (!strcmp(argv[i], "-g")) gb = atof(argv[i + 1]);
+    double gb = 8.0, cta_mb = 0;
+    int S = 640;
+    std::vector<double> slice_mb;
+    for (int i = 1; i + 1 < argc; i += 2) {
+        if (!strcmp(argv[i], "-g")) gb = atof(argv[i + 1]);
+        else if (!strcmp(argv[i], "-c")) cta_mb = atof(argv[i + 1]);
+        else if (!strcmp(argv[i], "-S")) S = atoi(argv[i + 1]);
+        else if (!strcmp(argv[i], "-r")) slice_mb.push_back(atof(argv[i + 1]));
+    }
     cudaDeviceProp p; CK(cudaGetDeviceProperties(&p, 0));
     const int G = p.multiProcessorCount * 2;
+    if (cta_mb > 0) {
+        if (slice_mb.empty()) slice_mb.push_back(cta_mb);
+        const size_t out_bytes = (size_t)(cta_mb * 1e6 * G * 1.3) + (64u << 20);
+        uint64_t *d_out;
+        CK(cudaMalloc(&d_out, out_bytes));
+        CK(cudaMemset(d_out, 0, out_bytes));
+        CK(cudaFuncSetAttribute(slice_k, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 << 10));
+        printf("%s, %d CTAs x 512 threads, %d streams, %.1f MB per CTA (%.1f GB per run); GB/s of record bytes, best of 3\n", p.name, G, S, cta_mb,
+               cta_mb * G / 1e3);
+        for (int round = 0; round < 3; ++round)      // alternating: every slice size once per round
+            for (double r : slice_mb) {
+                printf("round %d  slice %6.1f MB  %8.0f GB/s\n", round, r, run_slices(cta_mb, r, S, G, d_out, out_bytes, 3));
+                fflush(stdout);
+            }
+        CK(cudaFree(d_out));
+        return 0;
+    }
     const size_t out_bytes = (size_t)(gb * 1.4e9) + (64u << 20);
     uint64_t *d_out;
     CK(cudaMalloc(&d_out, out_bytes));

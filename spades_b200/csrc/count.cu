@@ -525,7 +525,8 @@ __global__ void __launch_bounds__(kRollThreads, 2) levelA_count_roll_k(ReadsSrc 
 
 // base rows are `row_stride` cursors long; this launch handles the partitions [q_lo, q_lo + p.PA) of a row (p.PA = the
 // sub-range's size, id_lo = id of its first partition): a bucket-group pass may be split into partition sub-ranges so that
-// the lines and pages a CTA has open at any time stay few (DESIGN.md: TLB reach).
+// the streams (partial lines) a CTA has open at any time stay few. What sets the rate of these 16-byte scattered stores is the
+// number of open streams per CTA and the store width, not how many pages a CTA's region spans (DESIGN.md 6.2).
 // (A sector-pairing variant of this kernel -- two records of a stream leave as one 32-byte store through shared-memory
 // mailboxes -- was parity clean but slower: the CAS traffic on the mailboxes cost more than the full sectors won. Removed.)
 template <int NW, bool HAS_IDS>
@@ -595,7 +596,13 @@ __global__ void __launch_bounds__(kRollThreads, 2) levelA_scatter_roll_k(ReadsSr
                     mine = part < PA;
                     if (mine) {
                         const uint32_t slot = atomicAdd(&cur[part], 1u);
-                        store_rec_stream<NW>(out0 + (size_t)slot * NW, kmer_is_minimal<NW>(st.f, st.r) ? st.f : st.r);
+                        // a word-by-word select: `cond ? st.f : st.r` bound to the store's reference argument made the compiler
+                        // keep the whole roll state in local memory (5 spill stores per window) to pick an address
+                        const bool fwd = kmer_is_minimal<NW>(st.f, st.r);
+                        Kmer<NW> k;
+#pragma unroll
+                        for (int j = 0; j < NW; ++j) k.w[j] = fwd ? st.f.w[j] : st.r.w[j];
+                        store_rec_stream<NW>(out0 + (size_t)slot * NW, k);
                     }
                 } else {
                     const Kmer<NW> k = kmer_is_minimal<NW>(st.f, st.r) ? st.f : st.r;
@@ -643,15 +650,15 @@ __global__ void seg_init_k(const uint64_t *__restrict__ part_start, const uint64
 }
 
 // ---- CTA-major staging of the level-A output ------------------------------------------------------------------------------
-// A partition kernel with a partition-major output runs at the same low rate whatever its instruction count per record and
-// however many partitions a CTA has open, while the MSD refinement -- same 16-byte scattered stores, same number of open
-// lines -- runs several times faster. The difference is WHERE a CTA's stores go: with a partition-major output every CTA
-// writes all over a buffer of tens of GB (thousands of 2-MB pages against the TLB reach of an SM), the refinement writes
-// inside one segment of a few MB. So level A writes CTA-major: CTA g owns one contiguous region of the staging
+// Level A writes CTA-major: CTA g owns one contiguous region of the staging
 // buffer, partitioned inside ([g][partition]); a partition is then G pieces, and the FIRST refinement round reads its
 // segment piece by piece (sequential runs: one page at a time) and writes the children partition-major into the partner
 // buffer -- the gather costs no extra pass over the data. Partitions that need no refinement take the same kernel with
 // r = 0 (a copy into the partner buffer).
+// The layout is not what sets the partition kernel's store rate: in scripts/microbench/scatter_bench.cu, CTA-major and
+// partition-major outputs run within 6 % of each other at every stream count, and confining a CTA's stores to 2 MB slices of
+// its 57 MB region at a time changes nothing (DESIGN.md 6.2). The rate falls with the open streams per CTA, and at 512 to
+// 1024 streams it doubles with 32-byte instead of 16-byte stores.
 struct Pieces {
     const uint64_t *pbase;     // [G][PA]  first record of piece (g, partition) in the staging buffer
     const uint32_t *cnt;       // blk_counts + p_lo: cnt[g * cnt_stride + partition]
@@ -1561,7 +1568,7 @@ static void levelA_scatter(LevelAJob<NW, Src> &job, int b_lo, int b_hi, uint64_t
             SG_CUDA(cudaFuncSetAttribute(levelA_scatter_roll_k<NW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             SG_CUDA(cudaFuncSetAttribute(levelA_scatter_roll_k<NW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             {
-            // partition sub-ranges (only with the id array, where a foreign window costs just the roll): fewer lines and pages open
+            // partition sub-ranges (only with the id array, where a foreign window costs just the roll): fewer streams open
             // per CTA. A sub-range costs one more roll over ALL windows of the source: worth it when the pass holds most of the job's
             // records (a single-pass job gains from 4 sub-ranges, a job of several passes loses from even 2)
             int nsub_auto = (int)(4.0 * (double)I_pass / (double)std::max<uint64_t>(1, total_records) + 0.5);
