@@ -15,6 +15,14 @@
 // consecutive slices of R MB each (-r, repeatable): the cursors restart in a fresh sub-region of R MB at every slice, so only the
 // current slice's pages take stores. Same bytes, same streams per slice, same instructions; only the live footprint differs.
 //   ./scatter_bench -c 57 -S 640 -r 57 -r 16 -r 4 -r 2
+//
+// Refinement mode (-b 1): the write pattern of refine_k's scatter sweep. One CTA per SM of 1024 threads (or two of 512), 1024 or
+// 2048 bins per CTA, each bin a contiguous child region of its CTA, records to pseudo-random bins. Three ways to write them:
+//   lone   one 16-byte store per record as it takes its slot (shared-memory atomic cursor)
+//   pair   32-byte pairs: two records of a bin written back to back by one thread (an idealised sector mailbox)
+//   batch  N records per CTA per batch: rank in the bin (one shared-memory atomic), block scan of the batch counts, the owner of a
+//          bin claims its run, permute into bin order in shared memory, flush with consecutive threads on consecutive addresses
+//   ./scatter_bench -b 1 -g 8
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -65,6 +73,134 @@ __global__ void __launch_bounds__(512, 2) slice_k(uint64_t *out, int S, uint32_t
         }
         __syncthreads();
     }
+}
+
+// ---- refinement mode ------------------------------------------------------------------------------------------------------
+// CTA g owns bins [g * B, (g + 1) * B), bin b's region starts at b * per_bin records of W bytes. PAIR: two records per store.
+template <int T, int W, bool PAIR>
+__global__ void __launch_bounds__(T) rlone_k(uint64_t *out, int B, uint32_t per_bin, uint32_t records_per_cta) {
+    extern __shared__ uint32_t cur[];
+    for (int i = threadIdx.x; i < B; i += T) cur[i] = 0;
+    __syncthreads();
+    constexpr uint32_t RPS = PAIR ? 2 : 1;
+    for (uint32_t i = threadIdx.x; i < records_per_cta / RPS; i += T) {
+        const uint32_t h = mix(i * 2654435761u + blockIdx.x * 40503u);
+        const uint32_t b = h % (uint32_t)B;
+        const uint32_t slot = atomicAdd(&cur[b], RPS);
+        if (slot + RPS > per_bin) continue;
+        uint64_t *dst = out + ((uint64_t)blockIdx.x * B + b) * per_bin * 2 + (uint64_t)slot * 2;
+        asm volatile("st.global.L1::no_allocate.v2.u64 [%0], {%1, %2};" ::"l"(dst), "l"((uint64_t)h), "l"(~(uint64_t)h) : "memory");
+        if (PAIR) asm volatile("st.global.L1::no_allocate.v2.u64 [%0], {%1, %2};" ::"l"(dst + 2), "l"((uint64_t)h + 1), "l"(~(uint64_t)h) : "memory");
+    }
+}
+
+// records of W bytes (8, 16, 32) in batches of N per CTA
+template <int T, int W, int N>
+__global__ void __launch_bounds__(T) rbatch_k(uint64_t *out, int B, uint32_t per_bin, uint32_t records_per_cta) {
+    constexpr int NW = W / 8, RPT = N / T, BPT = 2048 / T;       // records and bins per thread
+    extern __shared__ uint64_t sm[];
+    uint64_t *stage = sm;                                                         // [N][NW]
+    uint32_t *sslot = reinterpret_cast<uint32_t *>(stage + (size_t)N * NW);       // [N] global record index
+    uint32_t *cnt = sslot + N, *roff = cnt + 2048, *rbase = roff + 2048;          // [2048] each
+    __shared__ uint32_t wtot[T / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint32_t cur[BPT];
+    for (int q = 0; q < BPT; ++q) {
+        const uint32_t b = threadIdx.x * BPT + q;
+        cur[q] = 0;
+        if (b < (uint32_t)B) cnt[b] = 0;
+    }
+    __syncthreads();
+    for (uint32_t b0 = 0; b0 < records_per_cta; b0 += N) {
+        uint32_t tag[RPT];
+        uint64_t v[RPT];
+#pragma unroll
+        for (int j = 0; j < RPT; ++j) {
+            const uint32_t i = b0 + threadIdx.x + T * j;
+            const uint32_t h = mix(i * 2654435761u + blockIdx.x * 40503u);
+            const uint32_t b = h % (uint32_t)B;
+            v[j] = h;
+            tag[j] = i < records_per_cta ? (atomicAdd(&cnt[b], 1u) << 11) | b : ~0u;
+        }
+        __syncthreads();
+        uint32_t c[BPT], tsum = 0;
+        for (int q = 0; q < BPT; ++q) {
+            const uint32_t b = threadIdx.x * BPT + q;
+            c[q] = b < (uint32_t)B ? cnt[b] : 0u;
+            tsum += c[q];
+        }
+        uint32_t inc = tsum;
+        for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
+        if (lane == 31) wtot[warp] = inc;
+        __syncthreads();
+        uint32_t w = lane < T / 32 ? wtot[lane] : 0u, winc = w;
+        for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, winc, o); if (lane >= o) winc += t; }
+        const uint32_t total = __shfl_sync(0xffffffffu, winc, 31);
+        uint32_t off = __shfl_sync(0xffffffffu, winc - w, warp) + inc - tsum;
+        for (int q = 0; q < BPT; ++q) {
+            const uint32_t b = threadIdx.x * BPT + q;
+            if (b < (uint32_t)B) { roff[b] = off; rbase[b] = b * per_bin + cur[q]; cnt[b] = 0; }
+            off += c[q]; cur[q] += c[q];
+        }
+        __syncthreads();
+#pragma unroll
+        for (int j = 0; j < RPT; ++j) {
+            if (tag[j] == ~0u) continue;
+            const uint32_t b = tag[j] & 2047u, rank = tag[j] >> 11;
+            const uint32_t p = roff[b] + rank;
+            for (int k = 0; k < NW; ++k) stage[(size_t)p * NW + k] = v[j] + k;
+            sslot[p] = rank + rbase[b];
+        }
+        __syncthreads();
+        uint64_t *cta_out = out + (uint64_t)blockIdx.x * B * per_bin * NW;
+        for (uint32_t p = threadIdx.x; p < total; p += T) {
+            uint64_t *dst = cta_out + (uint64_t)sslot[p] * NW;
+            if (NW == 1) asm volatile("st.global.L1::no_allocate.u64 [%0], %1;" ::"l"(dst), "l"(stage[p]) : "memory");
+            for (int k = 0; k + 1 < NW; k += 2)
+                asm volatile("st.global.L1::no_allocate.v2.u64 [%0], {%1, %2};" ::"l"(dst + k), "l"(stage[(size_t)p * NW + k]), "l"(stage[(size_t)p * NW + k + 1]) : "memory");
+        }
+    }
+}
+
+// GB/s of record bytes, best of 3 (per_bin leaves 25 % slack over the mean: far more than the spread of the pseudo-random bins)
+template <class F>
+static float rtime(F launch, double bytes) {
+    cudaEvent_t e0, e1;
+    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+    float best = 1e30f;
+    for (int rep = 0; rep < 3; ++rep) {
+        CK(cudaEventRecord(e0));
+        launch();
+        CK(cudaEventRecord(e1));
+        CK(cudaEventSynchronize(e1));
+        float ms; CK(cudaEventElapsedTime(&ms, e0, e1));
+        if (ms < best) best = ms;
+    }
+    CK(cudaGetLastError());
+    return (float)(bytes / 1e9 / (best / 1e3));
+}
+
+template <int T>
+static void refine_row(int B, double gb, int SMs, uint64_t *d_out, size_t out_bytes) {
+    const int G = SMs * (1024 / T);
+    auto lone = [&](bool pair) {
+        const uint32_t per_cta = (uint32_t)(gb * 1e9 / 16 / G), per_bin = (uint32_t)((uint64_t)per_cta * 5 / 4 / B + 8) & ~1u;
+        if ((uint64_t)per_bin * B * G * 16 > out_bytes) { fprintf(stderr, "buffer too small\n"); exit(1); }
+        auto k = pair ? rlone_k<T, 16, true> : rlone_k<T, 16, false>;
+        return rtime([&] { k<<<G, T, B * 4>>>(d_out, B, per_bin, per_cta); }, (double)per_cta * G * 16);
+    };
+    auto batch = [&](auto kern, int W, int N) {
+        const uint32_t per_cta = (uint32_t)(gb * 1e9 / W / G), per_bin = (uint32_t)((uint64_t)per_cta * 5 / 4 / B + 8) & ~1u;
+        if ((uint64_t)per_bin * B * G * W > out_bytes) { fprintf(stderr, "buffer too small\n"); exit(1); }
+        const size_t sm = (size_t)N * (W + 4) + 3 * 2048 * 4;
+        if (sm > 220u << 10 || (1024 / T) * sm > 226u << 10) return -1.f;          // does not fit (1024 / T) CTAs per SM
+        CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+        return rtime([&] { kern<<<G, T, sm>>>(d_out, B, per_bin, per_cta); }, (double)per_cta * G * W);
+    };
+    printf("%5d x %4d | %5d | %6.0f %6.0f | %6.0f %6.0f %6.0f | %6.0f %6.0f | %6.0f\n", 1024 / T, T, B, lone(false), lone(true),
+           batch(rbatch_k<T, 16, 2048>, 16, 2048), batch(rbatch_k<T, 16, 4096>, 16, 4096), batch(rbatch_k<T, 16, 8192>, 16, 8192),
+           batch(rbatch_k<T, 8, 8192>, 8, 8192), batch(rbatch_k<T, 8, 16384>, 8, 16384), batch(rbatch_k<T, 32, 4096>, 32, 4096));
+    fflush(stdout);
 }
 
 // GB/s of record bytes, best of `reps`, for C MB per CTA written in slices of R MB
@@ -120,16 +256,32 @@ static float run(int width, int S, bool cta_major, double gb, int G, uint64_t *d
 
 int main(int argc, char **argv) {
     double gb = 8.0, cta_mb = 0;
-    int S = 640;
+    int S = 640, refine_mode = 0;
     std::vector<double> slice_mb;
     for (int i = 1; i + 1 < argc; i += 2) {
         if (!strcmp(argv[i], "-g")) gb = atof(argv[i + 1]);
         else if (!strcmp(argv[i], "-c")) cta_mb = atof(argv[i + 1]);
         else if (!strcmp(argv[i], "-S")) S = atoi(argv[i + 1]);
         else if (!strcmp(argv[i], "-r")) slice_mb.push_back(atof(argv[i + 1]));
+        else if (!strcmp(argv[i], "-b")) refine_mode = atoi(argv[i + 1]);
     }
     cudaDeviceProp p; CK(cudaGetDeviceProperties(&p, 0));
     const int G = p.multiProcessorCount * 2;
+    if (refine_mode) {
+        const size_t out_bytes = (size_t)(gb * 1.4e9) + (64u << 20);
+        uint64_t *d_out;
+        CK(cudaMalloc(&d_out, out_bytes));
+        CK(cudaMemset(d_out, 0, out_bytes));
+        printf("%s, refinement write pattern, %.1f GB per run; GB/s of record bytes, best of 3 (-: does not fit shared memory)\n", p.name, gb);
+        printf("%12s | %5s | %6s %6s | %6s %6s %6s | %6s %6s | %6s\n", "CTAs x thr", "bins", "lone16", "pair32", "b16/2k", "b16/4k",
+               "b16/8k", "b8/8k", "b8/16k", "b32/4k");
+        for (int B : {1024, 2048}) {
+            refine_row<1024>(B, gb, p.multiProcessorCount, d_out, out_bytes);
+            refine_row<512>(B, gb, p.multiProcessorCount, d_out, out_bytes);
+        }
+        CK(cudaFree(d_out));
+        return 0;
+    }
     if (cta_mb > 0) {
         if (slice_mb.empty()) slice_mb.push_back(cta_mb);
         const size_t out_bytes = (size_t)(cta_mb * 1e6 * G * 1.3) + (64u << 20);

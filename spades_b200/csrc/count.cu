@@ -22,7 +22,6 @@
 #include <type_traits>
 
 #include "sgpu_internal.h"
-#include "pair_mailbox.cuh"
 
 namespace sg {
 
@@ -729,39 +728,47 @@ __global__ void refine_copy_k(const Seg *__restrict__ segs, uint64_t n, const ui
     else nsegs[child_base[i]] = segs[i];
 }
 
-// stores of the pairing refinement (pair_mailbox.cuh): one full 32-byte sector for two records of a bin, 16 bytes for a lone record.
-// sm_90 has no 32-byte store instruction: the two halves of the sector leave one thread back to back and reach L2 together.
-struct PairSink {
-    uint64_t *out;
-    __device__ __forceinline__ void pair(uint64_t pos, uint64_t a0, uint64_t a1, uint64_t b0, uint64_t b1) {
-        asm volatile("st.global.L1::no_allocate.v2.u64 [%0], {%1, %2};\n\t"
-                     "st.global.L1::no_allocate.v2.u64 [%3], {%4, %5};" ::"l"(out + pos * 2), "l"(a0), "l"(a1), "l"(out + pos * 2 + 2), "l"(b0), "l"(b1) : "memory");
-    }
-    __device__ __forceinline__ void single(uint64_t pos, uint64_t w0, uint64_t w1) {
-        asm volatile("st.global.L1::no_allocate.v2.u64 [%0], {%1, %2};" ::"l"(out + pos * 2), "l"(w0), "l"(w1) : "memory");
-    }
-};
-
 static const int kRThreads = 1024;
+static const int kRWarps = kRThreads / 32;
 static const int kRMaxBins = 2048;
+// The scatter sweep collects a batch of records per CTA in shared memory and writes it out bin by bin. A thread holds a batch's
+// share in registers between its loads and the permute: 128 bytes of records at 1 and 2 words (16384 / 8192 records, 4 per bin
+// on average at 2048 bins for 16-byte records), 96 at 3 and 4 words, where 128 spill in the gather (64 registers at one CTA of
+// 1024 threads per SM). At 8-byte records the batch is capped at 12 per thread so that it and its slot array fit shared memory.
+template <int NW> struct RBatch {
+    static const int RPT = NW == 1 ? 12 : NW == 2 ? 8 : NW == 3 ? 4 : 3;                              // records per thread
+    static const int N = RPT * kRThreads;                                                                  // records per batch
+    static constexpr size_t smem() { return (size_t)N * (NW * sizeof(uint64_t) + sizeof(uint32_t)); }
+};
 
 // one CTA splits one oversize segment by its next r key bits: buf[bb&1] -> buf[(bb&1)^1]
 // PIECED: the segments are level-A partitions whose records lie in G pieces of the CTA-major staging buffer (buf0); segment
-// index == partition. The pieces are read one after the other, the children are written contiguously into buf1.
-// PAIR (opt-in, 16-byte records): the scatter phase pairs the two records of a 32-byte sector through one mailbox per bin
-// (pair_mailbox.cuh) -- at 2048 bins a bin receives a record only every ~8 us and half-written sectors do not survive in L2.
-template <int NW, bool PIECED, bool PAIR>
+// index == partition. A warp streams the pieces g = warp, warp + 32, ... one after the other; the children are written
+// contiguously into buf1.
+// Two sweeps over the segment: a histogram of the r-bit digits (-> the children's ranges), then the scatter. At 2048 bins a bin
+// receives a record only every few microseconds, so records stored one by one as they arrive leave L2 as partly written sectors
+// that each cost a fill read. The scatter therefore works in batches of RBatch<NW>::N records: every record takes a rank in its
+// bin with one shared-memory atomic, a block scan of the batch counts gives each bin's run in the batch, the owner thread of a
+// bin (2 bins per thread, as in the segment scan) claims the run from the bin's cursor, which it keeps in registers, and the batch
+// is permuted into bin order in shared memory and flushed with consecutive threads storing consecutive records of a run. The
+// next batch's loads are issued before the flush. The order inside a child is arbitrary, as it was with atomic slots.
+template <int NW, bool PIECED>
 __global__ void __launch_bounds__(kRThreads) refine_k(const Seg *__restrict__ segs, const uint64_t *__restrict__ worklist, uint64_t nwork,
                                                      const uint64_t *__restrict__ child_base, RefinePlan rp, int K,
                                                      uint64_t *__restrict__ buf0, uint64_t *__restrict__ buf1, Seg *__restrict__ nsegs,
                                                      unsigned long long *__restrict__ work_counter, Pieces pc) {
-    __shared__ uint32_t hist[kRMaxBins];
-    __shared__ uint32_t warp_tot[kRThreads / 32];
+    constexpr int RPT = RBatch<NW>::RPT, N = RBatch<NW>::N;
+    __shared__ uint32_t hist[kRMaxBins];        // segment histogram, then the batch counts
+    __shared__ uint32_t run_off[kRMaxBins];     // a bin's first position in the batch
+    __shared__ uint32_t run_slot[kRMaxBins];    // ... and its first slot in the child
+    __shared__ uint32_t warp_tot[kRWarps];
     __shared__ unsigned long long s_w;
     __shared__ uint64_t pc_start[PIECED ? kMaxPieces : 1];
     __shared__ uint32_t pc_len[PIECED ? kMaxPieces : 1];
     extern __shared__ uint64_t sm_refine_dyn[];
-    PmBox *boxes = reinterpret_cast<PmBox *>(sm_refine_dyn);           // PAIR: one mailbox per bin
+    uint64_t *stage = sm_refine_dyn;                                                    // [N][NW] the batch in bin order
+    uint32_t *stage_slot = reinterpret_cast<uint32_t *>(stage + (size_t)N * NW);         // [N]     their slots in the segment
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (;;) {
         if (threadIdx.x == 0) s_w = atomicAdd(work_counter, 1ull);
         __syncthreads();
@@ -785,10 +792,10 @@ __global__ void __launch_bounds__(kRThreads) refine_k(const Seg *__restrict__ se
         if (PIECED) {
             // a WARP streams a piece (a few thousand consecutive records), four independent 512-byte loads in flight per warp:
             // with the whole CTA striding over one piece at a time a thread had a single 16-byte load outstanding
-            for (int g = (int)(threadIdx.x >> 5); g < pc.G; g += kRThreads / 32) {
+            for (int g = warp; g < pc.G; g += kRWarps) {
                 const uint64_t *ps = buf0 + pc_start[g] * NW;
                 const uint32_t n = pc_len[g];
-                uint32_t i = threadIdx.x & 31;
+                uint32_t i = lane;
                 for (; i + 96 < n; i += 128) {
                     const Kmer<NW> k0 = load_rec<NW>(ps + (uint64_t)i * NW), k1 = load_rec<NW>(ps + (uint64_t)(i + 32) * NW);
                     const Kmer<NW> k2 = load_rec<NW>(ps + (uint64_t)(i + 64) * NW), k3 = load_rec<NW>(ps + (uint64_t)(i + 96) * NW);
@@ -814,10 +821,9 @@ __global__ void __launch_bounds__(kRThreads) refine_k(const Seg *__restrict__ se
         // exclusive scan of hist[0..nb) (nb <= 2048 = 2 per thread)
         uint32_t a = 0, b = 0;
         const uint32_t i0 = 2 * threadIdx.x;
-        if (i0 < nb) a = hist[i0];
-        if (i0 + 1 < nb) b = hist[i0 + 1];
+        if (i0 < nb) { a = hist[i0]; hist[i0] = 0; }          // the owner's bins: the batch counts start at zero (the scan's
+        if (i0 + 1 < nb) { b = hist[i0 + 1]; hist[i0 + 1] = 0; }   // barriers order this before the first batch's atomics)
         uint32_t v = a + b, inc = v;
-        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) {
             uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
@@ -845,43 +851,84 @@ __global__ void __launch_bounds__(kRThreads) refine_k(const Seg *__restrict__ se
             Seg c; c.start = s.start + ex + a; c.len = b; c.bits = s.bits + (uint32_t)r; c.bb = s.bb ^ 1u;
             nsegs[cb + i0 + 1] = c;
         }
-        __syncthreads();
-        if (i0 < nb) hist[i0] = ex;
-        if (i0 + 1 < nb) hist[i0 + 1] = ex + a;
-        if (PAIR)
-            for (uint32_t i = threadIdx.x; i < nb; i += blockDim.x) boxes[i].state = 0u;
-        __syncthreads();
-        uint64_t *dbuf = (s.bb & 1) ? buf0 : buf1;                    // dst = dbuf + s.start * NW
-        auto put = [&](const Kmer<NW> &k) {
-            const uint32_t bin = key_bits<NW>(k, K, (int)s.bits, r);
-            const uint32_t slot = atomicAdd(&hist[bin], 1u);
-            if constexpr (PAIR && NW == 2) {
-                PairSink sink{dbuf};
-                pm_put<1>(boxes + bin, s.start, slot, k.w[0], k.w[1], sink);
+        uint32_t cur0 = ex, cur1 = ex + a;                            // the owner's two bins: next free slot in the child
+
+        // ---- scatter sweep, batch by batch
+        Kmer<NW> rec[RPT];
+        uint32_t have = 0;                        // bit j: rec[j] holds a record
+        int pg = warp;                            // PIECED: the warp's piece ...
+        uint32_t ppos = 0;                        // ... and its next record (warp-uniform)
+        uint64_t cpos = 0;                        // contiguous: the batch's first record
+        auto load_batch = [&]() {
+            have = 0;
+            if (PIECED) {
+                while (pg < pc.G && ppos >= pc_len[pg]) { pg += kRWarps; ppos = 0; }
+                if (pg < pc.G) {
+                    const uint64_t *ps = buf0 + pc_start[pg] * NW;
+                    const uint32_t n = pc_len[pg];
+#pragma unroll
+                    for (int j = 0; j < RPT; ++j) {
+                        const uint32_t i = ppos + lane + 32 * j;
+                        if (i < n) { rec[j] = load_rec<NW>(ps + (uint64_t)i * NW); have |= 1u << j; }
+                    }
+                    ppos += 32 * RPT;
+                }
             } else {
-                store_rec<NW>(dst + (uint64_t)slot * NW, k);
+#pragma unroll
+                for (int j = 0; j < RPT; ++j) {
+                    const uint64_t i = cpos + threadIdx.x + (uint64_t)kRThreads * j;
+                    if (i < s.len) { rec[j] = load_rec<NW>(src + i * NW); have |= 1u << j; }
+                }
+                cpos += N;
             }
         };
-        if (PIECED) {
-            for (int g = (int)(threadIdx.x >> 5); g < pc.G; g += kRThreads / 32) {
-                const uint64_t *ps = buf0 + pc_start[g] * NW;
-                const uint32_t n = pc_len[g];
-                uint32_t i = threadIdx.x & 31;
-                for (; i + 96 < n; i += 128) {
-                    const Kmer<NW> k0 = load_rec<NW>(ps + (uint64_t)i * NW), k1 = load_rec<NW>(ps + (uint64_t)(i + 32) * NW);
-                    const Kmer<NW> k2 = load_rec<NW>(ps + (uint64_t)(i + 64) * NW), k3 = load_rec<NW>(ps + (uint64_t)(i + 96) * NW);
-                    put(k0); put(k1); put(k2); put(k3);
+        load_batch();
+        for (;;) {
+            uint32_t tag[RPT];                    // (rank in its bin's run << 11) | bin
+#pragma unroll
+            for (int j = 0; j < RPT; ++j) {
+                if (have >> j & 1u) {
+                    const uint32_t bin = key_bits<NW>(rec[j], K, (int)s.bits, r);
+                    tag[j] = (atomicAdd(&hist[bin], 1u) << 11) | bin;
                 }
-                for (; i < n; i += 32) put(load_rec<NW>(ps + (uint64_t)i * NW));
             }
-        } else {
-            for (uint64_t i = threadIdx.x; i < s.len; i += blockDim.x) put(load_rec<NW>(src + i * NW));
-        }
-        __syncthreads();
-        if constexpr (PAIR && NW == 2) {
-            PairSink sink{dbuf};
-            for (uint32_t i = threadIdx.x; i < nb; i += blockDim.x) pm_flush_box(&boxes[i], s.start, sink);
+            if (!__syncthreads_or(have)) break;
+            // block scan of the batch counts; the owner claims each of its bins' runs and clears the count for the next batch
+            const uint32_t c0 = i0 < nb ? hist[i0] : 0u, c1 = i0 + 1 < nb ? hist[i0 + 1] : 0u;
+            const uint32_t bv = c0 + c1;
+            uint32_t binc = bv;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                uint32_t t = __shfl_up_sync(0xffffffffu, binc, o);
+                if (lane >= o) binc += t;
+            }
+            if (lane == 31) warp_tot[warp] = binc;
             __syncthreads();
+            uint32_t w = warp_tot[lane], winc = w;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                uint32_t t = __shfl_up_sync(0xffffffffu, winc, o);
+                if (lane >= o) winc += t;
+            }
+            const uint32_t total = __shfl_sync(0xffffffffu, winc, 31);
+            const uint32_t off = __shfl_sync(0xffffffffu, winc - w, warp) + binc - bv;
+            if (i0 < nb) { run_off[i0] = off; run_slot[i0] = cur0; hist[i0] = 0; cur0 += c0; }
+            if (i0 + 1 < nb) { run_off[i0 + 1] = off + c0; run_slot[i0 + 1] = cur1; hist[i0 + 1] = 0; cur1 += c1; }
+            __syncthreads();
+            // permute into bin order, then put the next batch's loads in flight before the flush
+#pragma unroll
+            for (int j = 0; j < RPT; ++j) {
+                if (have >> j & 1u) {
+                    const uint32_t bin = tag[j] & (kRMaxBins - 1), rank = tag[j] >> 11;
+                    const uint32_t p = run_off[bin] + rank;
+                    store_rec<NW>(stage + (size_t)p * NW, rec[j]);
+                    stage_slot[p] = run_slot[bin] + rank;
+                }
+            }
+            load_batch();
+            __syncthreads();
+            for (uint32_t p = threadIdx.x; p < total; p += kRThreads)
+                store_rec_stream<NW>(dst + (uint64_t)stage_slot[p] * NW, load_rec<NW>(stage + (size_t)p * NW));
         }
     }
 }
@@ -1358,21 +1405,14 @@ static void sort_pass(Ctx *ctx, int K, DArr<uint64_t> &X, DArr<uint64_t> &Y, con
         refine_copy_k<<<div_up(nsegs, 256), 256, 0, st>>>(segs.p, nsegs, isw.p, cbase.p, wpos.p, nsegs_arr.p, worklist.p);
         ctx->launches++;
         SG_CUDA(cudaMemsetAsync(wcounter.p, 0, 8, st));
-        const int grid = (int)std::min<uint64_t>(tot[1], (uint64_t)ctx->num_sms * 2);
-        // 16-byte records: the scatter phase pairs the two records of a 32-byte sector (lone 16-byte stores cost a fill read each)
-        if (NW == 2) {
-            const size_t sm = (size_t)kRMaxBins * sizeof(PmBox);
-            if (pieced) {
-                SG_CUDA(cudaFuncSetAttribute(refine_k<NW, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-                refine_k<NW, true, true><<<grid, kRThreads, sm, st>>>(segs.p, worklist.p, tot[1], cbase.p, rp, K, X.p, Y.p, nsegs_arr.p, wcounter.p, *pieces);
-            } else {
-                SG_CUDA(cudaFuncSetAttribute(refine_k<NW, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-                refine_k<NW, false, true><<<grid, kRThreads, sm, st>>>(segs.p, worklist.p, tot[1], cbase.p, rp, K, X.p, Y.p, nsegs_arr.p, wcounter.p, Pieces());
-            }
-        } else if (pieced) {
-            refine_k<NW, true, false><<<grid, kRThreads, 0, st>>>(segs.p, worklist.p, tot[1], cbase.p, rp, K, X.p, Y.p, nsegs_arr.p, wcounter.p, *pieces);
+        const int grid = (int)std::min<uint64_t>(tot[1], (uint64_t)ctx->num_sms);     // one CTA per SM: the batch fills shared memory
+        const size_t sm = RBatch<NW>::smem();
+        if (pieced) {
+            SG_CUDA(cudaFuncSetAttribute(refine_k<NW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+            refine_k<NW, true><<<grid, kRThreads, sm, st>>>(segs.p, worklist.p, tot[1], cbase.p, rp, K, X.p, Y.p, nsegs_arr.p, wcounter.p, *pieces);
         } else {
-            refine_k<NW, false, false><<<grid, kRThreads, 0, st>>>(segs.p, worklist.p, tot[1], cbase.p, rp, K, X.p, Y.p, nsegs_arr.p, wcounter.p, Pieces());
+            SG_CUDA(cudaFuncSetAttribute(refine_k<NW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+            refine_k<NW, false><<<grid, kRThreads, sm, st>>>(segs.p, worklist.p, tot[1], cbase.p, rp, K, X.p, Y.p, nsegs_arr.p, wcounter.p, Pieces());
         }
         ctx->launches++;
         SG_CUDA(cudaGetLastError());
