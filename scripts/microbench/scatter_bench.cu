@@ -23,6 +23,11 @@
 //   batch  N records per CTA per batch: rank in the bin (one shared-memory atomic), block scan of the batch counts, the owner of a
 //          bin claims its run, permute into bin order in shared memory, flush with consecutive threads on consecutive addresses
 //   ./scatter_bench -b 1 -g 8
+//
+// Level-A mode (-a 1): the same lone and batched writes at level A's shape: 640 and 2560 streams per CTA, 16- and 32-byte
+// records, two CTAs of 512 or one of 1024 threads per SM, and only the batch sizes that fit next to the shared memory the
+// partition kernel's roll state takes.
+//   ./scatter_bench -a 1 -g 8
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -94,14 +99,16 @@ __global__ void __launch_bounds__(T) rlone_k(uint64_t *out, int B, uint32_t per_
     }
 }
 
-// records of W bytes (8, 16, 32) in batches of N per CTA
-template <int T, int W, int N>
+// records of W bytes (8, 16, 32) in batches of N per CTA, up to MAXB bins (tag = rank << log2(MAXB) | bin)
+template <int T, int W, int N, int MAXB = 2048>
 __global__ void __launch_bounds__(T) rbatch_k(uint64_t *out, int B, uint32_t per_bin, uint32_t records_per_cta) {
-    constexpr int NW = W / 8, RPT = N / T, BPT = 2048 / T;       // records and bins per thread
+    constexpr int NW = W / 8, RPT = N / T, BPT = MAXB / T;       // records and bins per thread
+    constexpr int TB = MAXB == 2048 ? 11 : 12;
+    static_assert(MAXB == 2048 || MAXB == 4096, "tag layout");
     extern __shared__ uint64_t sm[];
     uint64_t *stage = sm;                                                         // [N][NW]
     uint32_t *sslot = reinterpret_cast<uint32_t *>(stage + (size_t)N * NW);       // [N] global record index
-    uint32_t *cnt = sslot + N, *roff = cnt + 2048, *rbase = roff + 2048;          // [2048] each
+    uint32_t *cnt = sslot + N, *roff = cnt + B, *rbase = roff + B;                // [B] each
     __shared__ uint32_t wtot[T / 32];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     uint32_t cur[BPT];
@@ -120,7 +127,7 @@ __global__ void __launch_bounds__(T) rbatch_k(uint64_t *out, int B, uint32_t per
             const uint32_t h = mix(i * 2654435761u + blockIdx.x * 40503u);
             const uint32_t b = h % (uint32_t)B;
             v[j] = h;
-            tag[j] = i < records_per_cta ? (atomicAdd(&cnt[b], 1u) << 11) | b : ~0u;
+            tag[j] = i < records_per_cta ? (atomicAdd(&cnt[b], 1u) << TB) | b : ~0u;
         }
         __syncthreads();
         uint32_t c[BPT], tsum = 0;
@@ -146,7 +153,7 @@ __global__ void __launch_bounds__(T) rbatch_k(uint64_t *out, int B, uint32_t per
 #pragma unroll
         for (int j = 0; j < RPT; ++j) {
             if (tag[j] == ~0u) continue;
-            const uint32_t b = tag[j] & 2047u, rank = tag[j] >> 11;
+            const uint32_t b = tag[j] & (MAXB - 1u), rank = tag[j] >> TB;
             const uint32_t p = roff[b] + rank;
             for (int k = 0; k < NW; ++k) stage[(size_t)p * NW + k] = v[j] + k;
             sslot[p] = rank + rbase[b];
@@ -192,7 +199,7 @@ static void refine_row(int B, double gb, int SMs, uint64_t *d_out, size_t out_by
     auto batch = [&](auto kern, int W, int N) {
         const uint32_t per_cta = (uint32_t)(gb * 1e9 / W / G), per_bin = (uint32_t)((uint64_t)per_cta * 5 / 4 / B + 8) & ~1u;
         if ((uint64_t)per_bin * B * G * W > out_bytes) { fprintf(stderr, "buffer too small\n"); exit(1); }
-        const size_t sm = (size_t)N * (W + 4) + 3 * 2048 * 4;
+        const size_t sm = (size_t)N * (W + 4) + 3 * (size_t)B * 4;
         if (sm > 220u << 10 || (1024 / T) * sm > 226u << 10) return -1.f;          // does not fit (1024 / T) CTAs per SM
         CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
         return rtime([&] { kern<<<G, T, sm>>>(d_out, B, per_bin, per_cta); }, (double)per_cta * G * W);
@@ -200,6 +207,42 @@ static void refine_row(int B, double gb, int SMs, uint64_t *d_out, size_t out_by
     printf("%5d x %4d | %5d | %6.0f %6.0f | %6.0f %6.0f %6.0f | %6.0f %6.0f | %6.0f\n", 1024 / T, T, B, lone(false), lone(true),
            batch(rbatch_k<T, 16, 2048>, 16, 2048), batch(rbatch_k<T, 16, 4096>, 16, 4096), batch(rbatch_k<T, 16, 8192>, 16, 8192),
            batch(rbatch_k<T, 8, 8192>, 8, 8192), batch(rbatch_k<T, 8, 16384>, 8, 16384), batch(rbatch_k<T, 32, 4096>, 32, 4096));
+    fflush(stdout);
+}
+
+// Level-A mode (-a 1): the write pattern of levelA_scatter_roll_k -- S = 640 or 2560 partition streams per CTA, CTA-major
+// regions, 16- or 32-byte records -- at two CTAs of 512 threads or one of 1024 per SM. Every CTA also holds the shared memory of
+// the roll kernel's warp slices (2952 bytes per warp), so a batch only gets what is left next to them and the batch tables
+// (3 x 4 bytes per stream); "-" marks a batch that does not fit that room.
+template <int T>
+static void levela_row(int S, int W, double gb, int SMs, uint64_t *d_out, size_t out_bytes) {
+    const int G = SMs * (1024 / T);
+    const size_t roll = (size_t)(T / 32) * 2952;
+    const size_t room = T == 1024 ? 232448 - 128 : 115584 - 128;        // opt-in limit per CTA; half an SM minus the reservation
+    const uint32_t per_cta = (uint32_t)(gb * 1e9 / W / G), per_bin = (uint32_t)((uint64_t)per_cta * 5 / 4 / S + 8) & ~1u;
+    if ((uint64_t)per_bin * S * G * W > out_bytes) { fprintf(stderr, "buffer too small\n"); exit(1); }
+    auto lone = [&]() {
+        auto k = W == 16 ? rlone_k<T, 16, false> : rlone_k<T, 16, true>;
+        const size_t sm = roll + (size_t)S * 4;
+        CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+        const uint32_t pc = W == 16 ? per_cta : 2 * per_cta, pb = W == 16 ? per_bin : 2 * per_bin;    // 16-byte units
+        return rtime([&] { k<<<G, T, sm>>>(d_out, S, pb, pc); }, (double)per_cta * G * W);
+    };
+    auto batch = [&](auto kern, int N) {
+        const size_t sm = (size_t)N * (W + 4) + 3 * (size_t)S * 4 + roll;
+        if (N % T || sm > room) return -1.f;
+        CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+        return rtime([&] { kern<<<G, T, sm>>>(d_out, S, per_bin, per_cta); }, (double)per_cta * G * W);
+    };
+    printf("%5d x %4d | %5d | %3d | %6.0f", 1024 / T, T, S, W, lone());
+    if (W == 16)
+        printf(" | %6.0f %6.0f %6.0f %6.0f %6.0f %6.0f\n", batch(rbatch_k<T, 16, 1024, 4096>, 1024), batch(rbatch_k<T, 16, 2048, 4096>, 2048),
+               batch(rbatch_k<T, 16, 3072, 4096>, 3072), batch(rbatch_k<T, 16, 4096, 4096>, 4096), batch(rbatch_k<T, 16, 5120, 4096>, 5120),
+               batch(rbatch_k<T, 16, 6144, 4096>, 6144));
+    else
+        printf(" | %6.0f %6.0f %6.0f %6.0f %6.0f %6.0f\n", batch(rbatch_k<T, 32, 1024, 4096>, 1024), batch(rbatch_k<T, 32, 2048, 4096>, 2048),
+               batch(rbatch_k<T, 32, 3072, 4096>, 3072), batch(rbatch_k<T, 32, 4096, 4096>, 4096), batch(rbatch_k<T, 32, 5120, 4096>, 5120),
+               batch(rbatch_k<T, 32, 6144, 4096>, 6144));
     fflush(stdout);
 }
 
@@ -256,7 +299,7 @@ static float run(int width, int S, bool cta_major, double gb, int G, uint64_t *d
 
 int main(int argc, char **argv) {
     double gb = 8.0, cta_mb = 0;
-    int S = 640, refine_mode = 0;
+    int S = 640, refine_mode = 0, levela_mode = 0;
     std::vector<double> slice_mb;
     for (int i = 1; i + 1 < argc; i += 2) {
         if (!strcmp(argv[i], "-g")) gb = atof(argv[i + 1]);
@@ -264,9 +307,27 @@ int main(int argc, char **argv) {
         else if (!strcmp(argv[i], "-S")) S = atoi(argv[i + 1]);
         else if (!strcmp(argv[i], "-r")) slice_mb.push_back(atof(argv[i + 1]));
         else if (!strcmp(argv[i], "-b")) refine_mode = atoi(argv[i + 1]);
+        else if (!strcmp(argv[i], "-a")) levela_mode = atoi(argv[i + 1]);
     }
     cudaDeviceProp p; CK(cudaGetDeviceProperties(&p, 0));
     const int G = p.multiProcessorCount * 2;
+    if (levela_mode) {
+        const size_t out_bytes = (size_t)(gb * 1.4e9) + (64u << 20);
+        uint64_t *d_out;
+        CK(cudaMalloc(&d_out, out_bytes));
+        CK(cudaMemset(d_out, 0, out_bytes));
+        printf("%s, level-A write pattern next to the roll kernel's warp slices, %.1f GB per run; GB/s of record bytes, best of 3 "
+               "(-: does not fit)\n", p.name, gb);
+        printf("%12s | %5s | %3s | %6s | %6s %6s %6s %6s %6s %6s\n", "CTAs x thr", "strms", "W", "lone", "b/1k", "b/2k", "b/3k", "b/4k",
+               "b/5k", "b/6k");
+        for (int S2 : {640, 2560})
+            for (int W : {16, 32}) {
+                levela_row<512>(S2, W, gb, p.multiProcessorCount, d_out, out_bytes);
+                levela_row<1024>(S2, W, gb, p.multiProcessorCount, d_out, out_bytes);
+            }
+        CK(cudaFree(d_out));
+        return 0;
+    }
     if (refine_mode) {
         const size_t out_bytes = (size_t)(gb * 1.4e9) + (64u << 20);
         uint64_t *d_out;

@@ -524,110 +524,221 @@ __global__ void __launch_bounds__(kRollThreads, 2) levelA_count_roll_k(ReadsSrc 
 
 // base rows are `row_stride` cursors long; this launch handles the partitions [q_lo, q_lo + p.PA) of a row (p.PA = the
 // sub-range's size, id_lo = id of its first partition): a bucket-group pass may be split into partition sub-ranges so that
-// the streams (partial lines) a CTA has open at any time stay few. What sets the rate of these 16-byte scattered stores is the
-// number of open streams per CTA and the store width, not how many pages a CTA's region spans (DESIGN.md 6.2).
-// (A sector-pairing variant of this kernel -- two records of a stream leave as one 32-byte store through shared-memory
-// mailboxes -- was parity clean but slower: the CAS traffic on the mailboxes cost more than the full sectors won. Removed.)
+// the streams a CTA has open at any time stay few.
+// Records stored one by one as they are rolled leave L2 as partly written sectors: with PA = 640 streams per CTA a stream
+// receives a record only every few microseconds, and lone 16-byte stores at 640 streams run at about a ninth of the HBM rate
+// (DESIGN.md 6.2). The kernel therefore collects its own windows in a shared-memory batch and writes it out partition by
+// partition, as refine_k does:
+// - a warp reserves room for one window step of its lanes with one shared-memory atomic, and a record takes its rank in its
+//   partition with another (the cursor atomic of the store-as-you-go form);
+// - when a reservation does not fit, the warp stops with that window pending, and every warp meets at the flush: a scan of the
+//   batch counts places each partition's run in the batch and claims it from the partition's cursor, an index array permutes
+//   the batch into partition order, and consecutive threads store consecutive records of a run;
+// - warps without work left, and lanes without a chunk, keep reaching the barriers (__syncthreads_or on "work left").
+// The order inside a partition is arbitrary, as it was with atomic slots.
+// `-Xptxas -v` at 64 registers: no stack frame at 1 and 2 words per record; 16 / 56 bytes with ids and 0 / 32 bytes without at 3
+// and 4 words (the chunk's id queue, the pending window and the tile state all live across the flush). Their cost at K > 64 is
+// not measured.
+// (A sector-pairing variant -- two records of a stream leave as one 32-byte store through shared-memory mailboxes -- was
+// parity clean but slower: the CAS traffic on the mailboxes cost more than the full sectors won. Removed.)
+static const uint32_t kABatchNoTag = 0xffffffffu;      // an arrival slot of the batch that a warp reserved but did not fill
+static const int kABatchPartBits = 13;                 // tag = (rank << 13) | partition, partition < kLevelAMaxParts
+// Below kABatchMin records at two CTAs per SM, one CTA per SM takes a larger batch. The threshold itself is not tuned; in
+// scatter_bench -a 1 (DESIGN.md 6.2) 1024-record batches at two CTAs of 512 run at 546 / 278 GB/s (640 / 2560 streams, 16-byte
+// records); the fallback's shape, one CTA of 512 threads per SM with the larger batch, is not in that table.
+static const uint32_t kABatchMin = 1024;
+template <int NW> struct ABatch {
+    static constexpr size_t rec_bytes() { return NW * sizeof(uint64_t) + sizeof(uint32_t) + sizeof(uint16_t); }   // record, tag, index
+};
+// dynamic shared memory: [cursor | batch count] per partition, the warps' RollWarp slices, then the batch
+__host__ __device__ __forceinline__ size_t abatch_offset(uint32_t PA) {
+    return ((((size_t)2 * PA * 4 + 15) & ~(size_t)15) + (size_t)kRollWarps * sizeof(RollWarp) + 15) & ~(size_t)15;
+}
+
 template <int NW, bool HAS_IDS>
 __global__ void __launch_bounds__(kRollThreads, 2) levelA_scatter_roll_k(ReadsSrc src, LevelA p, uint64_t *__restrict__ base, uint64_t *__restrict__ out,
                                                                         const uint64_t *__restrict__ tile_off, const uint16_t *__restrict__ ids,
-                                                                        uint32_t id_lo, uint32_t row_stride, uint32_t q_lo, uint64_t ids_len) {
+                                                                        uint32_t id_lo, uint32_t row_stride, uint32_t q_lo, uint64_t ids_len, uint32_t cap) {
     extern __shared__ __align__(16) unsigned char sm_raw[];
+    __shared__ uint32_t s_fill;                   // arrival slots reserved in the batch (may run past cap)
+    __shared__ uint32_t warp_tot[kRollWarps];
+    const uint32_t PA = p.PA;
     // one 32-bit cursor per partition, relative to the first record this launch may write (a CTA's share of a pass is far below
-    // 2^32 records): the slot of a record is ONE shared-memory atomic, no base lookup and no 64-bit add behind it
-    uint32_t *cur = reinterpret_cast<uint32_t *>(sm_raw);               // PA u32
-    RollWarp &rw = *roll_warp_slice(sm_raw, p.PA);
+    // 2^32 records); the batch count of a partition in the low 16 bits of cnt, the end of its run in the batch in the high 16
+    uint32_t *cur = reinterpret_cast<uint32_t *>(sm_raw);               // PA
+    uint32_t *cnt = cur + PA;                                           // PA
+    RollWarp &rw = *roll_warp_slice(sm_raw, 2 * PA);
+    uint64_t *stage = reinterpret_cast<uint64_t *>(sm_raw + abatch_offset(PA));    // [cap][NW] records in arrival order
+    uint32_t *tags = reinterpret_cast<uint32_t *>(stage + (size_t)cap * NW);      // [cap]     (rank << 13) | partition
+    uint16_t *idx = reinterpret_cast<uint16_t *>(tags + cap);                     // [cap]     arrival slot of a batch position
     uint64_t *mybase = base + (size_t)blockIdx.x * row_stride + q_lo;
     const uint64_t region0 = mybase[0];                                 // cursors of a row ascend with the partition
-    for (uint32_t i = threadIdx.x; i < p.PA; i += blockDim.x) cur[i] = (uint32_t)(mybase[i] - region0);
+    for (uint32_t i = threadIdx.x; i < PA; i += blockDim.x) { cur[i] = (uint32_t)(mybase[i] - region0); cnt[i] = 0; }
+    if (threadIdx.x == 0) s_fill = 0;
     __syncthreads();
     uint64_t *const out0 = out + region0 * NW;
     const int K = p.K;
-    const uint32_t PA = p.PA;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t lt_mask = (1u << lane) - 1u;
     const int64_t ntiles = (src.n + kRollTile - 1) / kRollTile;
     const int64_t per = (ntiles + gridDim.x - 1) / gridDim.x;
     const int64_t t0 = (int64_t)blockIdx.x * per, t1 = min(ntiles, t0 + per);
-    for (int64_t t = t0 + warp; t < t1; t += kRollWarps) {
-        const int64_t item0 = t * kRollTile;
-        const int nitems = (int)min((int64_t)kRollTile, src.n - item0);
-        uint32_t unif = 0;
-        bool staged = false;
-        // the warp's next tile is kRollWarps tiles ahead: its lengths and offsets go to L2 now, its packed reads (and id rows) at the
-        // end of this tile, when the loads of their addresses issued here have long returned
-        const bool has_next = t + kRollWarps < t1;
-        const int64_t nx = (t + kRollWarps) * kRollTile;
-        uint64_t next_w0 = 0;
-        if (has_next) {
-            next_w0 = src.offs[nx];
-            if (lane == 0) prefetch_l2(src.lens + nx);
-            else if (lane == 1 && nx + 16 < src.n) prefetch_l2(src.offs + nx + 16);
-        }
-        uint64_t next_row = 0;
-        if (HAS_IDS && has_next) next_row = tile_off[t + kRollWarps];
-        const uint32_t nunits = roll_warp_setup(src, item0, nitems, rw, &unif, &staged);
-        const ulonglong2 *row = HAS_IDS ? reinterpret_cast<const ulonglong2 *>(ids + tile_off[t]) : nullptr;
-        for (uint32_t u = lane; u < nunits; u += 32) {
-            uint64_t idw[kRollC / 4];
-            if (HAS_IDS) {
-                // the chunk's 24 ids, in flight while the window is set up
+
+    // the warp's tile and the lane's chunk survive a flush: a warp that finds the batch full resumes at its pending window
+    int64_t t = t0 + warp;
+    bool need_setup = true;
+    int nitems = 0;
+    uint32_t nunits = 0, unif = 0;
+    bool staged = false;
+    uint64_t next_w0 = 0, next_row = 0;
+    const ulonglong2 *row = nullptr;
+    int u = 0, s = 0, cnt_w = 0;                  // the lane's chunk, its window (st is at it), its windows
+    RollState<NW> st;
+    uint64_t idq[kRollC / 4];                     // HAS_IDS: the chunk's ids from window s on, two bytes each
+    for (;;) {
+        while (t < t1) {                          // warp-uniform
+            if (need_setup) {
+                const int64_t item0 = t * kRollTile;
+                nitems = (int)min((int64_t)kRollTile, src.n - item0);
+                // the warp's next tile is kRollWarps tiles ahead: its lengths and offsets go to L2 now, its packed reads (and id
+                // rows) at the end of this tile, when the loads of their addresses issued here have long returned
+                const int64_t nx = (t + kRollWarps) * kRollTile;
+                if (t + kRollWarps < t1) {
+                    next_w0 = src.offs[nx];
+                    if (lane == 0) prefetch_l2(src.lens + nx);
+                    else if (lane == 1 && nx + 16 < src.n) prefetch_l2(src.offs + nx + 16);
+                    if (HAS_IDS) next_row = tile_off[t + kRollWarps];
+                }
+                nunits = roll_warp_setup(src, item0, nitems, rw, &unif, &staged);
+                if (HAS_IDS) row = reinterpret_cast<const ulonglong2 *>(ids + tile_off[t]);
+                u = lane - 32; s = cnt_w = 0;
+                need_setup = false;
+            }
+            if (s >= cnt_w && u < (int)nunits) {  // the lane's next chunk
+                u += 32;
+                if (u < (int)nunits) {
+                    if (HAS_IDS) {
 #pragma unroll
-                for (int v = 0; v < kRollC / 8; ++v) {
-                    const ulonglong2 x = __ldg(row + (size_t)u * (kRollC / 8) + v);
-                    idw[2 * v] = x.x; idw[2 * v + 1] = x.y;
+                        for (int v = 0; v < kRollC / 8; ++v) {
+                            const ulonglong2 x = __ldg(row + (size_t)u * (kRollC / 8) + v);
+                            idq[2 * v] = x.x; idq[2 * v + 1] = x.y;
+                        }
+                    }
+                    const RollUnit q = roll_unit(rw, nitems, (uint32_t)u, unif, K);
+                    const uint64_t *seq = staged ? static_cast<const uint64_t *>(rw.words + rw.off[q.it]) : src.words + src.offs[t * kRollTile + q.it];
+                    roll_init<NW>(st, seq, q.j0, K, q.cnt);
+                    s = 0; cnt_w = q.cnt;
                 }
             }
-            const RollUnit q = roll_unit(rw, nitems, u, unif, K);
-            const uint64_t *seq = staged ? static_cast<const uint64_t *>(rw.words + rw.off[q.it]) : src.words + src.offs[item0 + q.it];
-            RollState<NW> st;
-            roll_init<NW>(st, seq, q.j0, K, q.cnt);
-            // (Delaying a window's store by one window, so that the atomic's latency hides behind the next roll, and 3..6 CTAs per
-            // SM to even out the tail were both tried: no gain either way.)
-#pragma unroll
-            for (int s = 0; s < kRollC; ++s) {
-                if (s >= q.cnt) break;
-                if (s > 0) roll_next<NW>(st, K);
-                uint32_t part;
-                bool mine;
+            const bool act = s < cnt_w;
+            if (!__any_sync(0xffffffffu, act)) {  // the tile is done
+                if (t + kRollWarps < t1) {
+                    if (lane < 10 && next_w0 + 16 * lane < src.nwords) prefetch_l2(src.words + next_w0 + 16 * lane);   // 10 lines = 32 reads x 5 words
+                    if (HAS_IDS) {                                                                                      // 48 lines for 128 chunks
+                        if (next_row + 64 * lane < ids_len) prefetch_l2(ids + next_row + 64 * lane);
+                        if (lane < 16 && next_row + 64 * (32 + lane) < ids_len) prefetch_l2(ids + next_row + 64 * (32 + lane));
+                    }
+                }
+                __syncwarp();                     // the slice is rewritten by the next tile's setup
+                t += kRollWarps;
+                need_setup = true;
+                continue;
+            }
+            uint32_t part = 0;
+            bool mine = false;
+            Kmer<NW> k;
+            if (act) {
+                // a foreign window costs the roll and this compare; the canonical choice is made for own windows only
+                // (a word-by-word select: `cond ? st.f : st.r` bound to a reference made the compiler keep the roll state in
+                // local memory to pick an address)
                 if (HAS_IDS) {
-                    // a foreign window costs the roll and this compare; the canonical choice is made for own windows only
-                    part = (uint32_t)((idw[s >> 2] >> (16 * (s & 3))) & 0xffffu) - id_lo;         // 0xffff - id_lo stays >= PA
+                    part = (uint32_t)(idq[0] & 0xffffu) - id_lo;               // 0xffff - id_lo stays >= PA
                     mine = part < PA;
-                    if (mine) {
-                        const uint32_t slot = atomicAdd(&cur[part], 1u);
-                        // a word-by-word select: `cond ? st.f : st.r` bound to the store's reference argument made the compiler
-                        // keep the whole roll state in local memory (5 spill stores per window) to pick an address
-                        const bool fwd = kmer_is_minimal<NW>(st.f, st.r);
-                        Kmer<NW> k;
+                }
+                if (!HAS_IDS || mine) {
+                    const bool fwd = kmer_is_minimal<NW>(st.f, st.r);
 #pragma unroll
-                        for (int j = 0; j < NW; ++j) k.w[j] = fwd ? st.f.w[j] : st.r.w[j];
-                        store_rec_stream<NW>(out0 + (size_t)slot * NW, k);
-                    }
-                } else {
-                    const Kmer<NW> k = kmer_is_minimal<NW>(st.f, st.r) ? st.f : st.r;
-                    mine = part_of<NW>(p, k, &part);
-                    if (mine) {
-                        const uint32_t slot = atomicAdd(&cur[part], 1u);
-                        store_rec_stream<NW>(out0 + (size_t)slot * NW, k);
+                    for (int j = 0; j < NW; ++j) k.w[j] = fwd ? st.f.w[j] : st.r.w[j];
+                }
+                if (!HAS_IDS) mine = part_of<NW>(p, k, &part);
+            }
+            const uint32_t bal = __ballot_sync(0xffffffffu, mine);
+            if (bal) {
+                const uint32_t n = __popc(bal);
+                uint32_t b0 = 0;
+                if (lane == 0) b0 = atomicAdd(&s_fill, n);
+                b0 = __shfl_sync(0xffffffffu, b0, 0);
+                if (b0 + n > cap) {               // full: the window stays pending; the slots reserved below cap stay empty
+                    if (b0 < cap && (uint32_t)lane < cap - b0) tags[b0 + lane] = kABatchNoTag;
+                    break;
+                }
+                if (mine) {
+                    const uint32_t i = b0 + __popc(bal & lt_mask);
+                    const uint32_t rank = atomicAdd(&cnt[part], 1u) & 0xffffu;
+                    store_rec<NW>(stage + (size_t)i * NW, k);
+                    tags[i] = (rank << kABatchPartBits) | part;
+                }
+            }
+            if (act && ++s < cnt_w) {
+                roll_next<NW>(st, K);
+                if (HAS_IDS) {
+                    if ((s & 3) == 0) {
+#pragma unroll
+                        for (int v = 0; v + 1 < kRollC / 4; ++v) idq[v] = idq[v + 1];
+                    } else {
+                        idq[0] >>= 16;
                     }
                 }
             }
         }
-        if (has_next && lane < 10 && next_w0 + 16 * lane < src.nwords) prefetch_l2(src.words + next_w0 + 16 * lane);   // 10 lines = 32 reads x 5 words
-        if (HAS_IDS && has_next) {                                              // the next tile's id rows: 48 lines for 128 chunks
-            if (next_row + 64 * lane < ids_len) prefetch_l2(ids + next_row + 64 * lane);
-            if (lane < 16 && next_row + 64 * (32 + lane) < ids_len) prefetch_l2(ids + next_row + 64 * (32 + lane));
+        const bool more = __syncthreads_or(t < t1);
+        // ---- flush: scan of the batch counts (a thread owns a run of consecutive partitions), the runs claimed from the cursors
+        const uint32_t nslots = min(s_fill, cap);
+        const uint32_t own = (PA + kRollThreads - 1) / kRollThreads;
+        const uint32_t j0 = min(PA, threadIdx.x * own), j1 = min(PA, j0 + own);
+        uint32_t sum = 0;
+        for (uint32_t j = j0; j < j1; ++j) sum += cnt[j] & 0xffffu;
+        uint32_t inc = sum;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t v = __shfl_up_sync(0xffffffffu, inc, o);
+            if (lane >= o) inc += v;
         }
-        __syncwarp();                                   // the slice is rewritten by the next tile's setup
+        if (lane == 31) warp_tot[warp] = inc;
+        __syncthreads();
+        uint32_t wb = 0, total = 0;
+#pragma unroll
+        for (int w = 0; w < kRollWarps; ++w) { const uint32_t v = warp_tot[w]; if (w < warp) wb += v; total += v; }
+        uint32_t o = wb + inc - sum;
+        for (uint32_t j = j0; j < j1; ++j) {
+            const uint32_t c = cnt[j] & 0xffffu;
+            o += c;
+            cnt[j] = o << 16;                     // run end; the count starts again at zero
+            cur[j] += c;                          // the run takes slots [cur - c, cur)
+        }
+        if (threadIdx.x == 0) s_fill = 0;
+        __syncthreads();
+        // rank r of a run goes to position end - 1 - r and slot cur - 1 - r: consecutive positions, consecutive slots
+        for (uint32_t i = threadIdx.x; i < nslots; i += kRollThreads) {
+            const uint32_t tg = tags[i];
+            if (tg == kABatchNoTag) continue;
+            idx[(cnt[tg & ((1u << kABatchPartBits) - 1)] >> 16) - 1 - (tg >> kABatchPartBits)] = (uint16_t)i;
+        }
+        __syncthreads();
+        for (uint32_t q = threadIdx.x; q < total; q += kRollThreads) {
+            const uint32_t i = idx[q], tg = tags[i];
+            const uint32_t slot = cur[tg & ((1u << kABatchPartBits) - 1)] - 1 - (tg >> kABatchPartBits);
+            store_rec_stream<NW>(out0 + (size_t)slot * NW, load_rec<NW>(stage + (size_t)i * NW));
+        }
+        __syncthreads();                          // the next batch overwrites the stage
+        if (!more) break;
     }
-    __syncthreads();
     for (uint32_t i = threadIdx.x; i < PA; i += blockDim.x) mybase[i] = region0 + cur[i];   // chained launches continue here
 }
-
-// (A third generation of this kernel -- id sweep, 32-bit keys collected without atomics, ballot-ranked LSD sort of the batch in
-// shared memory, run-by-run flush with consecutive threads storing consecutive records of one partition -- was parity clean with
-// full-sector stores, and slower: about twice the thread instructions per record (barriers + dependent ballot / shared-memory
-// chains) of roll + atomic + 16-byte store. Removed.)
+// Measured (H100 80GB HBM3, 700 W, 40 M x 150 bp, k = 55, 4 passes, PA = 640, batches of 2848 records at two CTAs per SM): 129 ms
+// per step against 189 ms for the form that stored each record as it was rolled. (A third generation of this kernel -- id sweep,
+// 32-bit keys collected without atomics, ballot-ranked LSD sort of the batch in shared memory, run-by-run flush -- was parity
+// clean and slower than the store-as-you-go form: about twice the thread instructions per record. Removed.)
 
 // ------------------------------------------------------------------------------------------------------------
 // segments
@@ -1502,6 +1613,25 @@ struct LevelAJob {
 // CTAs of the level-A grid per SM: the two that are resident. (More waves -- 3, 4, 6 per SM -- for tail balance gained a few
 // per cent at best, with 3x smaller pieces for the gather. Not kept.)
 static int levelA_ctas_per_sm() { return 2; }
+// dynamic shared memory of one levelA_scatter_roll_k launch over PA partitions, and its batch capacity in records: the batch
+// takes what the tables and warp slices leave of an SM's share for the two CTAs per SM the grid is sized for (2 x 113 KB of the
+// 228 KB of an H100 SM). Where the largest tables would leave less than kABatchMin records, the batch takes what a single CTA
+// may opt into, and one CTA per SM is resident.
+template <int NW>
+static size_t levelA_batch_smem(uint32_t PA, uint32_t *cap) {
+    static_assert(kLevelAMaxParts <= (1 << kABatchPartBits), "a batch tag holds the partition");
+    int dev = 0, per_sm = 0, per_cta = 0, reserved = 0;
+    SG_CUDA(cudaGetDevice(&dev));
+    SG_CUDA(cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
+    SG_CUDA(cudaDeviceGetAttribute(&per_cta, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    SG_CUDA(cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev));
+    const size_t rec = ABatch<NW>::rec_bytes(), fixed = abatch_offset(PA), kStatic = 128;   // s_fill, warp_tot
+    size_t room = (size_t)per_sm / levelA_ctas_per_sm() - (size_t)reserved - kStatic;
+    if (room < fixed + kABatchMin * rec) room = (size_t)per_cta - kStatic;
+    SG_CHECK(room >= fixed + kABatchMin * rec, 6, "internal: level-A batch does not fit shared memory");
+    *cap = (uint32_t)std::min<size_t>((room - fixed) / rec, 32768) & ~31u;     // positions in a batch are 16-bit
+    return fixed + (size_t)*cap * rec;
+}
 static int levelA_key_bits(uint64_t est_records, int B, int total_bits, uint32_t target, uint32_t pa_max) {
     const int want = ilog2_floor(est_records / target + 1) + 1;
     const int bbits = ilog2_floor((uint64_t)B) + (((1u << ilog2_floor((uint64_t)B)) < (uint32_t)B) ? 1 : 0);
@@ -1604,9 +1734,6 @@ static void levelA_scatter(LevelAJob<NW, Src> &job, int b_lo, int b_hi, uint64_t
     tm.start();
     if (job.roll) {
         if constexpr (std::is_same<Src, ReadsSrc>::value) {
-            const size_t smem = roll_smem_bytes(PA);
-            SG_CUDA(cudaFuncSetAttribute(levelA_scatter_roll_k<NW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            SG_CUDA(cudaFuncSetAttribute(levelA_scatter_roll_k<NW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             {
             // partition sub-ranges (only with the id array, where a foreign window costs just the roll): fewer streams open
             // per CTA. A sub-range costs one more roll over ALL windows of the source: worth it when the pass holds most of the job's
@@ -1620,14 +1747,17 @@ static void levelA_scatter(LevelAJob<NW, Src> &job, int b_lo, int b_hi, uint64_t
                 if (q_hi == q_lo) continue;
                 LevelA pa_sub = pa;
                 pa_sub.PA = q_hi - q_lo;
-                const size_t smem_sub = roll_smem_bytes(pa_sub.PA);
+                uint32_t cap = 0;
+                const size_t smem = levelA_batch_smem<NW>(pa_sub.PA, &cap);
+                if (job.use_ids) SG_CUDA(cudaFuncSetAttribute(levelA_scatter_roll_k<NW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                else SG_CUDA(cudaFuncSetAttribute(levelA_scatter_roll_k<NW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
                 for (size_t si = 0; si < job.srcs.size(); ++si) {
                     const Src &src = job.srcs[si];
                     if (src.n == 0) continue;
                     if (job.use_ids)
-                        levelA_scatter_roll_k<NW, true><<<G, kRollThreads, smem_sub, st>>>(src, pa_sub, base.p, X, job.tile_off[si].p, job.ids[si].p, p_lo + q_lo, PA, q_lo, (uint64_t)job.ids[si].n);
+                        levelA_scatter_roll_k<NW, true><<<G, kRollThreads, smem, st>>>(src, pa_sub, base.p, X, job.tile_off[si].p, job.ids[si].p, p_lo + q_lo, PA, q_lo, (uint64_t)job.ids[si].n, cap);
                     else
-                        levelA_scatter_roll_k<NW, false><<<G, kRollThreads, smem, st>>>(src, pa, base.p, X, nullptr, nullptr, 0u, PA, 0u, 0ull);
+                        levelA_scatter_roll_k<NW, false><<<G, kRollThreads, smem, st>>>(src, pa, base.p, X, nullptr, nullptr, 0u, PA, 0u, 0ull, cap);
                     ctx->launches++; ctx->times.level_a_scatters++;
                 }
             }
