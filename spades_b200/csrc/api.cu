@@ -595,13 +595,14 @@ __host__ __device__ uint64_t selftest_one(int op, int K, uint64_t arg, const uin
     }
 }
 // op 10: the rolling window of the level-A kernels against direct extraction. keys = one packed sequence of n*NW words,
-// arg = its length in bases; unit u walks windows [24u, 24u+24). out[u] = (windows walked << 32) | mismatches.
+// arg = (C << 32) | its length in bases, C = windows per chunk (24 canonical, 12 all-windows; 0 = 24); unit u walks windows
+// [C u, C u + C). out[u] = (windows walked << 32) | mismatches.
 template <int NW>
-__host__ __device__ uint64_t selftest_roll_unit(int K, int L, const uint64_t *seq, int64_t u) {
+__host__ __device__ uint64_t selftest_roll_unit(int K, int L, int C, const uint64_t *seq, int64_t u) {
     const int nwin = L - K + 1;
-    const int64_t j0 = u * 24;
+    const int64_t j0 = u * C;
     if (j0 >= nwin) return 0;
-    const int cnt = nwin - j0 < 24 ? (int)(nwin - j0) : 24;
+    const int cnt = nwin - j0 < C ? (int)(nwin - j0) : C;
     RollState<NW> st;
     roll_init<NW>(st, seq, (int)j0, K, cnt);
     uint64_t bad = 0;
@@ -614,9 +615,9 @@ __host__ __device__ uint64_t selftest_roll_unit(int K, int L, const uint64_t *se
     return ((uint64_t)cnt << 32) | bad;
 }
 template <int NW>
-__global__ void selftest_roll_k(int K, int L, const uint64_t *seq, int64_t n, uint64_t *out) {
+__global__ void selftest_roll_k(int K, int L, int C, const uint64_t *seq, int64_t n, uint64_t *out) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = selftest_roll_unit<NW>(K, L, seq, i);
+    if (i < n) out[i] = selftest_roll_unit<NW>(K, L, C, seq, i);
 }
 template <int NW>
 __global__ void selftest_k(int op, int K, uint64_t arg, const uint64_t *keys, int64_t n, uint64_t *out) {
@@ -625,32 +626,26 @@ __global__ void selftest_k(int op, int K, uint64_t arg, const uint64_t *keys, in
 }
 template <int NW>
 static void selftest_nw(Ctx *c, int on_device, int op, int K, uint64_t arg, const uint64_t *keys, int64_t n, uint64_t *out) {
-    if (op == 10) SG_CHECK((int64_t)arg >= K && (int64_t)arg <= 32 * n * NW, SGPU_EINVAL, "roll self test: bad sequence length");
+    const int64_t L = (int64_t)(uint32_t)arg, C = (arg >> 32) ? (int64_t)(arg >> 32) : 24;
+    if (op == 10) SG_CHECK(L >= K && L <= 32 * n * NW && C >= 1 && C <= 33, SGPU_EINVAL, "roll self test: bad sequence length or chunk width");
     if (!on_device) {
-        for (int64_t i = 0; i < n; ++i) out[i] = op == 10 ? selftest_roll_unit<NW>(K, (int)arg, keys, i) : selftest_one<NW>(op, K, arg, keys + i * NW);
+        for (int64_t i = 0; i < n; ++i) out[i] = op == 10 ? selftest_roll_unit<NW>(K, (int)L, (int)C, keys, i) : selftest_one<NW>(op, K, arg, keys + i * NW);
         return;
     }
     SG_CHECK(c, SGPU_EINVAL, "device self test needs a context");
     DArr<uint64_t> dk(c, (size_t)n * NW), dout(c, (size_t)n);
     SG_CUDA(cudaMemcpyAsync(dk.p, keys, (size_t)n * NW * 8, cudaMemcpyHostToDevice, c->stream));
-    if (op == 10) selftest_roll_k<NW><<<div_up(n, 256), 256, 0, c->stream>>>(K, (int)arg, dk.p, n, dout.p);
+    if (op == 10) selftest_roll_k<NW><<<div_up(n, 256), 256, 0, c->stream>>>(K, (int)L, (int)C, dk.p, n, dout.p);
     else selftest_k<NW><<<div_up(n, 256), 256, 0, c->stream>>>(op, K, arg, dk.p, n, dout.p);
     c->launches++;
     SG_CUDA(cudaGetLastError());
     SG_CUDA(cudaMemcpyAsync(out, dout.p, (size_t)n * 8, cudaMemcpyDeviceToHost, c->stream));
     SG_CUDA(cudaStreamSynchronize(c->stream));
 }
-// op 11 (host only): the sector-pairing mailbox protocol of pair_mailbox.cuh under real concurrency, see selftest_host.cpp
-extern "C" int sg_selftest_pair_mailbox(uint64_t arg, int64_t per_thread, uint64_t *out);
-
 extern "C" int sgpu_selftest(sgpu_ctx *ctx, int on_device, int op, int K, uint64_t arg, const uint64_t *keys, int64_t n, uint64_t *out) {
     if (K < 1 || K > 128 || n < 0 || (n && (!keys || !out))) return SGPU_EINVAL;
     Ctx *c = ctx ? &ctx->c : nullptr;
     if (on_device && !c) return SGPU_EINVAL;
-    if (op == 11) {
-        if (on_device || n < 3) return SGPU_EINVAL;
-        return sg_selftest_pair_mailbox(arg, (int64_t)keys[0], out);
-    }
     API_TRY(c, {
         if (on_device) SG_CUDA(cudaSetDevice(c->device));
         switch (nwords_of(K)) {

@@ -19,15 +19,18 @@
 #include <time.h>
 
 #include <algorithm>
-#include <type_traits>
 
 #include "sgpu_internal.h"
 
 namespace sg {
 
 // ------------------------------------------------------------------------------------------------------------
-// record sources
+// record sources: items are packed sequences (nucleotide i at bits 2(i%32) of word i/32, kmer_dev.cuh) whose K-windows are the
+// records. The level-A kernels see an item through first_word / len / words only. kIds: partition ids per chunk (the id row of
+// a chunk, a whole number of 16-byte words); kIdLines: 128-byte lines of id rows prefetched for a warp's next tile.
 // ------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void prefetch_l2(const void *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+
 struct ReadsSrc {
     const uint64_t *words;
     const uint64_t *offs;
@@ -35,51 +38,33 @@ struct ReadsSrc {
     int64_t n;          // items = reads
     uint64_t nwords;    // length of `words`
     int K;
-    int both;           // 1: every window emits fwd and rc (spades-kmercount), 0: canonical form once
-    __device__ __forceinline__ uint32_t nrec(int64_t item) const {
-        int L = (int)lens[item];
-        uint32_t w = L >= K ? (uint32_t)(L - K + 1) : 0u;
-        return both ? 2u * w : w;
-    }
-    template <int NW, typename Ptr>
-    __device__ __forceinline__ Kmer<NW> get_at(Ptr s, uint32_t j) const {
-        uint32_t pos = both ? (j >> 1) : j;
-        Kmer<NW> f = kmer_window<NW>(s, (int64_t)pos, K);
-        Kmer<NW> r = kmer_rc<NW>(f, K);
-        if (both) return (j & 1) ? r : f;
-        return kmer_is_minimal<NW>(f, r) ? f : r;
-    }
-    template <int NW>
-    __device__ __forceinline__ Kmer<NW> get(int64_t item, uint32_t j) const { return get_at<NW>(words + offs[item], j); }
-    // staging of a tile's packed reads in shared memory
-    static constexpr bool kStage = true;
+    static constexpr int kIds = 24;         // a chunk's records
+    static constexpr int kIdLines = 48;     // 128 chunks: 32 reads of 150 bp at k = 55
+    static constexpr bool kSubRanges = true;  // a pass may scatter in partition sub-ranges (levelA_scatter)
     __device__ __forceinline__ uint64_t first_word(int64_t item) const { return offs[item]; }
-    __device__ __forceinline__ uint64_t end_word(int64_t item) const { return offs[item] + (((uint64_t)lens[item] + 31) >> 5); }
-    __device__ __forceinline__ uint64_t stage_word(uint64_t w) const { return words[w]; }
+    __device__ __forceinline__ uint32_t len(int64_t item) const { return lens[item]; }
+    // the lengths and offsets of the reads from `item` on, to L2
+    __device__ __forceinline__ void prefetch_items(int64_t item, int lane) const {
+        if (lane == 0) prefetch_l2(lens + item);
+        else if (lane == 1 && item + 16 < n) prefetch_l2(offs + item + 16);
+    }
 };
 
-// distinct (K+1)-mers -> their two K-mers in canonical form (DeBruijnKMerKMerSplitter with add_rc + IsMinimal filter)
-template <int NWS>
-struct KpomerSrc {
-    const uint64_t *keys;   // NWS words per record
-    int64_t n;
-    int K;                  // target K
-    __device__ __forceinline__ uint32_t nrec(int64_t) const { return 2u; }
-    static constexpr bool kStage = false;
-    __device__ __forceinline__ uint64_t first_word(int64_t) const { return 0; }
-    __device__ __forceinline__ uint64_t end_word(int64_t) const { return 0; }
-    __device__ __forceinline__ uint64_t stage_word(uint64_t) const { return 0; }
-    template <int NW, typename Ptr>
-    __device__ __forceinline__ Kmer<NW> get_at(Ptr, uint32_t) const { return Kmer<NW>(); }
-    template <int NW>
-    __device__ __forceinline__ Kmer<NW> get(int64_t item, uint32_t j) const {
-        Kmer<NWS> x;
-#pragma unroll
-        for (int q = 0; q < NWS; ++q) x.w[q] = keys[item * NWS + q];
-        Kmer<NW> f = j ? kmer_suffix<NW, NWS>(x, K) : kmer_prefix<NW, NWS>(x, K);
-        Kmer<NW> r = kmer_rc<NW>(f, K);
-        return kmer_is_minimal<NW>(f, r) ? f : r;
-    }
+// the distinct (K+1)-mers of a k-mer set chunk as reads of K+1 bases at implicit offsets: item i is key words [i * stride, ..).
+// Its two windows are the (K+1)-mer's prefix and suffix, and the canonical record of each is what DeBruijnKMerKMerSplitter
+// (add_rc + IsMinimal filter) emits. An item is one chunk of two records, so its id row is one 16-byte word.
+struct KmerSetSrc {
+    const uint64_t *words;
+    int64_t n;          // items = (K+1)-mers
+    uint64_t nwords;    // n * stride
+    int K;              // target K
+    uint32_t stride;    // words per key
+    static constexpr int kIds = 8;
+    static constexpr int kIdLines = 4;      // 32 chunks
+    static constexpr bool kSubRanges = false;
+    __device__ __forceinline__ uint64_t first_word(int64_t item) const { return (uint64_t)item * stride; }
+    __device__ __forceinline__ uint32_t len(int64_t) const { return (uint32_t)K + 1; }
+    __device__ __forceinline__ void prefetch_items(int64_t, int) const {}
 };
 
 template <int NW>
@@ -121,89 +106,6 @@ struct LevelA {
     uint32_t PA;            // (b_hi-b_lo) << rA
 };
 
-static const int kATile = 256;        // items (reads) per tile
-static const int kAThreads = 1024;
-
-// tile prologue: per-item record counts -> exclusive prefix in shared memory; returns the tile total
-template <class Src>
-__device__ __forceinline__ uint32_t tile_prefix(const Src &src, int64_t item0, int nitems, uint32_t *pref /*kATile+1*/, uint32_t *uniform = nullptr) {
-    // kAThreads >= kATile: thread t owns item t
-    uint32_t c = 0;
-    if ((int)threadIdx.x < nitems) c = src.nrec(item0 + threadIdx.x);
-    // block scan over the first kATile threads (8 warps)
-    __shared__ uint32_t wsum[kATile / 32 + 1];
-    __shared__ uint32_t s_c0;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) s_c0 = c;
-    uint32_t inc = c;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += t;
-    }
-    if (warp < kATile / 32 && lane == 31) wsum[warp] = inc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        uint32_t run = 0;
-        for (int w = 0; w < kATile / 32; ++w) { uint32_t t = wsum[w]; wsum[w] = run; run += t; }
-        wsum[kATile / 32] = run;
-    }
-    // every item yields the same number of records (fixed-length reads): item = i / c0 instead of a binary search
-    const uint32_t c0 = s_c0;
-    const int same = __syncthreads_and((int)threadIdx.x >= nitems || c == c0);
-    if ((int)threadIdx.x < kATile) pref[threadIdx.x] = wsum[warp] + inc - c;
-    uint32_t total = wsum[kATile / 32];
-    if (threadIdx.x == 0) pref[kATile] = total;
-    __syncthreads();
-    if (uniform) *uniform = (same && c0) ? c0 : 0u;
-    return total;
-}
-
-__device__ __forceinline__ int find_item_u(const uint32_t *pref, int nitems, uint32_t i, uint32_t uniform);
-__device__ __forceinline__ int find_item(const uint32_t *pref, int nitems, uint32_t i) {
-    // largest t with pref[t] <= i   (pref is exclusive, nitems <= kATile)
-    int lo = 0, hi = nitems - 1;
-    while (lo < hi) {
-        int mid = (lo + hi + 1) >> 1;
-        if (pref[mid] <= i) lo = mid; else hi = mid - 1;
-    }
-    return lo;
-}
-
-// Stage a tile's packed reads in shared memory (the partition kernel's own store traffic evicts the read words from L1, and
-// waiting on their global loads becomes its top stall). The reads of a tile are one contiguous word range
-// in every layout this library produces; anything else (or very long reads) falls back to global loads.
-static const int kStageWords = 2560;      // 20 KB: 256 reads x 10 words (<= 320 bp each)
-struct TileStage {
-    uint64_t words[kStageWords];
-    uint32_t off[kATile];
-};
-template <class Src>
-__device__ __forceinline__ bool tile_stage(const Src &src, int64_t item0, int nitems, TileStage &ts) {
-    if (!Src::kStage) return false;
-    __shared__ unsigned s_maxend;
-    const uint64_t w0 = src.first_word(item0);
-    if (threadIdx.x == 0) s_maxend = 0;
-    __syncthreads();
-    bool ok = true;
-    if ((int)threadIdx.x < nitems) {
-        const uint64_t a = src.first_word(item0 + threadIdx.x), b = src.end_word(item0 + threadIdx.x);
-        ok = a >= w0 && b >= a && b - w0 <= (uint64_t)kStageWords;
-        if (ok) { ts.off[threadIdx.x] = (uint32_t)(a - w0); atomicMax(&s_maxend, (unsigned)(b - w0)); }
-    }
-    const bool staged = __syncthreads_and(ok) != 0;
-    if (staged) {
-        const uint32_t nwords = s_maxend;
-        for (uint32_t i = threadIdx.x; i < nwords; i += blockDim.x) ts.words[i] = src.stage_word(w0 + i);
-    }
-    __syncthreads();
-    return staged;
-}
-template <int NW, class Src>
-__device__ __forceinline__ Kmer<NW> tile_get(const Src &src, bool staged, const TileStage &ts, int64_t item0, int it, uint32_t j) {
-    if (Src::kStage && staged) return src.template get_at<NW>(ts.words + ts.off[it], j);
-    return src.template get<NW>(item0 + it, j);
-}
 // record stores bypass L1 allocation (they are never re-read by this kernel)
 template <int NW>
 __device__ __forceinline__ void store_rec_stream(uint64_t *dst, const Kmer<NW> &k) {
@@ -218,8 +120,15 @@ __device__ __forceinline__ void store_rec_stream(uint64_t *dst, const Kmer<NW> &
     }
 }
 
+// the item of unit i: i / uniform when every item has `uniform` units, else the largest t with pref[t] <= i (pref is exclusive)
 __device__ __forceinline__ int find_item_u(const uint32_t *pref, int nitems, uint32_t i, uint32_t uniform) {
-    return uniform ? (int)(i / uniform) : find_item(pref, nitems, i);
+    if (uniform) return (int)(i / uniform);
+    int lo = 0, hi = nitems - 1;
+    while (lo < hi) {
+        int mid = (lo + hi + 1) >> 1;
+        if (pref[mid] <= i) lo = mid; else hi = mid - 1;
+    }
+    return lo;
 }
 
 template <int NW>
@@ -228,54 +137,6 @@ __device__ __forceinline__ bool part_of(const LevelA &p, const Kmer<NW> &k, uint
     if (b < p.b_lo || b >= p.b_hi) return false;
     *part = ((b - p.b_lo) << p.rA) | key_top_bits<NW>(k, p.K, p.rA);
     return true;
-}
-
-// records per tile (kATile items), for the per-record partition-id array
-template <class Src>
-__global__ void tile_totals_k(Src src, int64_t ntiles, uint32_t *__restrict__ out, uint32_t pad) {
-    const int64_t t = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if (t >= ntiles) return;
-    const int lane = threadIdx.x & 31;
-    const int64_t item0 = t * kATile;
-    uint32_t s = 0;
-    for (int i = lane; i < kATile && item0 + i < src.n; i += 32) s += src.nrec(item0 + i);
-    for (int o = 16; o; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
-    if (lane == 0) out[t] = (s + pad - 1) / pad * pad;       // rows of the id array start 2*pad-byte aligned
-}
-
-// items are split statically: CTA g owns tiles [g*tiles_per, ...) so that count and scatter agree
-template <int NW, class Src>
-__global__ void __launch_bounds__(kAThreads) levelA_count_k(Src src, LevelA p, uint32_t *__restrict__ blk_counts,
-                                                            const uint64_t *__restrict__ tile_off, uint16_t *__restrict__ ids) {
-    extern __shared__ uint32_t sm_dyn[];
-    uint32_t *hist = sm_dyn;                  // PA
-    __shared__ uint32_t pref[kATile + 1];
-    __shared__ TileStage ts;
-    for (uint32_t i = threadIdx.x; i < p.PA; i += blockDim.x) hist[i] = 0;
-    __syncthreads();
-    const int64_t ntiles = (src.n + kATile - 1) / kATile;
-    const int64_t per = (ntiles + gridDim.x - 1) / gridDim.x;
-    const int64_t t0 = (int64_t)blockIdx.x * per, t1 = min(ntiles, t0 + per);
-    for (int64_t t = t0; t < t1; ++t) {
-        const int64_t item0 = t * kATile;
-        const int nitems = (int)min((int64_t)kATile, src.n - item0);
-        uint32_t unif = 0;
-        const uint32_t total = tile_prefix(src, item0, nitems, pref, &unif);
-        const bool staged = tile_stage(src, item0, nitems, ts);
-        const uint64_t toff = ids ? tile_off[t] : 0;
-        for (uint32_t i = threadIdx.x; i < total; i += blockDim.x) {
-            int it = find_item_u(pref, nitems, i, unif);
-            Kmer<NW> k = tile_get<NW>(src, staged, ts, item0, it, i - pref[it]);
-            uint32_t part = 0xffffu;
-            if (part_of<NW>(p, k, &part)) atomicAdd(&hist[part], 1u); else part = 0xffffu;
-            // remember the partition of every record: the scatter passes (one per bucket group) then neither hash nor
-            // even extract the records that are not theirs
-            if (ids) ids[toff + i] = (uint16_t)part;
-        }
-        __syncthreads();
-    }
-    uint32_t *out = blk_counts + (size_t)blockIdx.x * p.PA;
-    for (uint32_t i = threadIdx.x; i < p.PA; i += blockDim.x) out[i] += hist[i];
 }
 
 // one thread per partition: totals and per-CTA bases. base[g][part] is the running cursor of CTA g.
@@ -297,89 +158,34 @@ __global__ void levelA_bases_k(const uint32_t *__restrict__ blk_counts, uint32_t
     }
 }
 
-template <int NW, class Src>
-__global__ void __launch_bounds__(kAThreads) levelA_scatter_k(Src src, LevelA p, uint64_t *__restrict__ base, uint64_t *__restrict__ out,
-                                                              const uint64_t *__restrict__ tile_off, const uint16_t *__restrict__ ids, uint32_t id_lo) {
-    extern __shared__ uint32_t sm_dyn[];
-    uint64_t *cur_base = reinterpret_cast<uint64_t *>(sm_dyn);          // PA u64
-    uint32_t *cnt = reinterpret_cast<uint32_t *>(cur_base + p.PA);      // PA u32
-    __shared__ uint32_t pref[kATile + 1];
-    __shared__ TileStage ts;
-    uint64_t *mybase = base + (size_t)blockIdx.x * p.PA;
-    for (uint32_t i = threadIdx.x; i < p.PA; i += blockDim.x) { cur_base[i] = mybase[i]; cnt[i] = 0; }
-    __syncthreads();
-    const int64_t ntiles = (src.n + kATile - 1) / kATile;
-    const int64_t per = (ntiles + gridDim.x - 1) / gridDim.x;
-    const int64_t t0 = (int64_t)blockIdx.x * per, t1 = min(ntiles, t0 + per);
-    for (int64_t t = t0; t < t1; ++t) {
-        const int64_t item0 = t * kATile;
-        const int nitems = (int)min((int64_t)kATile, src.n - item0);
-        uint32_t unif = 0;
-        const uint32_t total = tile_prefix(src, item0, nitems, pref, &unif);
-        const bool staged = tile_stage(src, item0, nitems, ts);
-        if (ids) {
-            // the consumer of the per-record 2-byte id load and the binary search are this kernel's main stalls: issue four id
-            // loads before touching any of them, divide instead of searching
-            const uint16_t *row = ids + tile_off[t];
-            constexpr int U = 4;
-            for (uint32_t i0 = threadIdx.x; i0 < total; i0 += U * blockDim.x) {
-                uint32_t part[U];
-#pragma unroll
-                for (int u = 0; u < U; ++u) {
-                    const uint32_t i = i0 + u * blockDim.x;
-                    part[u] = i < total ? (uint32_t)__ldg(row + i) - id_lo : 0xffffffffu;      // 0xffff - id_lo stays >= PA
-                }
-#pragma unroll
-                for (int u = 0; u < U; ++u) {
-                    if (part[u] >= p.PA) continue;
-                    const uint32_t i = i0 + u * blockDim.x;
-                    const int it = find_item_u(pref, nitems, i, unif);
-                    Kmer<NW> k = tile_get<NW>(src, staged, ts, item0, it, i - pref[it]);
-                    uint32_t slot = atomicAdd(&cnt[part[u]], 1u);
-                    store_rec_stream<NW>(out + (cur_base[part[u]] + slot) * NW, k);
-                }
-            }
-        } else {
-            for (uint32_t i = threadIdx.x; i < total; i += blockDim.x) {
-                uint32_t part;
-                int it = find_item_u(pref, nitems, i, unif);
-                Kmer<NW> k = tile_get<NW>(src, staged, ts, item0, it, i - pref[it]);
-                if (part_of<NW>(p, k, &part)) {
-                    uint32_t slot = atomicAdd(&cnt[part], 1u);
-                    store_rec_stream<NW>(out + (cur_base[part] + slot) * NW, k);
-                }
-            }
-        }
-        __syncthreads();
-    }
-    for (uint32_t i = threadIdx.x; i < p.PA; i += blockDim.x) mybase[i] = cur_base[i] + cnt[i];   // chained launches continue here
-}
-
-// ---- level A, rolling generation ------------------------------------------------------------------------------------
-// The kernels above spend a few hundred thread instructions per window -- every record re-extracted its window from up to three packed words, re-ran FastRC, divided to
-// find its read and (scatter) waited for a 2-byte id load. Here the unit of work is a CHUNK of kRollC consecutive windows of
-// one read, walked by one thread with a rolling window + rolling reverse complement (kmer_dev.cuh roll_*): one shared-memory
-// word load per 32 bases, ~20 integer instructions per window, and in a bucket-group pass the windows of other groups cost
-// only the roll. The 2-byte partition ids of a chunk are 48 contiguous bytes: written as six 8-byte words by the count pass,
-// fetched as three 16-byte loads before the walk starts by every scatter pass. Reads only (canonical mode).
-static const int kRollC = 24;            // windows per chunk
+// ---- level A: rolling kernels ------------------------------------------------------------------------------------------
+// The unit of work is a CHUNK of consecutive windows of one item, walked by one thread with a rolling window + rolling reverse
+// complement (kmer_dev.cuh roll_*): one shared-memory word load per 32 bases, ~20 integer instructions per window, and in a
+// bucket-group pass the windows of other groups cost only the roll. A chunk holds kRollC records: kRollC windows in canonical
+// mode (one record per window, the canonical one of its two strands), kRollC / 2 windows in all-windows mode (BOTH: record s
+// is window s / 2 and strand s & 1, the roll advances every second record). The 2-byte partition ids of a chunk's records are
+// one row of Src::kIds ids: written as 8-byte words by the count pass, fetched as 16-byte loads before the walk starts by every
+// scatter pass. (Re-extracting every window from the packed words, the kernels of the first generation, cost a few hundred
+// thread instructions per window. Removed.)
+static const int kRollC = 24;            // records per chunk
+template <bool BOTH> constexpr int kRollWin = BOTH ? kRollC / 2 : kRollC;      // windows per chunk
 static_assert(kRollC <= 33 && kRollC % 8 == 0, "roll_init fetches a chunk's bases from two words; an id row is a whole number of 16-byte words");
+static_assert(ReadsSrc::kIds == kRollC && KmerSetSrc::kIds % 8 == 0, "an id row holds a chunk's records");
 static const int kRollThreads = 512;     // 2-3 CTAs per SM; units of a tile are dealt round-robin to the threads
 
-// Round 2: the tile of the rolling kernels is a WARP's: 32 consecutive reads, staged, scanned and walked by one warp with
+// The tile of the rolling kernels is a WARP's: 32 consecutive items, staged, scanned and walked by one warp with
 // shuffles and __syncwarp only. (The CTA-wide tiles of the first version cost five __syncthreads per 256 reads, and barrier
 // and global-load stalls dominated the partition kernel.) A CTA
 // still owns a contiguous range of tiles -- the same range in the count and in every scatter launch, which is what makes the
 // per-CTA histogram of the count the cursor table of the scatter -- and deals them round-robin to its warps.
-static const int kRollTile = 32;                      // reads per warp tile
+static const int kRollTile = 32;                      // items per warp tile
 static const int kRollWarps = kRollThreads / 32;
 static const int kRollStageWords = 320;               // per warp: 32 reads x 10 words (<= 320 bp each), else global loads
-__device__ __forceinline__ void prefetch_l2(const void *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 struct RollWarp {
-    uint64_t words[kRollStageWords];     // the tile's packed reads
-    uint32_t pref[kRollTile + 1];        // exclusive prefix of chunks per read
-    uint32_t len[kRollTile];             // read lengths
-    uint32_t off[kRollTile];             // first staged word of a read
+    uint64_t words[kRollStageWords];     // the tile's packed items
+    uint32_t pref[kRollTile + 1];        // exclusive prefix of chunks per item
+    uint32_t len[kRollTile];             // item lengths
+    uint32_t off[kRollTile];             // first staged word of an item
     uint32_t pad_;
 };
 static_assert(sizeof(RollWarp) % 8 == 0, "per-warp slices stay 8-byte aligned");
@@ -388,18 +194,19 @@ __device__ __forceinline__ RollWarp *roll_warp_slice(unsigned char *raw, uint32_
     return reinterpret_cast<RollWarp *>(raw + (((size_t)nslots * 4 + 15) & ~(size_t)15)) + (threadIdx.x >> 5);
 }
 
-// one warp: chunk counts of the tile's reads -> exclusive prefix, the reads' words -> shared memory. Returns the tile's chunk
-// total; *uniform = chunks per read when every read has the same (non-zero) count, else 0; *staged = words are in rw.words.
-__device__ __forceinline__ uint32_t roll_warp_setup(const ReadsSrc &src, int64_t item0, int nitems, RollWarp &rw, uint32_t *uniform, bool *staged) {
+// one warp: chunk counts of the tile's items -> exclusive prefix, the items' words -> shared memory. Returns the tile's chunk
+// total; *uniform = chunks per item when every item has the same (non-zero) count, else 0; *staged = words are in rw.words.
+template <bool BOTH, class Src>
+__device__ __forceinline__ uint32_t roll_warp_setup(const Src &src, int64_t item0, int nitems, RollWarp &rw, uint32_t *uniform, bool *staged) {
     const int lane = threadIdx.x & 31;
     uint32_t c = 0, L = 0;
     uint64_t a = 0, b = 0;
     if (lane < nitems) {
-        L = src.lens[item0 + lane];
-        a = src.offs[item0 + lane];
+        L = src.len(item0 + lane);
+        a = src.first_word(item0 + lane);
         b = a + (((uint64_t)L + 31) >> 5);
         const uint32_t w = (int)L >= src.K ? (uint32_t)((int)L - src.K + 1) : 0u;
-        c = (w + kRollC - 1) / kRollC;
+        c = (w + kRollWin<BOTH> - 1) / kRollWin<BOTH>;
     }
     uint32_t inc = c;
 #pragma unroll
@@ -434,35 +241,38 @@ __device__ __forceinline__ uint32_t roll_warp_setup(const ReadsSrc &src, int64_t
     return total;
 }
 
-// chunks per warp tile x kRollC = ids per tile (rows of the id array: 48 bytes per chunk, so every row is 16-byte aligned)
-__global__ void roll_tile_ids_k(ReadsSrc src, int64_t ntiles, uint32_t *__restrict__ out) {
+// chunks per warp tile x Src::kIds = ids per tile (rows of the id array: a whole number of 16-byte words per chunk)
+template <bool BOTH, class Src>
+__global__ void roll_tile_ids_k(Src src, int64_t ntiles, uint32_t *__restrict__ out) {
     const int64_t t = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (t >= ntiles) return;
     const int lane = threadIdx.x & 31;
     const int64_t item = t * kRollTile + lane;
     uint32_t s = 0;
     if (item < src.n) {
-        const int L = (int)src.lens[item];
+        const int L = (int)src.len(item);
         const uint32_t w = L >= src.K ? (uint32_t)(L - src.K + 1) : 0u;
-        s = (w + kRollC - 1) / kRollC;
+        s = (w + kRollWin<BOTH> - 1) / kRollWin<BOTH>;
     }
     for (int o = 16; o; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
-    if (lane == 0) out[t] = s * kRollC;
+    if (lane == 0) out[t] = s * Src::kIds;
 }
 
-// geometry of one unit (chunk): which read, which windows
+// geometry of one unit (chunk): which item, which windows (first, count)
 struct RollUnit { int it, j0, cnt; };
+template <bool BOTH>
 __device__ __forceinline__ RollUnit roll_unit(const RollWarp &rw, int nitems, uint32_t u, uint32_t unif, int K) {
+    constexpr int C = kRollWin<BOTH>;
     RollUnit q;
     q.it = find_item_u(rw.pref, nitems, u, unif);
-    q.j0 = (int)(u - rw.pref[q.it]) * kRollC;
+    q.j0 = (int)(u - rw.pref[q.it]) * C;
     const int nwin = (int)rw.len[q.it] - K + 1;
-    q.cnt = nwin - q.j0 < kRollC ? nwin - q.j0 : kRollC;
+    q.cnt = nwin - q.j0 < C ? nwin - q.j0 : C;
     return q;
 }
 
-template <int NW>
-__global__ void __launch_bounds__(kRollThreads, 2) levelA_count_roll_k(ReadsSrc src, LevelA p, uint32_t *__restrict__ blk_counts,
+template <int NW, class Src, bool BOTH>
+__global__ void __launch_bounds__(kRollThreads, 2) levelA_count_roll_k(Src src, LevelA p, uint32_t *__restrict__ blk_counts,
                                                                       const uint64_t *__restrict__ tile_off, uint16_t *__restrict__ ids) {
     extern __shared__ __align__(16) unsigned char sm_raw[];
     uint32_t *hist = reinterpret_cast<uint32_t *>(sm_raw);     // PA
@@ -479,39 +289,39 @@ __global__ void __launch_bounds__(kRollThreads, 2) levelA_count_roll_k(ReadsSrc 
         const int nitems = (int)min((int64_t)kRollTile, src.n - item0);
         uint32_t unif = 0;
         bool staged = false;
-        // the warp's next tile is kRollWarps tiles ahead: its lengths and offsets go to L2 now, its packed reads (and id rows) at the
+        // the warp's next tile is kRollWarps tiles ahead: its item metadata goes to L2 now, its packed items (and id rows) at the
         // end of this tile, when the loads of their addresses issued here have long returned
         const bool has_next = t + kRollWarps < t1;
         const int64_t nx = (t + kRollWarps) * kRollTile;
         uint64_t next_w0 = 0;
         if (has_next) {
-            next_w0 = src.offs[nx];
-            if (lane == 0) prefetch_l2(src.lens + nx);
-            else if (lane == 1 && nx + 16 < src.n) prefetch_l2(src.offs + nx + 16);
+            next_w0 = src.first_word(nx);
+            src.prefetch_items(nx, lane);
         }
-        const uint32_t nunits = roll_warp_setup(src, item0, nitems, rw, &unif, &staged);
+        const uint32_t nunits = roll_warp_setup<BOTH>(src, item0, nitems, rw, &unif, &staged);
         uint64_t *row = ids ? reinterpret_cast<uint64_t *>(ids + tile_off[t]) : nullptr;
         for (uint32_t u = lane; u < nunits; u += 32) {
-            const RollUnit q = roll_unit(rw, nitems, u, unif, K);
-            const uint64_t *seq = staged ? static_cast<const uint64_t *>(rw.words + rw.off[q.it]) : src.words + src.offs[item0 + q.it];
+            const RollUnit q = roll_unit<BOTH>(rw, nitems, u, unif, K);
+            const uint64_t *seq = staged ? static_cast<const uint64_t *>(rw.words + rw.off[q.it]) : src.words + src.first_word(item0 + q.it);
             RollState<NW> st;
             roll_init<NW>(st, seq, q.j0, K, q.cnt);
+            const int nrec = BOTH ? 2 * q.cnt : q.cnt;
 #pragma unroll 1
-            for (int g = 0; g < kRollC / 4; ++g) {
+            for (int g = 0; g < Src::kIds / 4; ++g) {
                 uint64_t acc = 0;
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                     const int s = 4 * g + e;
                     uint32_t id = 0xffffu;
-                    if (s < q.cnt) {
-                        if (s > 0) roll_next<NW>(st, K);
-                        const Kmer<NW> k = kmer_is_minimal<NW>(st.f, st.r) ? st.f : st.r;
+                    if (s < nrec) {
+                        if (s > 0 && !(BOTH && (e & 1))) roll_next<NW>(st, K);
+                        const Kmer<NW> k = BOTH ? ((e & 1) ? st.r : st.f) : kmer_is_minimal<NW>(st.f, st.r) ? st.f : st.r;
                         uint32_t part;
                         if (part_of<NW>(p, k, &part)) { atomicAdd(&hist[part], 1u); id = part; }
                     }
                     acc |= (uint64_t)id << (16 * e);
                 }
-                if (row) row[(size_t)u * (kRollC / 4) + g] = acc;
+                if (row) row[(size_t)u * (Src::kIds / 4) + g] = acc;
             }
         }
         if (has_next && lane < 10 && next_w0 + 16 * lane < src.nwords) prefetch_l2(src.words + next_w0 + 16 * lane);   // 10 lines = 32 reads x 5 words
@@ -555,8 +365,8 @@ __host__ __device__ __forceinline__ size_t abatch_offset(uint32_t PA) {
     return ((((size_t)2 * PA * 4 + 15) & ~(size_t)15) + (size_t)kRollWarps * sizeof(RollWarp) + 15) & ~(size_t)15;
 }
 
-template <int NW, bool HAS_IDS>
-__global__ void __launch_bounds__(kRollThreads, 2) levelA_scatter_roll_k(ReadsSrc src, LevelA p, uint64_t *__restrict__ base, uint64_t *__restrict__ out,
+template <int NW, class Src, bool BOTH, bool HAS_IDS>
+__global__ void __launch_bounds__(kRollThreads, 2) levelA_scatter_roll_k(Src src, LevelA p, uint64_t *__restrict__ base, uint64_t *__restrict__ out,
                                                                         const uint64_t *__restrict__ tile_off, const uint16_t *__restrict__ ids,
                                                                         uint32_t id_lo, uint32_t row_stride, uint32_t q_lo, uint64_t ids_len, uint32_t cap) {
     extern __shared__ __align__(16) unsigned char sm_raw[];
@@ -592,24 +402,23 @@ __global__ void __launch_bounds__(kRollThreads, 2) levelA_scatter_roll_k(ReadsSr
     bool staged = false;
     uint64_t next_w0 = 0, next_row = 0;
     const ulonglong2 *row = nullptr;
-    int u = 0, s = 0, cnt_w = 0;                  // the lane's chunk, its window (st is at it), its windows
+    int u = 0, s = 0, cnt_w = 0;                  // the lane's chunk, its record (st is at its window), its records
     RollState<NW> st;
-    uint64_t idq[kRollC / 4];                     // HAS_IDS: the chunk's ids from window s on, two bytes each
+    uint64_t idq[Src::kIds / 4];                  // HAS_IDS: the chunk's ids from record s on, two bytes each
     for (;;) {
         while (t < t1) {                          // warp-uniform
             if (need_setup) {
                 const int64_t item0 = t * kRollTile;
                 nitems = (int)min((int64_t)kRollTile, src.n - item0);
-                // the warp's next tile is kRollWarps tiles ahead: its lengths and offsets go to L2 now, its packed reads (and id
+                // the warp's next tile is kRollWarps tiles ahead: its item metadata goes to L2 now, its packed items (and id
                 // rows) at the end of this tile, when the loads of their addresses issued here have long returned
                 const int64_t nx = (t + kRollWarps) * kRollTile;
                 if (t + kRollWarps < t1) {
-                    next_w0 = src.offs[nx];
-                    if (lane == 0) prefetch_l2(src.lens + nx);
-                    else if (lane == 1 && nx + 16 < src.n) prefetch_l2(src.offs + nx + 16);
+                    next_w0 = src.first_word(nx);
+                    src.prefetch_items(nx, lane);
                     if (HAS_IDS) next_row = tile_off[t + kRollWarps];
                 }
-                nunits = roll_warp_setup(src, item0, nitems, rw, &unif, &staged);
+                nunits = roll_warp_setup<BOTH>(src, item0, nitems, rw, &unif, &staged);
                 if (HAS_IDS) row = reinterpret_cast<const ulonglong2 *>(ids + tile_off[t]);
                 u = lane - 32; s = cnt_w = 0;
                 need_setup = false;
@@ -619,24 +428,24 @@ __global__ void __launch_bounds__(kRollThreads, 2) levelA_scatter_roll_k(ReadsSr
                 if (u < (int)nunits) {
                     if (HAS_IDS) {
 #pragma unroll
-                        for (int v = 0; v < kRollC / 8; ++v) {
-                            const ulonglong2 x = __ldg(row + (size_t)u * (kRollC / 8) + v);
+                        for (int v = 0; v < Src::kIds / 8; ++v) {
+                            const ulonglong2 x = __ldg(row + (size_t)u * (Src::kIds / 8) + v);
                             idq[2 * v] = x.x; idq[2 * v + 1] = x.y;
                         }
                     }
-                    const RollUnit q = roll_unit(rw, nitems, (uint32_t)u, unif, K);
-                    const uint64_t *seq = staged ? static_cast<const uint64_t *>(rw.words + rw.off[q.it]) : src.words + src.offs[t * kRollTile + q.it];
+                    const RollUnit q = roll_unit<BOTH>(rw, nitems, (uint32_t)u, unif, K);
+                    const uint64_t *seq = staged ? static_cast<const uint64_t *>(rw.words + rw.off[q.it]) : src.words + src.first_word(t * kRollTile + q.it);
                     roll_init<NW>(st, seq, q.j0, K, q.cnt);
-                    s = 0; cnt_w = q.cnt;
+                    s = 0; cnt_w = BOTH ? 2 * q.cnt : q.cnt;
                 }
             }
             const bool act = s < cnt_w;
             if (!__any_sync(0xffffffffu, act)) {  // the tile is done
                 if (t + kRollWarps < t1) {
                     if (lane < 10 && next_w0 + 16 * lane < src.nwords) prefetch_l2(src.words + next_w0 + 16 * lane);   // 10 lines = 32 reads x 5 words
-                    if (HAS_IDS) {                                                                                      // 48 lines for 128 chunks
-                        if (next_row + 64 * lane < ids_len) prefetch_l2(ids + next_row + 64 * lane);
-                        if (lane < 16 && next_row + 64 * (32 + lane) < ids_len) prefetch_l2(ids + next_row + 64 * (32 + lane));
+                    if (HAS_IDS) {                                                                                      // Src::kIdLines <= 64 lines
+                        if ((Src::kIdLines >= 32 || lane < Src::kIdLines) && next_row + 64 * lane < ids_len) prefetch_l2(ids + next_row + 64 * lane);
+                        if (lane < Src::kIdLines - 32 && next_row + 64 * (32 + lane) < ids_len) prefetch_l2(ids + next_row + 64 * (32 + lane));
                     }
                 }
                 __syncwarp();                     // the slice is rewritten by the next tile's setup
@@ -656,7 +465,7 @@ __global__ void __launch_bounds__(kRollThreads, 2) levelA_scatter_roll_k(ReadsSr
                     mine = part < PA;
                 }
                 if (!HAS_IDS || mine) {
-                    const bool fwd = kmer_is_minimal<NW>(st.f, st.r);
+                    const bool fwd = BOTH ? !(s & 1) : kmer_is_minimal<NW>(st.f, st.r);
 #pragma unroll
                     for (int j = 0; j < NW; ++j) k.w[j] = fwd ? st.f.w[j] : st.r.w[j];
                 }
@@ -680,11 +489,11 @@ __global__ void __launch_bounds__(kRollThreads, 2) levelA_scatter_roll_k(ReadsSr
                 }
             }
             if (act && ++s < cnt_w) {
-                roll_next<NW>(st, K);
+                if (!BOTH || !(s & 1)) roll_next<NW>(st, K);
                 if (HAS_IDS) {
                     if ((s & 3) == 0) {
 #pragma unroll
-                        for (int v = 0; v + 1 < kRollC / 4; ++v) idq[v] = idq[v + 1];
+                        for (int v = 0; v + 1 < Src::kIds / 4; ++v) idq[v] = idq[v + 1];
                     } else {
                         idq[0] >>= 16;
                     }
@@ -1589,14 +1398,14 @@ static void sort_pass(Ctx *ctx, int K, DArr<uint64_t> &X, DArr<uint64_t> &Y, con
 
 // ---- level A as a job: one histogram (+ partition id) pass over the source, then one scatter per bucket-group pass -----------
 // Shared by the single-GPU count and the multi-GPU count (where a "pass" scatters this rank's shard for the pass's buckets).
-template <int NW, class Src>
+template <int NW, class Src, bool BOTH>
 struct LevelAJob {
     Ctx *ctx = nullptr;
     std::vector<Src> srcs;
     int K = 0, B = 0, rA = 0, G = 0;
     int s_lo = 0, s_hi = 0;               // buckets covered by this job (one histogram super-range)
     uint32_t PA_all = 0;                  // (s_hi - s_lo) << rA
-    bool roll = false, use_ids = false;
+    bool use_ids = false;
     DArr<uint32_t> blk_counts;            // [G][PA_all] records of (CTA, partition)
     DArr<uint64_t> part_total_all;        // [PA_all]
     std::vector<DArr<uint64_t>> tile_off; // per source: first id of every tile
@@ -1643,8 +1452,8 @@ static int levelA_key_bits(uint64_t est_records, int B, int total_bits, uint32_t
     return rA;
 }
 
-template <int NW, class Src>
-static void levelA_count(LevelAJob<NW, Src> &job, uint64_t est_records, Timer &tm, Trace &tr) {
+template <int NW, class Src, bool BOTH>
+static void levelA_count(LevelAJob<NW, Src, BOTH> &job, Timer &tm, Trace &tr) {
     Ctx *ctx = job.ctx;
     cudaStream_t st = ctx->stream;
     const uint32_t PA_all = job.PA_all;
@@ -1658,42 +1467,36 @@ static void levelA_count(LevelAJob<NW, Src> &job, uint64_t est_records, Timer &t
     SG_CUDA(cudaMemsetAsync(job.blk_counts.p, 0, job.blk_counts.bytes(), st));
     job.tile_off.clear(); job.ids.clear();
     job.tile_off.resize(job.srcs.size()); job.ids.resize(job.srcs.size());
-    // per-record partition ids (2 bytes per record slot): only when they fit comfortably next to the sort buffers
-    job.use_ids = PA_all < 0xffffu && (double)est_records * 2.0 < (double)ctx->free_bytes() * 0.20;
-    if (job.use_ids) {
-        for (size_t si = 0; si < job.srcs.size(); ++si) {
-            const Src &src = job.srcs[si];
-            if (src.n == 0) continue;
-            const int64_t ntiles = (src.n + (job.roll ? kRollTile : kATile) - 1) / (job.roll ? kRollTile : kATile);
-            DArr<uint32_t> ttot(ctx, (size_t)ntiles + 1);
-            job.tile_off[si].alloc(ctx, (size_t)ntiles + 1);
-            SG_CUDA(cudaMemsetAsync(ttot.p + ntiles, 0, 4, st));
-            if (job.roll) {
-                if constexpr (std::is_same<Src, ReadsSrc>::value) roll_tile_ids_k<<<div_up(ntiles, 8), 256, 0, st>>>(src, ntiles, ttot.p);
-            } else {
-                tile_totals_k<Src><<<div_up(ntiles, 8), 256, 0, st>>>(src, ntiles, ttot.p, 8u);
-            }
-            ctx->launches++;
-            exclusive_scan_u32_to_u64(ctx, ttot.p, job.tile_off[si].p, (size_t)ntiles + 1);
-            uint64_t nrec_src = 0;
-            SG_CUDA(cudaMemcpyAsync(&nrec_src, job.tile_off[si].p + ntiles, 8, cudaMemcpyDeviceToHost, st));
-            SG_CUDA(cudaStreamSynchronize(st));
-            job.ids[si].alloc(ctx, (size_t)nrec_src + 8);
-        }
-    }
-    tm.start();
+    // per-record partition ids (2 bytes per id slot, Src::kIds slots per chunk): only when they fit comfortably next to the
+    // sort buffers. The id rows of the tiles are laid out first; their total is the id array's size.
+    const double free0 = (double)ctx->free_bytes();
+    std::vector<uint64_t> nslots(job.srcs.size(), 0);
+    uint64_t all_slots = 0;
     for (size_t si = 0; si < job.srcs.size(); ++si) {
         const Src &src = job.srcs[si];
         if (src.n == 0) continue;
-        if (job.roll) {
-            if constexpr (std::is_same<Src, ReadsSrc>::value) {
-                SG_CUDA(cudaFuncSetAttribute(levelA_count_roll_k<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)roll_smem_bytes(PA_all)));
-                levelA_count_roll_k<NW><<<G, kRollThreads, roll_smem_bytes(PA_all), st>>>(src, pa_all, job.blk_counts.p, job.tile_off[si].p, job.ids[si].p);
-            }
-        } else {
-            SG_CUDA(cudaFuncSetAttribute(levelA_count_k<NW, Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(PA_all * sizeof(uint32_t))));
-            levelA_count_k<NW, Src><<<G, kAThreads, PA_all * sizeof(uint32_t), st>>>(src, pa_all, job.blk_counts.p, job.tile_off[si].p, job.ids[si].p);
-        }
+        const int64_t ntiles = (src.n + kRollTile - 1) / kRollTile;
+        DArr<uint32_t> ttot(ctx, (size_t)ntiles + 1);
+        job.tile_off[si].alloc(ctx, (size_t)ntiles + 1);
+        SG_CUDA(cudaMemsetAsync(ttot.p + ntiles, 0, 4, st));
+        roll_tile_ids_k<BOTH><<<div_up(ntiles, 8), 256, 0, st>>>(src, ntiles, ttot.p);
+        ctx->launches++;
+        exclusive_scan_u32_to_u64(ctx, ttot.p, job.tile_off[si].p, (size_t)ntiles + 1);
+        SG_CUDA(cudaMemcpyAsync(&nslots[si], job.tile_off[si].p + ntiles, 8, cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaStreamSynchronize(st));
+        all_slots += nslots[si];
+    }
+    job.use_ids = PA_all < 0xffffu && (double)all_slots * 2.0 < free0 * 0.20;
+    for (size_t si = 0; si < job.srcs.size(); ++si) {
+        if (!job.use_ids) job.tile_off[si] = DArr<uint64_t>();
+        else if (job.srcs[si].n) job.ids[si].alloc(ctx, (size_t)nslots[si] + 8);
+    }
+    tm.start();
+    SG_CUDA(cudaFuncSetAttribute(levelA_count_roll_k<NW, Src, BOTH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)roll_smem_bytes(PA_all)));
+    for (size_t si = 0; si < job.srcs.size(); ++si) {
+        const Src &src = job.srcs[si];
+        if (src.n == 0) continue;
+        levelA_count_roll_k<NW, Src, BOTH><<<G, kRollThreads, roll_smem_bytes(PA_all), st>>>(src, pa_all, job.blk_counts.p, job.tile_off[si].p, job.ids[si].p);
         ctx->launches++;
     }
     SG_CUDA(cudaGetLastError());
@@ -1708,8 +1511,8 @@ static void levelA_count(LevelAJob<NW, Src> &job, uint64_t est_records, Timer &t
 // Scatter the records of buckets [b_lo, b_hi) into X, CTA-major (see `Pieces`): CTA g of the level-A grid owns one contiguous
 // region, partitioned inside. pbase_buf ([G][PA], caller-owned) receives the first record of every (CTA, partition) piece.
 // I_pass / total_records only steer the number of partition sub-ranges.
-template <int NW, class Src>
-static void levelA_scatter(LevelAJob<NW, Src> &job, int b_lo, int b_hi, uint64_t I_pass, uint64_t total_records, uint64_t *X, uint64_t *pbase_buf,
+template <int NW, class Src, bool BOTH>
+static void levelA_scatter(LevelAJob<NW, Src, BOTH> &job, int b_lo, int b_hi, uint64_t I_pass, uint64_t total_records, uint64_t *X, uint64_t *pbase_buf,
                            Pieces &pcs, Timer &tm, Trace &tr) {
     Ctx *ctx = job.ctx;
     cudaStream_t st = ctx->stream;
@@ -1732,45 +1535,31 @@ static void levelA_scatter(LevelAJob<NW, Src> &job, int b_lo, int b_hi, uint64_t
     }
     pcs.pbase = pbase_buf; pcs.cnt = job.blk_counts.p + p_lo; pcs.cnt_stride = PA_all; pcs.PA = PA; pcs.G = G;
     tm.start();
-    if (job.roll) {
-        if constexpr (std::is_same<Src, ReadsSrc>::value) {
-            {
-            // partition sub-ranges (only with the id array, where a foreign window costs just the roll): fewer streams open
-            // per CTA. A sub-range costs one more roll over ALL windows of the source: worth it when the pass holds most of the job's
-            // records (a single-pass job gains from 4 sub-ranges, a job of several passes loses from even 2)
-            int nsub_auto = (int)(4.0 * (double)I_pass / (double)std::max<uint64_t>(1, total_records) + 0.5);
-            nsub_auto = std::min(4, std::max(1, nsub_auto));
-            uint32_t nsub = job.use_ids ? (uint32_t)(tuning().a_sub ? tuning().a_sub : nsub_auto) : 1u;
-            if (nsub > PA) nsub = PA;
-            for (uint32_t sb = 0; sb < nsub; ++sb) {
-                const uint32_t q_lo = (uint32_t)((uint64_t)PA * sb / nsub), q_hi = (uint32_t)((uint64_t)PA * (sb + 1) / nsub);
-                if (q_hi == q_lo) continue;
-                LevelA pa_sub = pa;
-                pa_sub.PA = q_hi - q_lo;
-                uint32_t cap = 0;
-                const size_t smem = levelA_batch_smem<NW>(pa_sub.PA, &cap);
-                if (job.use_ids) SG_CUDA(cudaFuncSetAttribute(levelA_scatter_roll_k<NW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                else SG_CUDA(cudaFuncSetAttribute(levelA_scatter_roll_k<NW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                for (size_t si = 0; si < job.srcs.size(); ++si) {
-                    const Src &src = job.srcs[si];
-                    if (src.n == 0) continue;
-                    if (job.use_ids)
-                        levelA_scatter_roll_k<NW, true><<<G, kRollThreads, smem, st>>>(src, pa_sub, base.p, X, job.tile_off[si].p, job.ids[si].p, p_lo + q_lo, PA, q_lo, (uint64_t)job.ids[si].n, cap);
-                    else
-                        levelA_scatter_roll_k<NW, false><<<G, kRollThreads, smem, st>>>(src, pa, base.p, X, nullptr, nullptr, 0u, PA, 0u, 0ull, cap);
-                    ctx->launches++; ctx->times.level_a_scatters++;
-                }
-            }
-            }
-        }
-    } else {
-        const size_t smem = (size_t)PA * (sizeof(uint64_t) + sizeof(uint32_t));
-        SG_CUDA(cudaFuncSetAttribute(levelA_scatter_k<NW, Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    // partition sub-ranges (only with the id array, where a foreign window costs just the roll): fewer streams open per CTA. A
+    // sub-range costs one more roll over ALL windows of the source: worth it when the pass holds most of the job's records (a
+    // single-pass job gains from 4 sub-ranges, a job of several passes loses from even 2). Measured for canonical reads only, so
+    // the all-windows count and the k-mer set source scatter once per pass (a (k+1)-mer rolled again for its two records made
+    // 4 sub-ranges slower than one, DESIGN.md 6.2).
+    int nsub_auto = (int)(4.0 * (double)I_pass / (double)std::max<uint64_t>(1, total_records) + 0.5);
+    nsub_auto = std::min(4, std::max(1, nsub_auto));
+    uint32_t nsub = job.use_ids && !BOTH && Src::kSubRanges ? (uint32_t)(tuning().a_sub ? tuning().a_sub : nsub_auto) : 1u;
+    if (nsub > PA) nsub = PA;
+    for (uint32_t sb = 0; sb < nsub; ++sb) {
+        const uint32_t q_lo = (uint32_t)((uint64_t)PA * sb / nsub), q_hi = (uint32_t)((uint64_t)PA * (sb + 1) / nsub);
+        if (q_hi == q_lo) continue;
+        LevelA pa_sub = pa;
+        pa_sub.PA = q_hi - q_lo;
+        uint32_t cap = 0;
+        const size_t smem = levelA_batch_smem<NW>(pa_sub.PA, &cap);
+        if (job.use_ids) SG_CUDA(cudaFuncSetAttribute(levelA_scatter_roll_k<NW, Src, BOTH, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        else SG_CUDA(cudaFuncSetAttribute(levelA_scatter_roll_k<NW, Src, BOTH, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         for (size_t si = 0; si < job.srcs.size(); ++si) {
             const Src &src = job.srcs[si];
             if (src.n == 0) continue;
-            levelA_scatter_k<NW, Src><<<G, kAThreads, smem, st>>>(src, pa, base.p, X, job.use_ids ? job.tile_off[si].p : nullptr,
-                                                                 job.use_ids ? job.ids[si].p : nullptr, p_lo);
+            if (job.use_ids)
+                levelA_scatter_roll_k<NW, Src, BOTH, true><<<G, kRollThreads, smem, st>>>(src, pa_sub, base.p, X, job.tile_off[si].p, job.ids[si].p, p_lo + q_lo, PA, q_lo, (uint64_t)job.ids[si].n, cap);
+            else
+                levelA_scatter_roll_k<NW, Src, BOTH, false><<<G, kRollThreads, smem, st>>>(src, pa, base.p, X, nullptr, nullptr, 0u, PA, 0u, 0ull, cap);
             ctx->launches++; ctx->times.level_a_scatters++;
         }
     }
@@ -1783,14 +1572,13 @@ static void levelA_scatter(LevelAJob<NW, Src> &job, int b_lo, int b_hi, uint64_t
 // against the arena when the output is allocated)
 static double pass_bytes_needed(uint64_t recs, size_t W) { return (double)recs * W * 2.0 + (double)recs * (W + 4) * 0.6 + (64 << 20); }
 
-template <int NW, class Src>
+template <int NW, bool BOTH, class Src>
 static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, int B, bool want_counts, bool double_selfrc, uint64_t est_records, KSet *out) {
     const int total_bits = 2 * K;
     const size_t W = 8 * NW;
     cudaStream_t st = ctx->stream;
     Timer tm(st);
     Trace tr(st);
-    constexpr bool kIsReads = std::is_same<Src, ReadsSrc>::value;
 
     out->bsz.assign(B, 0);
     DArr<unsigned long long> d_bsz(ctx, B);
@@ -1809,12 +1597,11 @@ static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, int B, bool
     int64_t first = 0;
     for (int s_lo = 0; s_lo < B; s_lo += SR) {
         const int share = (kMaxChunks - (int)out->chunks.size()) / (n_ranges - s_lo / SR);
-        LevelAJob<NW, Src> job;
+        LevelAJob<NW, Src, BOTH> job;
         job.ctx = ctx; job.srcs = srcs; job.K = K; job.B = B; job.rA = rA; job.G = ctx->num_sms * levelA_ctas_per_sm();
         job.s_lo = s_lo; job.s_hi = std::min(B, s_lo + SR);
         job.PA_all = (uint32_t)(job.s_hi - job.s_lo) << rA;
-        if constexpr (kIsReads) job.roll = !srcs.empty() && !srcs[0].both;
-        levelA_count(job, est_records, tm, tr);
+        levelA_count(job, tm, tr);
         // bucket-group passes: simulate the greedy "as many whole buckets as fit" plan to learn how many passes are needed, then
         // aim for equally sized passes (a tiny last pass still costs a full scan of the source), at most `share` of them
         auto current_limit = [&]() {
@@ -1909,9 +1696,9 @@ static uint64_t count_windows(Ctx *ctx, int K) {
     return (uint64_t)wn;
 }
 
-static ReadsSrc reads_source(Ctx *ctx, int K, bool both) {
+static ReadsSrc reads_source(Ctx *ctx, int K) {
     ReadsSrc src;
-    src.words = ctx->d_words; src.offs = ctx->d_offs; src.lens = ctx->d_lens; src.n = ctx->n_reads; src.nwords = ctx->n_words; src.K = K; src.both = both;
+    src.words = ctx->d_words; src.offs = ctx->d_offs; src.lens = ctx->d_lens; src.n = ctx->n_reads; src.nwords = ctx->n_words; src.K = K;
     return src;
 }
 
@@ -1921,10 +1708,10 @@ static KSet *count_reads_nw(Ctx *ctx, int K, int B, int mode) {
     KSet *ks = new KSet();
     ks->ctx = ctx; ks->K = K; ks->nw = NW; ks->B = B; ks->has_counts = (mode == kCanonical);
     try {
-        const bool both = (mode == kAllWindows);
         const uint64_t wn = count_windows(ctx, K);
-        std::vector<ReadsSrc> srcs{reads_source(ctx, K, both)};
-        run_count<NW, ReadsSrc>(ctx, srcs, K, B, mode == kCanonical, mode == kCanonical && (K % 2 == 0), wn * (both ? 2 : 1), ks);
+        std::vector<ReadsSrc> srcs{reads_source(ctx, K)};
+        if (mode == kAllWindows) run_count<NW, true>(ctx, srcs, K, B, false, false, wn * 2, ks);
+        else run_count<NW, false>(ctx, srcs, K, B, true, K % 2 == 0, wn, ks);
     } catch (...) { delete ks; throw; }
     return ks;
 }
@@ -1941,18 +1728,18 @@ KSet *count_from_reads(Ctx *ctx, int K, int B, int mode) {
     }
 }
 
-template <int NW, int NWS>
+template <int NW>
 static KSet *kmers_from_kpomers_nw(Ctx *ctx, const KSet *kp, int B) {
     const int K = kp->K - 1;
     KSet *ks = new KSet();
     ks->ctx = ctx; ks->K = K; ks->nw = NW; ks->B = B; ks->has_counts = false;
     try {
-        std::vector<KpomerSrc<NWS>> srcs;
+        std::vector<KmerSetSrc> srcs;
         for (const Chunk &c : kp->chunks) {
-            KpomerSrc<NWS> s; s.keys = c.keys.p; s.n = c.n; s.K = K;
+            KmerSetSrc s; s.words = c.keys.p; s.n = c.n; s.nwords = (uint64_t)c.n * kp->nw; s.K = K; s.stride = (uint32_t)kp->nw;
             srcs.push_back(s);
         }
-        run_count<NW, KpomerSrc<NWS>>(ctx, srcs, K, B, false, false, (uint64_t)kp->n * 2, ks);
+        run_count<NW, false>(ctx, srcs, K, B, false, false, (uint64_t)kp->n * 2, ks);
     } catch (...) { delete ks; throw; }
     return ks;
 }
@@ -1960,17 +1747,14 @@ static KSet *kmers_from_kpomers_nw(Ctx *ctx, const KSet *kp, int B) {
 KSet *kmers_from_kpomers(Ctx *ctx, const KSet *kp, int B) {
     SG_CHECK(kp->K >= 2, 2, "source k-mers too short");
     SG_CHECK(B >= 1 && B <= (1 << 20), 2, "num_buckets must be in [1, 2^20]");
-    const int K = kp->K - 1;
-    const int nw = nwords_of(K), nws = kp->nw;
+    SG_CHECK(kp->nw == nwords_of(kp->K), 2, "unsupported k-mer word combination");
     ctx->times = PhaseTimes();
-    if (nw == 1 && nws == 1) return kmers_from_kpomers_nw<1, 1>(ctx, kp, B);
-    if (nw == 1 && nws == 2) return kmers_from_kpomers_nw<1, 2>(ctx, kp, B);
-    if (nw == 2 && nws == 2) return kmers_from_kpomers_nw<2, 2>(ctx, kp, B);
-    if (nw == 2 && nws == 3) return kmers_from_kpomers_nw<2, 3>(ctx, kp, B);
-    if (nw == 3 && nws == 3) return kmers_from_kpomers_nw<3, 3>(ctx, kp, B);
-    if (nw == 3 && nws == 4) return kmers_from_kpomers_nw<3, 4>(ctx, kp, B);
-    if (nw == 4 && nws == 4) return kmers_from_kpomers_nw<4, 4>(ctx, kp, B);
-    throw Error(2, "unsupported k-mer word combination");
+    switch (nwords_of(kp->K - 1)) {
+        case 1: return kmers_from_kpomers_nw<1>(ctx, kp, B);
+        case 2: return kmers_from_kpomers_nw<2>(ctx, kp, B);
+        case 3: return kmers_from_kpomers_nw<3>(ctx, kp, B);
+        default: return kmers_from_kpomers_nw<4>(ctx, kp, B);
+    }
 }
 
 // checksums of a counted set (bench / multi-GPU self check): out = { n, sum of all key words, xor of all key words rotated by
@@ -2199,19 +1983,17 @@ __global__ void __launch_bounds__(kPullThreads) dist_pull_k(const PullSrc *__res
     }
 }
 
-template <int NW>
+template <int NW, bool BOTH>
 struct DistStateNW : DistState {
-    LevelAJob<NW, ReadsSrc> job;
+    LevelAJob<NW, ReadsSrc, BOTH> job;
 
     void begin() override {
         Timer tm(ctx->stream);
         Trace tr(ctx->stream);
-        const uint64_t wn = count_windows(ctx, K);
         job.ctx = ctx; job.K = K; job.B = B; job.rA = plan.rA; job.G = G;
-        job.srcs.assign(1, reads_source(ctx, K, mode == kAllWindows));
+        job.srcs.assign(1, reads_source(ctx, K));
         job.s_lo = 0; job.s_hi = B; job.PA_all = plan.PA_all;
-        job.roll = (mode == kCanonical);
-        levelA_count(job, wn * (mode == kAllWindows ? 2 : 1), tm, tr);
+        levelA_count(job, tm, tr);
     }
     void local_counts(uint64_t *h_out) override { memcpy(h_out, job.h_part.data(), (size_t)plan.PA_all * 8); }
     const uint32_t *blk_counts_ptr() override { return job.blk_counts.p; }
@@ -2294,6 +2076,12 @@ struct DistStateNW : DistState {
     }
 };
 
+template <int NW>
+static DistState *dist_state_new(int mode) {
+    if (mode == kAllWindows) return new DistStateNW<NW, true>();
+    return new DistStateNW<NW, false>();
+}
+
 DistState *dist_begin(Ctx *ctx, int K, int B, int mode, int world, int rank) {
     SG_CHECK(K >= 1 && K <= 128, 2, "K must be in [1,128]");
     SG_CHECK(B >= 1 && B <= kLevelAMaxParts, 2, "distributed count: num_buckets must be in [1, 8192]");
@@ -2303,10 +2091,10 @@ DistState *dist_begin(Ctx *ctx, int K, int B, int mode, int world, int rank) {
     ctx->times = PhaseTimes();
     DistState *d = nullptr;
     switch (nwords_of(K)) {
-        case 1: d = new DistStateNW<1>(); break;
-        case 2: d = new DistStateNW<2>(); break;
-        case 3: d = new DistStateNW<3>(); break;
-        default: d = new DistStateNW<4>(); break;
+        case 1: d = dist_state_new<1>(mode); break;
+        case 2: d = dist_state_new<2>(mode); break;
+        case 3: d = dist_state_new<3>(mode); break;
+        default: d = dist_state_new<4>(mode); break;
     }
     d->ctx = ctx; d->K = K; d->B = B; d->mode = mode; d->nw = nwords_of(K);
     d->G = ctx->num_sms * levelA_ctas_per_sm();

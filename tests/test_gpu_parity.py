@@ -170,8 +170,8 @@ def test_ragged_empty_and_short_reads():
 
 
 def test_long_reads_take_the_unstaged_path():
-    """reads of 400..6000 bp: a tile's packed reads no longer fit the shared-memory staging area (kStageWords), so the level-A
-    kernels read the words from global memory; mixed with short reads so that staged and unstaged tiles alternate"""
+    """reads of 400..6000 bp: a warp tile's packed reads no longer fit its shared-memory staging slice (kRollStageWords), so the
+    level-A kernels read the words from global memory; mixed with short reads so that staged and unstaged tiles alternate"""
     from gpu_util import gpu_graph_artifacts
     rng = np.random.default_rng(8)
     genome = "".join("ACGT"[i] for i in rng.integers(0, 4, 9000))

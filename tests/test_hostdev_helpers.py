@@ -70,41 +70,26 @@ def check_all(ctx_h, on_device):
 
 def check_roll(ctx_h, on_device):
     """op 10: the rolling window + rolling reverse complement of the level-A kernels (kmer_dev.cuh roll_init/roll_next)
-    against direct window extraction + FastRC, for every window of sequences whose lengths straddle word boundaries."""
+    against direct window extraction + FastRC, for every window of sequences whose lengths straddle word boundaries, in the
+    chunks of both strand modes: 24 windows (canonical) and 12 windows (all windows, two records per window)."""
     rng = np.random.default_rng(99)
-    for K in (1, 2, 5, 21, 22, 31, 32, 33, 55, 56, 63, 64, 65, 77, 78, 96, 97, 127, 128):
-        nw = (K + 31) // 32
-        for L in (K, K + 1, K + 23, K + 24, K + 25, 150, 151, 192, 257, 1000):
-            if L < K:
-                continue
-            nwords = (L + 31) // 32
-            nrec = max((nwords + nw - 1) // nw, (L - K + 1 + 23) // 24 + 1)
-            codes = np.zeros(nrec * nw * 32, np.uint64)
-            codes[:L] = rng.integers(0, 4, L, dtype=np.uint64)
-            sh = (np.arange(32, dtype=np.uint64) * np.uint64(2))
-            words = (codes.reshape(-1, 32) << sh).sum(axis=1, dtype=np.uint64).reshape(nrec, nw)
-            out = run_selftest(ctx_h, on_device, 10, K, L, words)
-            nwin = L - K + 1
-            for u in range(nrec):
-                cnt = min(24, max(0, nwin - 24 * u))
-                assert int(out[u]) == (cnt << 32), (K, L, u, hex(int(out[u])))
-
-
-def test_pair_mailbox_protocol_under_host_threads():
-    """op 11: the sector-pairing mailbox protocol (pair_mailbox.cuh; opt-in level-A variant for round 2) hammered by real host
-    threads: whatever the interleaving every position is written exactly once with its own record, and pairs do form."""
-    L = _lib.load()
-    for threads, streams, per_thread in ((8, 64, 200000), (16, 4096, 100000), (8, 1, 100000), (3, 7, 50001), (1, 16, 10000)):
-        keys = np.array([per_thread, 0, 0], np.uint64)
-        out = np.zeros(3, np.uint64)
-        rc = L.sgpu_selftest(None, 0, 11, 21, (threads << 32) | streams, keys.ctypes.data_as(C.c_void_p), 3, out.ctypes.data_as(C.c_void_p))
-        assert rc == 0
-        errors, pairs, singles = (int(x) for x in out)
-        assert errors == 0, (threads, streams, per_thread, errors)
-        assert 2 * pairs + singles == threads * per_thread
-        assert pairs > 0
-        if threads == 1:
-            assert singles <= 3 * streams          # a single producer pairs everything but the odd ends
+    for C_ in (24, 12):
+        for K in (1, 2, 5, 21, 22, 31, 32, 33, 55, 56, 63, 64, 65, 77, 78, 96, 97, 127, 128):
+            nw = (K + 31) // 32
+            for L in (K, K + 1, K + C_ - 1, K + C_, K + C_ + 1, 150, 151, 192, 257, 1000):
+                if L < K:
+                    continue
+                nwords = (L + 31) // 32
+                nrec = max((nwords + nw - 1) // nw, (L - K + 1 + C_ - 1) // C_ + 1)
+                codes = np.zeros(nrec * nw * 32, np.uint64)
+                codes[:L] = rng.integers(0, 4, L, dtype=np.uint64)
+                sh = (np.arange(32, dtype=np.uint64) * np.uint64(2))
+                words = (codes.reshape(-1, 32) << sh).sum(axis=1, dtype=np.uint64).reshape(nrec, nw)
+                out = run_selftest(ctx_h, on_device, 10, K, (C_ << 32) | L, words)
+                nwin = L - K + 1
+                for u in range(nrec):
+                    cnt = min(C_, max(0, nwin - C_ * u))
+                    assert int(out[u]) == (cnt << 32), (C_, K, L, u, hex(int(out[u])))
 
 
 def test_host_roll_matches_direct_extraction():
