@@ -332,43 +332,44 @@ __global__ void __launch_bounds__(kRollThreads, 2) levelA_count_roll_k(Src src, 
     for (uint32_t i = threadIdx.x; i < p.PA; i += blockDim.x) out[i] += hist[i];
 }
 
-// base rows are `row_stride` cursors long; this launch handles the partitions [q_lo, q_lo + p.PA) of a row (p.PA = the
-// sub-range's size, id_lo = id of its first partition): a bucket-group pass may be split into partition sub-ranges so that
-// the streams a CTA has open at any time stay few.
+// base rows are `row_stride` cursors long; a launch handles the partitions [q_lo, q_lo + p.PA) of a row (p.PA = the sub-range's
+// size, id_lo = id of its first partition): a bucket-group pass may be split into partition sub-ranges so that the streams a CTA
+// has open at any time stay few.
 // Records stored one by one as they are rolled leave L2 as partly written sectors: with PA = 640 streams per CTA a stream
 // receives a record only every few microseconds, and lone 16-byte stores at 640 streams run at about a ninth of the HBM rate
-// (DESIGN.md 6.2). The kernel therefore collects its own windows in a shared-memory batch and writes it out partition by
-// partition, as refine_k does:
-// - a warp reserves room for one window step of its lanes with one shared-memory atomic, and a record takes its rank in its
-//   partition with another (the cursor atomic of the store-as-you-go form);
-// - when a reservation does not fit, the warp stops with that window pending, and every warp meets at the flush: a scan of the
-//   batch counts places each partition's run in the batch and claims it from the partition's cursor, an index array permutes
-//   the batch into partition order, and consecutive threads store consecutive records of a run;
-// - warps without work left, and lanes without a chunk, keep reaching the barriers (__syncthreads_or on "work left").
-// The order inside a partition is arbitrary, as it was with atomic slots.
-// `-Xptxas -v` at 64 registers: no stack frame at 1 and 2 words per record; 16 / 56 bytes with ids and 0 / 32 bytes without at 3
-// and 4 words (the chunk's id queue, the pending window and the tile state all live across the flush). Their cost at K > 64 is
-// not measured.
+// (DESIGN.md 6.2). Both scatter kernels therefore collect a CTA's own records in a shared-memory batch and write it out partition
+// by partition, consecutive threads storing consecutive records of a run. The order inside a partition is arbitrary.
 // (A sector-pairing variant -- two records of a stream leave as one 32-byte store through shared-memory mailboxes -- was
 // parity clean but slower: the CAS traffic on the mailboxes cost more than the full sectors won. Removed.)
-static const uint32_t kABatchNoTag = 0xffffffffu;      // an arrival slot of the batch that a warp reserved but did not fill
-static const int kABatchPartBits = 13;                 // tag = (rank << 13) | partition, partition < kLevelAMaxParts
 // Below kABatchMin records at two CTAs per SM, one CTA per SM takes a larger batch. The threshold itself is not tuned; in
 // scatter_bench -a 1 (DESIGN.md 6.2) 1024-record batches at two CTAs of 512 run at 546 / 278 GB/s (640 / 2560 streams, 16-byte
 // records); the fallback's shape, one CTA of 512 threads per SM with the larger batch, is not in that table.
 static const uint32_t kABatchMin = 1024;
-template <int NW> struct ABatch {
-    static constexpr size_t rec_bytes() { return NW * sizeof(uint64_t) + sizeof(uint32_t) + sizeof(uint16_t); }   // record, tag, index
-};
+// the planned batch hands each warp an equal share of it, and a share must hold one record of each of a warp step's 32 chunks
+// (two, one window's both strands, in all-windows mode): else a warp could never advance
+static_assert(kABatchMin / kRollWarps >= 32 * 2, "a warp's share of the smallest batch holds one window of a warp step");
 // dynamic shared memory: [cursor | batch count] per partition, the warps' RollWarp slices, then the batch
 __host__ __device__ __forceinline__ size_t abatch_offset(uint32_t PA) {
     return ((((size_t)2 * PA * 4 + 15) & ~(size_t)15) + (size_t)kRollWarps * sizeof(RollWarp) + 15) & ~(size_t)15;
 }
+// shared-memory bytes per batched record: the arrival-order batch keeps the record, its tag and a permutation index; the planned
+// batch, already in partition order, keeps the record and its 2-byte partition
+template <int NW, bool PLANNED>
+constexpr size_t abatch_rec_bytes() { return NW * sizeof(uint64_t) + (PLANNED ? sizeof(uint16_t) : sizeof(uint32_t) + sizeof(uint16_t)); }
 
-template <int NW, class Src, bool BOTH, bool HAS_IDS>
+// ---- the id-less form: an arrival-order batch ---------------------------------------------------------------------------
+// Without the id array a record's partition is known only once it is rolled and hashed, so records enter the batch as they come:
+// - a warp reserves room for one window step of its lanes with one shared-memory atomic, and a record takes its rank in its
+//   partition with another;
+// - when a reservation does not fit, the warp stops with that window pending, and every warp meets at the flush: a scan of the
+//   batch counts places each partition's run in the batch and claims it from the partition's cursor, an index array permutes
+//   the batch into partition order, and consecutive threads store consecutive records of a run;
+// - warps without work left, and lanes without a chunk, keep reaching the barriers (__syncthreads_or on "work left").
+static const uint32_t kABatchNoTag = 0xffffffffu;      // an arrival slot of the batch that a warp reserved but did not fill
+static const int kABatchPartBits = 13;                 // tag = (rank << 13) | partition, partition < kLevelAMaxParts
+template <int NW, class Src, bool BOTH>
 __global__ void __launch_bounds__(kRollThreads, 2) levelA_scatter_roll_k(Src src, LevelA p, uint64_t *__restrict__ base, uint64_t *__restrict__ out,
-                                                                        const uint64_t *__restrict__ tile_off, const uint16_t *__restrict__ ids,
-                                                                        uint32_t id_lo, uint32_t row_stride, uint32_t q_lo, uint64_t ids_len, uint32_t cap) {
+                                                                        uint32_t row_stride, uint32_t cap) {
     extern __shared__ __align__(16) unsigned char sm_raw[];
     __shared__ uint32_t s_fill;                   // arrival slots reserved in the batch (may run past cap)
     __shared__ uint32_t warp_tot[kRollWarps];
@@ -381,7 +382,7 @@ __global__ void __launch_bounds__(kRollThreads, 2) levelA_scatter_roll_k(Src src
     uint64_t *stage = reinterpret_cast<uint64_t *>(sm_raw + abatch_offset(PA));    // [cap][NW] records in arrival order
     uint32_t *tags = reinterpret_cast<uint32_t *>(stage + (size_t)cap * NW);      // [cap]     (rank << 13) | partition
     uint16_t *idx = reinterpret_cast<uint16_t *>(tags + cap);                     // [cap]     arrival slot of a batch position
-    uint64_t *mybase = base + (size_t)blockIdx.x * row_stride + q_lo;
+    uint64_t *mybase = base + (size_t)blockIdx.x * row_stride;
     const uint64_t region0 = mybase[0];                                 // cursors of a row ascend with the partition
     for (uint32_t i = threadIdx.x; i < PA; i += blockDim.x) { cur[i] = (uint32_t)(mybase[i] - region0); cnt[i] = 0; }
     if (threadIdx.x == 0) s_fill = 0;
@@ -400,39 +401,28 @@ __global__ void __launch_bounds__(kRollThreads, 2) levelA_scatter_roll_k(Src src
     int nitems = 0;
     uint32_t nunits = 0, unif = 0;
     bool staged = false;
-    uint64_t next_w0 = 0, next_row = 0;
-    const ulonglong2 *row = nullptr;
+    uint64_t next_w0 = 0;
     int u = 0, s = 0, cnt_w = 0;                  // the lane's chunk, its record (st is at its window), its records
     RollState<NW> st;
-    uint64_t idq[Src::kIds / 4];                  // HAS_IDS: the chunk's ids from record s on, two bytes each
     for (;;) {
         while (t < t1) {                          // warp-uniform
             if (need_setup) {
                 const int64_t item0 = t * kRollTile;
                 nitems = (int)min((int64_t)kRollTile, src.n - item0);
-                // the warp's next tile is kRollWarps tiles ahead: its item metadata goes to L2 now, its packed items (and id
-                // rows) at the end of this tile, when the loads of their addresses issued here have long returned
+                // the warp's next tile is kRollWarps tiles ahead: its item metadata goes to L2 now, its packed items at the end of
+                // this tile, when the loads of their addresses issued here have long returned
                 const int64_t nx = (t + kRollWarps) * kRollTile;
                 if (t + kRollWarps < t1) {
                     next_w0 = src.first_word(nx);
                     src.prefetch_items(nx, lane);
-                    if (HAS_IDS) next_row = tile_off[t + kRollWarps];
                 }
                 nunits = roll_warp_setup<BOTH>(src, item0, nitems, rw, &unif, &staged);
-                if (HAS_IDS) row = reinterpret_cast<const ulonglong2 *>(ids + tile_off[t]);
                 u = lane - 32; s = cnt_w = 0;
                 need_setup = false;
             }
             if (s >= cnt_w && u < (int)nunits) {  // the lane's next chunk
                 u += 32;
                 if (u < (int)nunits) {
-                    if (HAS_IDS) {
-#pragma unroll
-                        for (int v = 0; v < Src::kIds / 8; ++v) {
-                            const ulonglong2 x = __ldg(row + (size_t)u * (Src::kIds / 8) + v);
-                            idq[2 * v] = x.x; idq[2 * v + 1] = x.y;
-                        }
-                    }
                     const RollUnit q = roll_unit<BOTH>(rw, nitems, (uint32_t)u, unif, K);
                     const uint64_t *seq = staged ? static_cast<const uint64_t *>(rw.words + rw.off[q.it]) : src.words + src.first_word(t * kRollTile + q.it);
                     roll_init<NW>(st, seq, q.j0, K, q.cnt);
@@ -441,13 +431,7 @@ __global__ void __launch_bounds__(kRollThreads, 2) levelA_scatter_roll_k(Src src
             }
             const bool act = s < cnt_w;
             if (!__any_sync(0xffffffffu, act)) {  // the tile is done
-                if (t + kRollWarps < t1) {
-                    if (lane < 10 && next_w0 + 16 * lane < src.nwords) prefetch_l2(src.words + next_w0 + 16 * lane);   // 10 lines = 32 reads x 5 words
-                    if (HAS_IDS) {                                                                                      // Src::kIdLines <= 64 lines
-                        if ((Src::kIdLines >= 32 || lane < Src::kIdLines) && next_row + 64 * lane < ids_len) prefetch_l2(ids + next_row + 64 * lane);
-                        if (lane < Src::kIdLines - 32 && next_row + 64 * (32 + lane) < ids_len) prefetch_l2(ids + next_row + 64 * (32 + lane));
-                    }
-                }
+                if (t + kRollWarps < t1 && lane < 10 && next_w0 + 16 * lane < src.nwords) prefetch_l2(src.words + next_w0 + 16 * lane);   // 10 lines = 32 reads x 5 words
                 __syncwarp();                     // the slice is rewritten by the next tile's setup
                 t += kRollWarps;
                 need_setup = true;
@@ -457,19 +441,12 @@ __global__ void __launch_bounds__(kRollThreads, 2) levelA_scatter_roll_k(Src src
             bool mine = false;
             Kmer<NW> k;
             if (act) {
-                // a foreign window costs the roll and this compare; the canonical choice is made for own windows only
-                // (a word-by-word select: `cond ? st.f : st.r` bound to a reference made the compiler keep the roll state in
-                // local memory to pick an address)
-                if (HAS_IDS) {
-                    part = (uint32_t)(idq[0] & 0xffffu) - id_lo;               // 0xffff - id_lo stays >= PA
-                    mine = part < PA;
-                }
-                if (!HAS_IDS || mine) {
-                    const bool fwd = BOTH ? !(s & 1) : kmer_is_minimal<NW>(st.f, st.r);
+                // a word-by-word select: `cond ? st.f : st.r` bound to a reference made the compiler keep the roll state in local
+                // memory to pick an address
+                const bool fwd = BOTH ? !(s & 1) : kmer_is_minimal<NW>(st.f, st.r);
 #pragma unroll
-                    for (int j = 0; j < NW; ++j) k.w[j] = fwd ? st.f.w[j] : st.r.w[j];
-                }
-                if (!HAS_IDS) mine = part_of<NW>(p, k, &part);
+                for (int j = 0; j < NW; ++j) k.w[j] = fwd ? st.f.w[j] : st.r.w[j];
+                mine = part_of<NW>(p, k, &part);
             }
             const uint32_t bal = __ballot_sync(0xffffffffu, mine);
             if (bal) {
@@ -488,17 +465,7 @@ __global__ void __launch_bounds__(kRollThreads, 2) levelA_scatter_roll_k(Src src
                     tags[i] = (rank << kABatchPartBits) | part;
                 }
             }
-            if (act && ++s < cnt_w) {
-                if (!BOTH || !(s & 1)) roll_next<NW>(st, K);
-                if (HAS_IDS) {
-                    if ((s & 3) == 0) {
-#pragma unroll
-                        for (int v = 0; v + 1 < Src::kIds / 4; ++v) idq[v] = idq[v + 1];
-                    } else {
-                        idq[0] >>= 16;
-                    }
-                }
-            }
+            if (act && ++s < cnt_w && (!BOTH || !(s & 1))) roll_next<NW>(st, K);
         }
         const bool more = __syncthreads_or(t < t1);
         // ---- flush: scan of the batch counts (a thread owns a run of consecutive partitions), the runs claimed from the cursors
@@ -544,10 +511,229 @@ __global__ void __launch_bounds__(kRollThreads, 2) levelA_scatter_roll_k(Src src
     }
     for (uint32_t i = threadIdx.x; i < PA; i += blockDim.x) mybase[i] = region0 + cur[i];   // chained launches continue here
 }
-// Measured (H100 80GB HBM3, 700 W, 40 M x 150 bp, k = 55, 4 passes, PA = 640, batches of 2848 records at two CTAs per SM): 129 ms
-// per step against 189 ms for the form that stored each record as it was rolled. (A third generation of this kernel -- id sweep,
-// 32-bit keys collected without atomics, ballot-ranked LSD sort of the batch in shared memory, run-by-run flush -- was parity
-// clean and slower than the store-as-you-go form: about twice the thread instructions per record. Removed.)
+
+// ---- the id form: a batch planned from the ids -----------------------------------------------------------------------------
+// With the id array a record's partition is known before it is rolled, so the batch is laid out before anything enters it. A
+// warp walks its tiles in STEPS of 32 chunks (chunk 32 j + lane of the tile for lane `lane`), and a batch runs in four phases:
+// 1. plan: each warp continues where its last batch stopped -- a (tile, step, record) position -- and reads the id rows of its
+//    next step (16-byte loads). It takes the step's records window by window as far as its share of the batch (cap /
+//    kRollWarps) allows: a popc of a ballot per record index counts the step's own records at that index, and each own id adds
+//    one to its partition's batch count. A step that does not fit is taken up to the last window that does, and the warp
+//    resumes there in the next batch. Equal shares keep every warp rolling in every batch: a shared reservation of whole steps
+//    let the first three of sixteen warps take a batch where every record is own (all-windows mode, one pass).
+// 2. claim: a block scan of the batch counts gives each partition its run in the batch, claimed from its cursor.
+// 3. roll: each warp rolls exactly what it planned, with no capacity test; an own record takes the next position of its run
+//    (one shared-memory atomic) and is written there, with its 2-byte partition next to it: the batch is in partition order.
+// 4. flush: consecutive threads store consecutive positions to their partition's slots.
+// Per own record that is two shared-memory atomics (the plan's count, the roll's position) and no tag, no permute pass and no
+// indirect read in the flush; a foreign window costs the roll and an id test. The flush needs no barrier behind it: the next plan
+// touches only the low halves of the batch counts.
+// `-Xptxas -v` (at most 64 registers): no stack frame at 1 to 3 words per record; at 4 words of reads a 16-byte frame with 20
+// bytes of spill stores, against 56 bytes and 68-84 bytes for the id form of the arrival-order kernel it replaced.
+template <int NW, class Src, bool BOTH>
+__global__ void __launch_bounds__(kRollThreads, 2) levelA_scatter_plan_k(Src src, LevelA p, uint64_t *__restrict__ base, uint64_t *__restrict__ out,
+                                                                        const uint64_t *__restrict__ tile_off, const uint16_t *__restrict__ ids,
+                                                                        uint32_t id_lo, uint32_t row_stride, uint32_t q_lo, uint64_t ids_len, uint32_t cap) {
+    extern __shared__ __align__(16) unsigned char sm_raw[];
+    __shared__ uint32_t warp_tot[kRollWarps];
+    constexpr int kR = BOTH ? 2 : 1;              // records per window
+    constexpr int kRowV = Src::kIds / 8;          // 16-byte words of an id row
+    const uint32_t PA = p.PA;
+    // one 32-bit cursor per partition, relative to the first record this launch may write; in `run` the partition's batch count
+    // (low 16 bits, the plan) and the next position of its run in the batch (high 16 bits, the roll; the run's end at the flush)
+    uint32_t *cur = reinterpret_cast<uint32_t *>(sm_raw);               // PA
+    uint32_t *run = cur + PA;                                           // PA
+    RollWarp &rw = *roll_warp_slice(sm_raw, 2 * PA);
+    uint64_t *stage = reinterpret_cast<uint64_t *>(sm_raw + abatch_offset(PA));    // [cap][NW] records in partition order
+    uint16_t *ptag = reinterpret_cast<uint16_t *>(stage + (size_t)cap * NW);      // [cap]     partition of a batch position
+    uint64_t *mybase = base + (size_t)blockIdx.x * row_stride + q_lo;
+    const uint64_t region0 = mybase[0];                                 // cursors of a row ascend with the partition
+    for (uint32_t i = threadIdx.x; i < PA; i += blockDim.x) { cur[i] = (uint32_t)(mybase[i] - region0); run[i] = 0; }
+    __syncthreads();
+    uint64_t *const out0 = out + region0 * NW;
+    const int K = p.K;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t ntiles = (src.n + kRollTile - 1) / kRollTile;
+    const int64_t per = (ntiles + gridDim.x - 1) / gridDim.x;
+    const int64_t t0 = (int64_t)blockIdx.x * per, t1 = min(ntiles, t0 + per);
+    const uint32_t share = cap / kRollWarps;
+
+    // plan position: tile pt, step pj, record ps of every chunk of the step; pn = the tile's chunks, prow = its id rows
+    int64_t pt = t0 + warp;
+    int pj = 0, ps = 0;
+    uint32_t pn = 0;
+    bool p_enter = true;
+    const ulonglong2 *prow = nullptr;
+    // roll position (the plan position the batch started from) and the tile staged in the warp's slice
+    int64_t rt = pt;
+    int rj = 0, rs = 0;
+    bool need_setup = true;
+    int nitems = 0;
+    uint32_t nunits = 0, unif = 0;
+    bool staged = false;
+    uint64_t next_w0 = 0;
+    const ulonglong2 *row = nullptr;
+    for (;;) {
+        // ---- 1. plan
+        uint32_t room = share;
+        while (pt < t1) {                         // warp-uniform
+            if (p_enter) {
+                const uint64_t a = tile_off[pt], b = tile_off[pt + 1];
+                // the id rows of the warp's next tile go to L2 now, a tile before the plan reads them (Src::kIdLines <= 64 lines)
+                if (pt + kRollWarps < t1) {
+                    const uint64_t nr = tile_off[pt + kRollWarps];
+                    if ((Src::kIdLines >= 32 || lane < Src::kIdLines) && nr + 64 * lane < ids_len) prefetch_l2(ids + nr + 64 * lane);
+                    if (lane < Src::kIdLines - 32 && nr + 64 * (32 + lane) < ids_len) prefetch_l2(ids + nr + 64 * (32 + lane));
+                }
+                pn = (uint32_t)((b - a) / Src::kIds);
+                prow = reinterpret_cast<const ulonglong2 *>(ids + a);
+                p_enter = false;
+            }
+            if ((uint32_t)pj * 32 >= pn) {        // the tile is planned
+                pt += kRollWarps; pj = 0; ps = 0; p_enter = true;
+                continue;
+            }
+            if (room < 32 * kR) break;            // not even one window of the step fits for sure
+            const uint32_t u = (uint32_t)pj * 32 + lane;
+            uint64_t idq[Src::kIds / 4];
+#pragma unroll
+            for (int v = 0; v < kRowV; ++v) {
+                ulonglong2 x = make_ulonglong2(~0ull, ~0ull);               // no chunk: foreign ids
+                if (u < pn) x = __ldg(prow + (size_t)u * kRowV + v);
+                idq[2 * v] = x.x; idq[2 * v + 1] = x.y;
+            }
+            int end = Src::kIds;                  // records [ps, end) of the step are taken
+#pragma unroll
+            for (int e = 0; e < Src::kIds; e += kR) {
+                uint32_t part[kR];
+                bool own[kR];
+                uint32_t c = 0;
+#pragma unroll
+                for (int r = 0; r < kR; ++r) {
+                    part[r] = (uint32_t)((idq[(e + r) / 4] >> (16 * ((e + r) % 4))) & 0xffffu) - id_lo;    // 0xffff - id_lo stays >= PA
+                    own[r] = e >= ps && part[r] < PA;
+                    c += __popc(__ballot_sync(0xffffffffu, own[r]));
+                }
+                if (c > room) { end = e; break; }
+                room -= c;
+#pragma unroll
+                for (int r = 0; r < kR; ++r) if (own[r]) atomicAdd(&run[part[r]], 1u);
+            }
+            if (end < Src::kIds) { ps = end; break; }
+            ++pj; ps = 0;
+        }
+        const bool more = __syncthreads_or(pt < t1);
+        // ---- 2. claim: scan of the batch counts (a thread owns a run of consecutive partitions), runs claimed from the cursors
+        const uint32_t own = (PA + kRollThreads - 1) / kRollThreads;
+        const uint32_t j0 = min(PA, threadIdx.x * own), j1 = min(PA, j0 + own);
+        uint32_t sum = 0;
+        for (uint32_t j = j0; j < j1; ++j) sum += run[j] & 0xffffu;
+        uint32_t inc = sum;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t v = __shfl_up_sync(0xffffffffu, inc, o);
+            if (lane >= o) inc += v;
+        }
+        if (lane == 31) warp_tot[warp] = inc;
+        __syncthreads();
+        uint32_t wb = 0, total = 0;
+#pragma unroll
+        for (int w = 0; w < kRollWarps; ++w) { const uint32_t v = warp_tot[w]; if (w < warp) wb += v; total += v; }
+        uint32_t o = wb + inc - sum;
+        for (uint32_t j = j0; j < j1; ++j) {
+            const uint32_t c = run[j] & 0xffffu;
+            run[j] = o << 16;                     // run start; the count starts again at zero
+            o += c;
+            cur[j] += c;                          // the run takes slots [cur - c, cur)
+        }
+        __syncthreads();
+        // ---- 3. roll: from the roll position up to the plan position
+        while (rt < pt || (rt == pt && (rj < pj || (rj == pj && rs < ps)))) {   // warp-uniform
+            if (need_setup) {
+                const int64_t item0 = rt * kRollTile;
+                nitems = (int)min((int64_t)kRollTile, src.n - item0);
+                // the warp's next tile is kRollWarps tiles ahead: its item metadata goes to L2 now, its packed items at the end of
+                // this tile, when the loads of their addresses issued here have long returned
+                const int64_t nx = (rt + kRollWarps) * kRollTile;
+                if (rt + kRollWarps < t1) {
+                    next_w0 = src.first_word(nx);
+                    src.prefetch_items(nx, lane);
+                }
+                nunits = roll_warp_setup<BOTH>(src, item0, nitems, rw, &unif, &staged);
+                row = reinterpret_cast<const ulonglong2 *>(ids + tile_off[rt]);
+                need_setup = false;
+            }
+            if ((uint32_t)rj * 32 >= nunits) {    // the tile is done
+                if (rt + kRollWarps < t1 && lane < 10 && next_w0 + 16 * lane < src.nwords) prefetch_l2(src.words + next_w0 + 16 * lane);   // 10 lines = 32 reads x 5 words
+                __syncwarp();                     // the slice is rewritten by the next tile's setup
+                rt += kRollWarps; rj = 0; rs = 0;
+                need_setup = true;
+                continue;
+            }
+            const int end = (rt == pt && rj == pj) ? ps : Src::kIds;
+            const int u = rj * 32 + lane;
+            if (u < (int)nunits) {
+                const RollUnit q = roll_unit<BOTH>(rw, nitems, (uint32_t)u, unif, K);
+                const int s_end = min(end, BOTH ? 2 * q.cnt : q.cnt);
+                if (rs < s_end) {
+                    uint64_t idq[Src::kIds / 4];
+#pragma unroll
+                    for (int v = 0; v < kRowV; ++v) {
+                        const ulonglong2 x = __ldg(row + (size_t)u * kRowV + v);
+                        idq[2 * v] = x.x; idq[2 * v + 1] = x.y;
+                    }
+                    // the id queue from record rs on (whole words moved register to register, then the rest of a word)
+                    for (int w = 0; w < rs / 4; ++w) {
+#pragma unroll
+                        for (int v = 0; v + 1 < Src::kIds / 4; ++v) idq[v] = idq[v + 1];
+                    }
+                    idq[0] >>= 16 * (rs & 3);
+                    const uint64_t *seq = staged ? static_cast<const uint64_t *>(rw.words + rw.off[q.it]) : src.words + src.first_word(rt * kRollTile + q.it);
+                    RollState<NW> st;
+                    roll_init<NW>(st, seq, q.j0 + rs / kR, K, q.cnt - rs / kR);
+                    for (int s = rs;;) {
+                        const uint32_t part = (uint32_t)(idq[0] & 0xffffu) - id_lo;
+                        if (part < PA) {
+                            // a word-by-word select: `cond ? st.f : st.r` bound to a reference made the compiler keep the roll
+                            // state in local memory to pick an address
+                            const bool fwd = BOTH ? !(s & 1) : kmer_is_minimal<NW>(st.f, st.r);
+                            Kmer<NW> k;
+#pragma unroll
+                            for (int j = 0; j < NW; ++j) k.w[j] = fwd ? st.f.w[j] : st.r.w[j];
+                            const uint32_t pos = atomicAdd(&run[part], 1u << 16) >> 16;
+                            store_rec<NW>(stage + (size_t)pos * NW, k);
+                            ptag[pos] = (uint16_t)part;
+                        }
+                        if (++s >= s_end) break;
+                        if (!BOTH || !(s & 1)) roll_next<NW>(st, K);
+                        if ((s & 3) == 0) {
+#pragma unroll
+                            for (int v = 0; v + 1 < Src::kIds / 4; ++v) idq[v] = idq[v + 1];
+                        } else {
+                            idq[0] >>= 16;
+                        }
+                    }
+                }
+            }
+            if (end == Src::kIds) { ++rj; rs = 0; } else rs = end;
+        }
+        __syncthreads();
+        // ---- 4. flush: position q of a run ending at e goes to slot cur - e + q
+        for (uint32_t q = threadIdx.x; q < total; q += kRollThreads) {
+            const uint32_t part = ptag[q];
+            const uint32_t slot = cur[part] - (run[part] >> 16) + q;
+            store_rec_stream<NW>(out0 + (size_t)slot * NW, load_rec<NW>(stage + (size_t)q * NW));
+        }
+        if (!more) break;
+    }
+    for (uint32_t i = threadIdx.x; i < PA; i += blockDim.x) mybase[i] = region0 + cur[i];   // chained launches continue here
+}
+// Measured (H100 80GB HBM3, 700 W, 40 M x 150 bp, k = 55, 4 passes, PA = 640, two CTAs per SM): the planned batch (3488 records
+// at 16 bytes) takes 114.8-114.9 ms per step against 128.3-129.0 ms for the arrival-order batch (2848 records) in the same form,
+// which took 129 ms against 189 ms for the form that stored each record as it was rolled. (A third generation of
+// this kernel -- id sweep, 32-bit keys collected without atomics, ballot-ranked LSD sort of the batch in shared memory,
+// run-by-run flush -- was parity clean and slower than the store-as-you-go form: about twice the thread instructions per
+// record. Removed.)
 
 // ------------------------------------------------------------------------------------------------------------
 // segments
@@ -1422,23 +1608,25 @@ struct LevelAJob {
 // CTAs of the level-A grid per SM: the two that are resident. (More waves -- 3, 4, 6 per SM -- for tail balance gained a few
 // per cent at best, with 3x smaller pieces for the gather. Not kept.)
 static int levelA_ctas_per_sm() { return 2; }
-// dynamic shared memory of one levelA_scatter_roll_k launch over PA partitions, and its batch capacity in records: the batch
-// takes what the tables and warp slices leave of an SM's share for the two CTAs per SM the grid is sized for (2 x 113 KB of the
+// dynamic shared memory of one level-A scatter launch over PA partitions, and its batch capacity in records: the batch takes
+// what the tables and warp slices leave of an SM's share for the two CTAs per SM the grid is sized for (2 x 113 KB of the
 // 228 KB of an H100 SM). Where the largest tables would leave less than kABatchMin records, the batch takes what a single CTA
-// may opt into, and one CTA per SM is resident.
-template <int NW>
+// may opt into, and one CTA per SM is resident. PLANNED: levelA_scatter_plan_k's batch, else levelA_scatter_roll_k's.
+template <int NW, bool PLANNED>
 static size_t levelA_batch_smem(uint32_t PA, uint32_t *cap) {
-    static_assert(kLevelAMaxParts <= (1 << kABatchPartBits), "a batch tag holds the partition");
+    static_assert(kLevelAMaxParts <= (1 << kABatchPartBits) && kLevelAMaxParts <= 0xffff, "a batch tag holds the partition");
     int dev = 0, per_sm = 0, per_cta = 0, reserved = 0;
     SG_CUDA(cudaGetDevice(&dev));
     SG_CUDA(cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
     SG_CUDA(cudaDeviceGetAttribute(&per_cta, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
     SG_CUDA(cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev));
-    const size_t rec = ABatch<NW>::rec_bytes(), fixed = abatch_offset(PA), kStatic = 128;   // s_fill, warp_tot
+    const size_t rec = abatch_rec_bytes<NW, PLANNED>(), fixed = abatch_offset(PA), kStatic = 128;   // s_fill, warp_tot
     size_t room = (size_t)per_sm / levelA_ctas_per_sm() - (size_t)reserved - kStatic;
     if (room < fixed + kABatchMin * rec) room = (size_t)per_cta - kStatic;
     SG_CHECK(room >= fixed + kABatchMin * rec, 6, "internal: level-A batch does not fit shared memory");
     *cap = (uint32_t)std::min<size_t>((room - fixed) / rec, 32768) & ~31u;     // positions in a batch are 16-bit
+    // the planned batch: a warp's share holds one window of each chunk of a warp step, else the warp could never advance
+    SG_CHECK(!PLANNED || *cap / kRollWarps >= 32 * 2, 6, "internal: level-A warp share below one window step");
     return fixed + (size_t)*cap * rec;
 }
 static int levelA_key_bits(uint64_t est_records, int B, int total_bits, uint32_t target, uint32_t pa_max) {
@@ -1550,16 +1738,16 @@ static void levelA_scatter(LevelAJob<NW, Src, BOTH> &job, int b_lo, int b_hi, ui
         LevelA pa_sub = pa;
         pa_sub.PA = q_hi - q_lo;
         uint32_t cap = 0;
-        const size_t smem = levelA_batch_smem<NW>(pa_sub.PA, &cap);
-        if (job.use_ids) SG_CUDA(cudaFuncSetAttribute(levelA_scatter_roll_k<NW, Src, BOTH, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        else SG_CUDA(cudaFuncSetAttribute(levelA_scatter_roll_k<NW, Src, BOTH, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        const size_t smem = job.use_ids ? levelA_batch_smem<NW, true>(pa_sub.PA, &cap) : levelA_batch_smem<NW, false>(pa_sub.PA, &cap);
+        if (job.use_ids) SG_CUDA(cudaFuncSetAttribute(levelA_scatter_plan_k<NW, Src, BOTH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        else SG_CUDA(cudaFuncSetAttribute(levelA_scatter_roll_k<NW, Src, BOTH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         for (size_t si = 0; si < job.srcs.size(); ++si) {
             const Src &src = job.srcs[si];
             if (src.n == 0) continue;
             if (job.use_ids)
-                levelA_scatter_roll_k<NW, Src, BOTH, true><<<G, kRollThreads, smem, st>>>(src, pa_sub, base.p, X, job.tile_off[si].p, job.ids[si].p, p_lo + q_lo, PA, q_lo, (uint64_t)job.ids[si].n, cap);
+                levelA_scatter_plan_k<NW, Src, BOTH><<<G, kRollThreads, smem, st>>>(src, pa_sub, base.p, X, job.tile_off[si].p, job.ids[si].p, p_lo + q_lo, PA, q_lo, (uint64_t)job.ids[si].n, cap);
             else
-                levelA_scatter_roll_k<NW, Src, BOTH, false><<<G, kRollThreads, smem, st>>>(src, pa, base.p, X, nullptr, nullptr, 0u, PA, 0u, 0ull, cap);
+                levelA_scatter_roll_k<NW, Src, BOTH><<<G, kRollThreads, smem, st>>>(src, pa, base.p, X, PA, cap);
             ctx->launches++; ctx->times.level_a_scatters++;
         }
     }
