@@ -1043,13 +1043,14 @@ __global__ void __launch_bounds__(kRThreads) refine_k(const Seg *__restrict__ se
 // local sort + unique + count
 // ------------------------------------------------------------------------------------------------------------
 template <int NW> struct SortCfg { static const int CAP = NW <= 2 ? 2048 : 1024; };
-static const int kSThreads = 256;
+static const int kSThreads = 512;     // two CTAs of 16 warps per SM: room for a second segment buffer at every record width
 static const int kSWarps = kSThreads / 32;
 
 // stable LSD pass over key bits [pos, pos+width) : A -> Bf
 template <int NW>
 __device__ __forceinline__ void lsd_pass(const uint64_t *A, uint64_t *Bf, uint32_t n, int K, int pos, int width, uint32_t *cnt /*[kSWarps][256]*/,
-                                         uint32_t *tot /*[256]*/) {
+                                         uint32_t *tot /*[256 / 32]*/) {
+    static_assert(kSThreads >= 256, "one thread per digit");
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t chunk = ((n + kSWarps * 32 - 1) / (kSWarps * 32)) * 32;   // items per warp, multiple of 32
     const uint32_t w0 = warp * chunk;
@@ -1064,27 +1065,30 @@ __device__ __forceinline__ void lsd_pass(const uint64_t *A, uint64_t *Bf, uint32
         __syncwarp();
     }
     __syncthreads();
-    // per digit: warp prefix + digit totals
+    // per digit (threads 0..255, one digit each): warp prefix + digit totals
     {
-        const uint32_t d = threadIdx.x;     // kSThreads == 256 digits
-        uint32_t run = 0;
+        const uint32_t d = threadIdx.x;
+        uint32_t run = 0, inc = 0;
+        if (d < 256) {
 #pragma unroll
-        for (int w = 0; w < kSWarps; ++w) { uint32_t t = cnt[w * 256 + d]; cnt[w * 256 + d] = run; run += t; }
-        // exclusive scan of run over 256 digits
-        uint32_t inc = run;
+            for (int w = 0; w < kSWarps; ++w) { uint32_t t = cnt[w * 256 + d]; cnt[w * 256 + d] = run; run += t; }
+            // exclusive scan of run over 256 digits
+            inc = run;
 #pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
-            if (lane >= o) inc += t;
+            for (int o = 1; o < 32; o <<= 1) {
+                uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
+                if (lane >= o) inc += t;
+            }
+            if (lane == 31) tot[warp] = inc;
         }
-        if (lane == 31) tot[warp] = inc;
         __syncthreads();
-        uint32_t wb = 0;
-        for (int w = 0; w < warp; ++w) wb += tot[w];
-        __syncthreads();
-        const uint32_t ex = wb + inc - run;
+        if (d < 256) {
+            uint32_t wb = 0;
+            for (int w = 0; w < warp; ++w) wb += tot[w];
+            const uint32_t ex = wb + inc - run;
 #pragma unroll
-        for (int w = 0; w < kSWarps; ++w) cnt[w * 256 + d] += ex;
+            for (int w = 0; w < kSWarps; ++w) cnt[w * 256 + d] += ex;
+        }
     }
     __syncthreads();
     for (uint32_t r = 0; r < chunk; r += 32) {
@@ -1118,273 +1122,312 @@ __device__ __forceinline__ uint64_t *lsd_sort_range(uint64_t *A, uint64_t *Bf, u
     return A;
 }
 
+// exclusive scan of one value per thread over the CTA; `all` receives the total. One barrier; `tot` is free again only after the
+// next barrier.
+__device__ __forceinline__ uint32_t cta_exscan(uint32_t v, uint32_t *tot, uint32_t &all) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint32_t inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += t;
+    }
+    if (lane == 31) tot[warp] = inc;
+    __syncthreads();
+    uint32_t wb = 0;
+    all = 0;
+#pragma unroll
+    for (int w = 0; w < kSWarps; ++w) { const uint32_t t = tot[w]; if (w < warp) wb += t; all += t; }
+    return wb + inc - v;
+}
+
+// +1 on the 16-bit counter c[i] (two counters share a 32-bit word; no counter exceeds CAP), returns its old value
+__device__ __forceinline__ uint32_t atomic_inc_u16(uint16_t *c, uint32_t i) {
+    const int sh = (i & 1) * 16;
+    return (atomicAdd(reinterpret_cast<uint32_t *>(c) + (i >> 1), 1u << sh) >> sh) & 0xffffu;
+}
+
+// asynchronous global -> shared copy of a segment's records by the whole CTA (cp.async; completes at cp_async_wait_all). Records
+// of an even number of words start on a 16-byte boundary and go as 16-byte copies; 8- and 24-byte records may start on an 8-byte
+// boundary and go as 8-byte copies. Empty and oversize segments are never loaded.
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
+template <int NW, int CAP>
+__device__ __forceinline__ void prefetch_segment(uint64_t *dst, const uint64_t *src, uint64_t len) {
+    if (len == 0 || len > (uint64_t)CAP) return;
+    const uint32_t sdst = (uint32_t)__cvta_generic_to_shared(dst);
+    if (NW % 2 == 0) {
+        for (uint32_t q = threadIdx.x; q < (uint32_t)len * NW / 2; q += kSThreads)
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(sdst + 16 * q), "l"(src + 2 * q) : "memory");
+    } else {
+        for (uint32_t q = threadIdx.x; q < (uint32_t)len * NW; q += kSThreads)
+            asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"(sdst + 8 * q), "l"(src + q) : "memory");
+    }
+}
+
 // ---- local sort: representative + residual -----------------------------------------------------------------------------
 // After level A + MSD refinement a segment holds ~CAP*3/4 records that agree on their first `bits` key bits. Most of them are
-// copies of a few keys (a genomic (k+1)-mer is seen ~coverage times) plus error singletons. Two earlier generations (a full LSD
-// radix sort per segment; one counting pass into 2^11 bins with one thread collapsing each bin) were replaced by the kernel
-// below; the LSD passes above survive as its exact fallback.
+// copies of a few keys (a genomic (k+1)-mer is seen ~coverage times) plus error singletons. Earlier generations (a full LSD
+// radix sort per segment; one counting pass into 2^11 bins with one thread collapsing each bin; one thread per bin
+// deduplicating its residual records and writing the bin) were replaced by the kernel below; the LSD passes above survive as its
+// exact fallback.
 static const int kSortBinBits = 11;   // bins per segment = 2^11: fewer bins = less per-segment bookkeeping (init + two scans over the bins) but more
                                       // keys sharing a bin (2^10 bins gave no gain)
 
-// The one-thread-per-bin generation ran with few active lanes per instruction and barrier stalls on top: one thread chewing
-// through the ~coverage copies of a genomic k-mer held up its whole CTA. Here every bin elects a representative (the
-// record with the smallest index, one shared-memory atomicMin per record); records equal to their bin's representative
-// only bump a counter. Only the few records that differ from it (bins holding two or more distinct keys) are scattered
-// into a small residual buffer and deduplicated by one thread per bin, so the per-bin work is a handful of compares.
-// Anything unusual (residual overflow, a bin with many distinct keys) falls back to the exact LSD radix path, which
-// uses the segment's region in the partner buffer as scratch.
+// Every bin elects a representative (any one of its records: a plain shared-memory store per record); records equal to it only
+// bump a counter. A bin holding records that differ from its representative gets a run of slots in a small residual buffer:
+// the representative first, then those records. Every residual slot then finds by itself, comparing within its bin's few
+// slots, whether it holds its key's first copy and how many copies there are, and every distinct key takes its rank in the
+// bin from the same compares, so each output record has its position without a thread walking a bin. Anything unusual
+// (residual overflow, a bin with more than kBinSlotsMax slots or more than kBinDistinctMax keys) falls back to the exact LSD
+// radix path, which uses the segment's region in the partner buffer as scratch.
+// The CTAs are persistent and load one segment ahead: while segment i is sorted, segment i+1 arrives in the second buffer by
+// cp.async, and the claim of segment i+2 is in flight.
 static const int kResCap = 512;
+static const int kBinSlotsMax = 128;
+static const int kBinDistinctMax = 16;
 
 template <int NW, int kBinBits, int CAP>
-__global__ void __launch_bounds__(kSThreads) local_sort3_k(const Seg *__restrict__ segs, uint64_t nsegs, int K, uint64_t *__restrict__ buf0,
-                                                          uint64_t *__restrict__ buf1, uint32_t *__restrict__ ndist,
-                                                          unsigned long long *__restrict__ work_counter, unsigned long long *__restrict__ stats) {
+struct SortSmem {
+    static constexpr int kBins = 1 << kBinBits;
+    // two segment buffers, the residual records, rep/repcnt/rhist/dres and rstart (u16 per bin), rcnt/rbin (u16 per residual slot)
+    static constexpr size_t bytes = ((size_t)2 * CAP + kResCap) * NW * sizeof(uint64_t) + ((size_t)5 * kBins + 2 + 2 * kResCap) * sizeof(uint16_t);
+};
+
+template <int NW, int kBinBits, int CAP>
+__device__ __forceinline__ void sort_segment(const uint64_t si, const Seg s, uint64_t *A, uint64_t *R, uint16_t *rep, uint16_t *rcnt, uint16_t *rbin,
+                                             uint32_t *lsdcnt, uint32_t *tot, int *s_flag, int K, uint64_t *buf0, uint64_t *buf1,
+                                             uint32_t *ndist, unsigned long long *stats) {
     constexpr int kBins = 1 << kBinBits;
     constexpr int BPT = kBins / kSThreads;
-    static_assert(3 * kBins >= CAP + 1 && 3 * kBins >= kSWarps * 256, "rep/repcnt/rhist double as scratch of the LSD fallback");
-    static_assert(CAP % kSThreads == 0 && CAP <= SortCfg<NW>::CAP, "segment capacity: a multiple of the CTA size, at most the default");
     constexpr int IPT = CAP / kSThreads;                  // records per thread
-    extern __shared__ uint64_t sm64[];
-    uint64_t *A = sm64;                                   // CAP*NW   the segment
-    uint64_t *R = A + (size_t)CAP * NW;                   // kResCap*NW residual records, grouped by bin
-    uint32_t *rep = reinterpret_cast<uint32_t *>(R + (size_t)kResCap * NW);   // kBins  index of the bin's representative
-    uint32_t *repcnt = rep + kBins;                       // kBins  copies of the representative besides itself
-    uint32_t *rhist = repcnt + kBins;                     // kBins  residual count -> cursor
-    uint16_t *rstart = reinterpret_cast<uint16_t *>(rhist + kBins);           // kBins+2
-    uint16_t *rcnt = rstart + kBins + 2;                  // kResCap multiplicity per residual slot
-    uint16_t *dres = rcnt + kResCap;                      // kBins  distinct residual keys per bin
-    uint32_t *lsdcnt = rep;                               // fallback only (kSWarps*256 <= 3*kBins)
-    __shared__ uint32_t tot[kSWarps + 1];
-    __shared__ unsigned long long s_w;
-    __shared__ int s_flag;
+    uint16_t *repcnt = rep + kBins;                       // copies of the representative besides itself
+    uint16_t *rhist = repcnt + kBins;                     // residual records -> slot cursor -> output offset of the bin
+    uint16_t *dres = rhist + kBins;                       // distinct keys in the bin's residual slots
+    uint16_t *rstart = dres + kBins;                      // kBins+1 first residual slot of the bin
     const int total_bits = 2 * K;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (;;) {
-        if (threadIdx.x == 0) { s_w = atomicAdd(work_counter, 1ull); s_flag = 0; }
-        __syncthreads();
-        const uint64_t si = s_w;
-        if (si >= nsegs) return;
-        const Seg s = segs[si];
-        uint64_t *gsrc = ((s.bb & 1) ? buf1 : buf0) + s.start * NW;
-        uint64_t *gpartner = ((s.bb & 1) ? buf0 : buf1) + s.start * NW;
-        uint32_t *gcnt = reinterpret_cast<uint32_t *>(gpartner);
-        if (s.len == 0) { if (threadIdx.x == 0) ndist[si] = 0; __syncthreads(); continue; }
-        if (s.len > (uint64_t)CAP) {
-            if (threadIdx.x == 0) {
-                gcnt[0] = (uint32_t)s.len; ndist[si] = 1;
-                atomicAdd(&stats[s.bits < (uint32_t)total_bits ? 0 : 2], 1ull);     // [0] is an internal error, [2] an equal-key segment
-            }
-            __syncthreads();
-            continue;
+    uint64_t *gsrc = ((s.bb & 1) ? buf1 : buf0) + s.start * NW;
+    uint64_t *gpartner = ((s.bb & 1) ? buf0 : buf1) + s.start * NW;
+    uint32_t *gcnt = reinterpret_cast<uint32_t *>(gpartner);
+    if (s.len == 0) { if (threadIdx.x == 0) ndist[si] = 0; return; }
+    if (s.len > (uint64_t)CAP) {
+        if (threadIdx.x == 0) {
+            gcnt[0] = (uint32_t)s.len; ndist[si] = 1;
+            atomicAdd(&stats[s.bits < (uint32_t)total_bits ? 0 : 2], 1ull);     // [0] is an internal error, [2] an equal-key segment
         }
-        const uint32_t n = (uint32_t)s.len;
-        const int lo = (int)s.bits;
-        const int r2 = (total_bits - lo) < kBinBits ? (total_bits - lo) : kBinBits;
-        const uint32_t nb = 1u << r2;
-        for (uint32_t i = threadIdx.x; i < nb; i += kSThreads) { rep[i] = 0xffffffffu; repcnt[i] = 0; rhist[i] = 0; dres[i] = 0; }
-        __syncthreads();
-        // ---- P1: load, elect representatives
-        uint32_t dig[IPT];
+        return;
+    }
+    const uint32_t n = (uint32_t)s.len;
+    const int lo = (int)s.bits;
+    const int r2 = (total_bits - lo) < kBinBits ? (total_bits - lo) : kBinBits;
+    const uint32_t nb = 1u << r2;
+    {   // rep = 0xffff (empty bin), repcnt = rhist = dres = 0: the four tables are contiguous, two bins per word
+        uint32_t *w = reinterpret_cast<uint32_t *>(rep);
+        const uint32_t nw = (nb + 1) / 2;
+        for (uint32_t i = threadIdx.x; i < nw; i += kSThreads) { w[i] = 0xffffffffu; w[kBins / 2 + i] = 0; w[kBins + i] = 0; w[3 * kBins / 2 + i] = 0; }
+        if (threadIdx.x == 0) *s_flag = 0;
+    }
+    __syncthreads();
+    // ---- P1: elect representatives
+    uint32_t dig[IPT];
 #pragma unroll
-        for (int j = 0; j < IPT; ++j) {
-            const uint32_t i = threadIdx.x + j * kSThreads;
-            dig[j] = 0;
-            if (i < n) {
-                Kmer<NW> k = load_rec<NW>(gsrc + (size_t)i * NW);
-                store_rec<NW>(A + (size_t)i * NW, k);
-                dig[j] = r2 ? key_bits<NW>(k, K, lo, r2) : 0u;
-                atomicMin(&rep[dig[j]], i);
-            }
+    for (int j = 0; j < IPT; ++j) {
+        const uint32_t i = threadIdx.x + j * kSThreads;
+        dig[j] = 0;
+        if (i < n) {
+            dig[j] = r2 ? key_bits<NW>(load_rec<NW>(A + (size_t)i * NW), K, lo, r2) : 0u;
+            rep[dig[j]] = (uint16_t)i;
         }
-        __syncthreads();
-        // ---- P2: copies of the representative only count; everything else is residual
-        uint32_t resmask = 0;
+    }
+    __syncthreads();
+    // ---- P2: copies of the representative only count; everything else is residual
+    uint32_t resmask = 0, repmask = 0;
 #pragma unroll
-        for (int j = 0; j < IPT; ++j) {
-            const uint32_t i = threadIdx.x + j * kSThreads;
-            if (i < n) {
-                const uint32_t r = rep[dig[j]];
-                if (r != i) {
-                    if (kmer_eq<NW>(load_rec<NW>(A + (size_t)i * NW), load_rec<NW>(A + (size_t)r * NW))) atomicAdd(&repcnt[dig[j]], 1u);
-                    else { atomicAdd(&rhist[dig[j]], 1u); resmask |= 1u << j; }
-                }
-            }
+    for (int j = 0; j < IPT; ++j) {
+        const uint32_t i = threadIdx.x + j * kSThreads;
+        if (i < n) {
+            const uint32_t r = rep[dig[j]];
+            if (r == i) repmask |= 1u << j;
+            else if (kmer_eq<NW>(load_rec<NW>(A + (size_t)i * NW), load_rec<NW>(A + (size_t)r * NW))) atomic_inc_u16(repcnt, dig[j]);
+            else { atomic_inc_u16(rhist, dig[j]); resmask |= 1u << j; }
         }
-        __syncthreads();
-        // ---- P3: exclusive scan of the residual counts
-        const uint32_t b0 = threadIdx.x * BPT;
-        uint32_t loc[BPT];
-        uint32_t sum = 0;
+    }
+    __syncthreads();
+    // ---- P3: residual slots of every bin (its representative + its residual records), exclusive scan
+    const uint32_t b0 = threadIdx.x * BPT;
+    uint32_t loc[BPT];
+    uint32_t sum = 0;
+    bool big = false;
 #pragma unroll
-        for (int q = 0; q < BPT; ++q) { loc[q] = (b0 + q < nb) ? rhist[b0 + q] : 0; sum += loc[q]; }
-        uint32_t inc = sum;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
-            if (lane >= o) inc += t;
-        }
-        if (lane == 31) tot[warp] = inc;
-        __syncthreads();
-        uint32_t wb = 0, rtotal = 0;
-        for (int w = 0; w < kSWarps; ++w) { if (w < warp) wb += tot[w]; rtotal += tot[w]; }
-        {
-            uint32_t run = wb + inc - sum;
-#pragma unroll
-            for (int q = 0; q < BPT; ++q) {
-                if (b0 + q < nb) { rstart[b0 + q] = (uint16_t)run; rhist[b0 + q] = run; }
-                run += loc[q];
-            }
-            if (threadIdx.x == kSThreads - 1) rstart[nb] = (uint16_t)rtotal;
-        }
-        bool bad = rtotal > (uint32_t)kResCap;
-        __syncthreads();
-        // ---- P4: scatter the residual records into their bins
-        if (!bad) {
-#pragma unroll
-            for (int j = 0; j < IPT; ++j) {
-                if (resmask & (1u << j)) {
-                    const uint32_t i = threadIdx.x + j * kSThreads;
-                    const uint32_t pos = atomicAdd(&rhist[dig[j]], 1u);
-                    store_rec<NW>(R + (size_t)pos * NW, load_rec<NW>(A + (size_t)i * NW));
-                }
-            }
-        }
-        __syncthreads();
-        // ---- P5: the thread that owns a bin's representative deduplicates + sorts that bin's residual (tiny) and records
-        //          how many distinct residual keys the bin has. Work is per occupied bin, not per bin.
-        if (!bad) {
-#pragma unroll
-            for (int j = 0; j < IPT; ++j) {
-                const uint32_t i = threadIdx.x + j * kSThreads;
-                if (i >= n || rep[dig[j]] != i) continue;
-                const uint32_t b = dig[j];
-                const uint32_t bs = rstart[b], be = rstart[b + 1];
-                if (be == bs) continue;
-                uint32_t d = 0;
-                if (be - bs == 1) { rcnt[bs] = 1; d = 1; }
-                else {
-                    uint32_t rem_end = be, p = bs, work = 0;
-                    while (p < rem_end) {
-                        const Kmer<NW> key = load_rec<NW>(R + (size_t)p * NW);
-                        uint32_t c = 1, w = p + 1;
-                        for (uint32_t z = p + 1; z < rem_end; ++z) {
-                            const Kmer<NW> x = load_rec<NW>(R + (size_t)z * NW);
-                            if (kmer_eq<NW>(x, key)) ++c;
-                            else { if (w != z) store_rec<NW>(R + (size_t)w * NW, x); ++w; }
-                        }
-                        work += rem_end - p;
-                        rcnt[p] = (uint16_t)c;
-                        rem_end = w;
-                        ++p;
-                        if (work > 1024u || p - bs > 16u) { bad = true; break; }
-                    }
-                    if (bad) break;
-                    d = p - bs;
-                    for (uint32_t a = bs + 1; a < bs + d; ++a) {
-                        const Kmer<NW> key = load_rec<NW>(R + (size_t)a * NW);
-                        const uint16_t kc = rcnt[a];
-                        uint32_t z = a;
-                        while (z > bs && kmer_word_cmp<NW>(load_rec<NW>(R + (size_t)(z - 1) * NW), key) > 0) {
-                            store_rec<NW>(R + (size_t)z * NW, load_rec<NW>(R + (size_t)(z - 1) * NW));
-                            rcnt[z] = rcnt[z - 1];
-                            --z;
-                        }
-                        store_rec<NW>(R + (size_t)z * NW, key);
-                        rcnt[z] = kc;
-                    }
-                }
-                dres[b] = (uint16_t)d;
-            }
-        }
-        if (bad) s_flag = 1;
-        __syncthreads();
-        if (s_flag) {
-            // exact fallback: LSD radix over every remaining key bit (scratch = the partner buffer's region), run-length unique
-            if (threadIdx.x == 0) atomicAdd(&stats[1], 1ull);
-            __syncthreads();
-            uint64_t *S = lsd_sort_range<NW>(A, gpartner, n, K, lo, total_bits, lsdcnt, tot);
-            if (S != A) {
-                for (uint32_t i = threadIdx.x; i < n * NW; i += kSThreads) A[i] = S[i];
-                __syncthreads();
-            }
-            uint32_t *heads = rep;      // the sort is done: the 3*kBins u32 of rep/repcnt/rhist (>= CAP+1) are free
-            __syncthreads();
-            const uint32_t per = (n + kSThreads - 1) / kSThreads;
-            const uint32_t i0 = threadIdx.x * per, i1 = min(n, i0 + per);
-            uint32_t nh = 0;
-            for (uint32_t i = i0; i < i1; ++i)
-                if (i == 0 || kmer_word_cmp<NW>(load_rec<NW>(A + (size_t)(i - 1) * NW), load_rec<NW>(A + (size_t)i * NW)) != 0) ++nh;
-            uint32_t hinc = nh;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                uint32_t t = __shfl_up_sync(0xffffffffu, hinc, o);
-                if (lane >= o) hinc += t;
-            }
-            if (lane == 31) tot[warp] = hinc;
-            __syncthreads();
-            uint32_t hb = 0, all = 0;
-            for (int w = 0; w < kSWarps; ++w) { if (w < warp) hb += tot[w]; all += tot[w]; }
-            uint32_t j = hb + hinc - nh;
-            for (uint32_t i = i0; i < i1; ++i)
-                if (i == 0 || kmer_word_cmp<NW>(load_rec<NW>(A + (size_t)(i - 1) * NW), load_rec<NW>(A + (size_t)i * NW)) != 0) heads[j++] = i;
-            if (threadIdx.x == 0) { heads[all] = n; ndist[si] = all; }
-            __syncthreads();
-            for (uint32_t q = threadIdx.x; q < all; q += kSThreads) {
-                const uint32_t h = heads[q];
-                store_rec<NW>(gsrc + (size_t)q * NW, load_rec<NW>(A + (size_t)h * NW));
-                gcnt[q] = heads[q + 1] - h;
-            }
-            __syncthreads();
-            continue;
-        }
-        // ---- P6: output offset of every bin (exclusive scan of 1 + residual-distinct over the occupied bins), then the
-        //          representative's owner writes its bin in key order (representative merged into the sorted residual)
-        uint32_t dsum = 0;
+    for (int q = 0; q < BPT; ++q) {
+        const uint32_t h = (b0 + q < nb) ? rhist[b0 + q] : 0u;
+        loc[q] = h ? h + 1 : 0u;
+        big |= loc[q] > (uint32_t)kBinSlotsMax;
+        sum += loc[q];
+    }
+    if (big) *s_flag = 1;
+    uint32_t rtotal;
+    {
+        uint32_t run = cta_exscan(sum, tot, rtotal);
 #pragma unroll
         for (int q = 0; q < BPT; ++q) {
-            loc[q] = (b0 + q < nb && rep[b0 + q] != 0xffffffffu) ? 1u + dres[b0 + q] : 0u;
-            dsum += loc[q];
+            if (b0 + q < nb) { rstart[b0 + q] = (uint16_t)run; rhist[b0 + q] = (uint16_t)(run + 1); }
+            run += loc[q];
         }
-        uint32_t dinc = dsum;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            uint32_t t = __shfl_up_sync(0xffffffffu, dinc, o);
-            if (lane >= o) dinc += t;
-        }
-        if (lane == 31) tot[warp] = dinc;
-        __syncthreads();
-        uint32_t db = 0, all = 0;
-        for (int w = 0; w < kSWarps; ++w) { if (w < warp) db += tot[w]; all += tot[w]; }
-        {
-            uint32_t run = db + dinc - dsum;
-#pragma unroll
-            for (int q = 0; q < BPT; ++q) {
-                if (b0 + q < nb) rhist[b0 + q] = run;        // rhist is free after P4: output offset of the bin
-                run += loc[q];
-            }
-        }
-        __syncthreads();
+        if (threadIdx.x == kSThreads - 1) rstart[nb] = (uint16_t)rtotal;
+    }
+    __syncthreads();
+    bool bad = rtotal > (uint32_t)kResCap || *s_flag;
+    if (!bad) {
+        // ---- P4: the representative of every bin with residual records takes the bin's first slot, the residual records the rest
 #pragma unroll
         for (int j = 0; j < IPT; ++j) {
             const uint32_t i = threadIdx.x + j * kSThreads;
-            if (i >= n || rep[dig[j]] != i) continue;
-            const uint32_t b = dig[j];
-            const Kmer<NW> rk = load_rec<NW>(A + (size_t)i * NW);
-            const uint32_t rc = repcnt[b] + 1;
-            const uint32_t bs = rstart[b], d = dres[b];
-            uint32_t o = rhist[b];
-            bool placed = false;
-            for (uint32_t z = 0; z < d; ++z) {
-                const Kmer<NW> x = load_rec<NW>(R + (size_t)(bs + z) * NW);
-                if (!placed && kmer_word_cmp<NW>(rk, x) < 0) {
-                    store_rec<NW>(gsrc + (size_t)o * NW, rk); gcnt[o] = rc; ++o; placed = true;
-                }
-                store_rec<NW>(gsrc + (size_t)o * NW, x); gcnt[o] = rcnt[bs + z]; ++o;
-            }
-            if (!placed) { store_rec<NW>(gsrc + (size_t)o * NW, rk); gcnt[o] = rc; }
+            uint32_t pos = 0xffffffffu;
+            if (resmask & (1u << j)) pos = atomic_inc_u16(rhist, dig[j]);
+            else if ((repmask & (1u << j)) && rstart[dig[j] + 1] != rstart[dig[j]]) pos = rstart[dig[j]];
+            if (pos != 0xffffffffu) { store_rec<NW>(R + (size_t)pos * NW, load_rec<NW>(A + (size_t)i * NW)); rbin[pos] = (uint16_t)dig[j]; }
         }
-        if (threadIdx.x == 0) ndist[si] = all;
         __syncthreads();
+        // ---- P5: one thread per slot: first copy of its key in the bin? how many copies? (a residual record never equals the
+        //          representative in its bin's first slot). rcnt = multiplicity at a key's first slot, 0 elsewhere.
+        for (uint32_t p = threadIdx.x; p < rtotal; p += kSThreads) {
+            const uint32_t b = rbin[p], bs = rstart[b], be = rstart[b + 1];
+            uint32_t c = 0;
+            bool head = true;
+            if (p == bs) c = repcnt[b] + 1u;
+            else {
+                const Kmer<NW> key = load_rec<NW>(R + (size_t)p * NW);
+                for (uint32_t z = bs + 1; z < be; ++z) {
+                    if (kmer_eq<NW>(load_rec<NW>(R + (size_t)z * NW), key)) { ++c; head = head && z >= p; }
+                }
+            }
+            rcnt[p] = head ? (uint16_t)c : (uint16_t)0;
+            if (head && atomic_inc_u16(dres, b) >= (uint32_t)kBinDistinctMax) *s_flag = 1;
+        }
+        __syncthreads();
+        bad = *s_flag;
+    }
+    if (bad) {
+        // exact fallback: LSD radix over every remaining key bit (scratch = the partner buffer's region, which no other segment's
+        // records share, the next segment's included), run-length unique
+        if (threadIdx.x == 0) atomicAdd(&stats[1], 1ull);
+        uint64_t *S = lsd_sort_range<NW>(A, gpartner, n, K, lo, total_bits, lsdcnt, tot);
+        if (S != A) {
+            for (uint32_t i = threadIdx.x; i < n * NW; i += kSThreads) A[i] = S[i];
+            __syncthreads();
+        }
+        uint32_t *heads = lsdcnt;   // the sort is done: its counters (>= CAP+1 u32) are free
+        const uint32_t per = (n + kSThreads - 1) / kSThreads;
+        const uint32_t i0 = threadIdx.x * per, i1 = min(n, i0 + per);
+        uint32_t nh = 0;
+        for (uint32_t i = i0; i < i1; ++i)
+            if (i == 0 || kmer_word_cmp<NW>(load_rec<NW>(A + (size_t)(i - 1) * NW), load_rec<NW>(A + (size_t)i * NW)) != 0) ++nh;
+        uint32_t all;
+        uint32_t j = cta_exscan(nh, tot, all);
+        for (uint32_t i = i0; i < i1; ++i)
+            if (i == 0 || kmer_word_cmp<NW>(load_rec<NW>(A + (size_t)(i - 1) * NW), load_rec<NW>(A + (size_t)i * NW)) != 0) heads[j++] = i;
+        if (threadIdx.x == 0) { heads[all] = n; ndist[si] = all; }
+        __syncthreads();
+        for (uint32_t q = threadIdx.x; q < all; q += kSThreads) {
+            const uint32_t h = heads[q];
+            store_rec<NW>(gsrc + (size_t)q * NW, load_rec<NW>(A + (size_t)h * NW));
+            gcnt[q] = heads[q + 1] - h;
+        }
+        return;
+    }
+    // ---- P6: output offset of every bin (exclusive scan of its distinct keys over the occupied bins), then every distinct key
+    //          is stored at its bin's offset + its rank in the bin
+    uint32_t dsum = 0;
+#pragma unroll
+    for (int q = 0; q < BPT; ++q) {
+        loc[q] = (b0 + q < nb && rep[b0 + q] != 0xffffu) ? (dres[b0 + q] ? (uint32_t)dres[b0 + q] : 1u) : 0u;
+        dsum += loc[q];
+    }
+    uint32_t all;
+    {
+        uint32_t run = cta_exscan(dsum, tot, all);
+#pragma unroll
+        for (int q = 0; q < BPT; ++q) {
+            if (b0 + q < nb) rhist[b0 + q] = (uint16_t)run;      // rhist is free after P4: output offset of the bin
+            run += loc[q];
+        }
+    }
+    __syncthreads();
+    // a bin without residual slots: its representative is its only key
+#pragma unroll
+    for (int j = 0; j < IPT; ++j) {
+        if (!(repmask & (1u << j)) || rstart[dig[j] + 1] != rstart[dig[j]]) continue;
+        const uint32_t i = threadIdx.x + j * kSThreads, o = rhist[dig[j]];
+        store_rec<NW>(gsrc + (size_t)o * NW, load_rec<NW>(A + (size_t)i * NW));
+        gcnt[o] = repcnt[dig[j]] + 1u;
+    }
+    // a key's first slot: rank among the first slots of its bin
+    for (uint32_t p = threadIdx.x; p < rtotal; p += kSThreads) {
+        const uint32_t c = rcnt[p];
+        if (!c) continue;
+        const uint32_t b = rbin[p], bs = rstart[b], be = rstart[b + 1];
+        const Kmer<NW> key = load_rec<NW>(R + (size_t)p * NW);
+        uint32_t o = rhist[b];
+        for (uint32_t z = bs; z < be; ++z)
+            if (rcnt[z] && kmer_word_cmp<NW>(load_rec<NW>(R + (size_t)z * NW), key) < 0) ++o;
+        store_rec<NW>(gsrc + (size_t)o * NW, key);
+        gcnt[o] = c;
+    }
+    if (threadIdx.x == 0) ndist[si] = all;
+}
+
+template <int NW, int kBinBits, int CAP>
+__global__ void __launch_bounds__(kSThreads, 2) local_sort3_k(const Seg *__restrict__ segs, uint64_t nsegs, int K, uint64_t *__restrict__ buf0,
+                                                             uint64_t *__restrict__ buf1, uint32_t *__restrict__ ndist,
+                                                             unsigned long long *__restrict__ work_counter, unsigned long long *__restrict__ stats) {
+    constexpr int kBins = 1 << kBinBits;
+    static_assert(kBins % kSThreads == 0, "bins: a multiple of the CTA size");
+    static_assert(CAP % kSThreads == 0 && CAP <= SortCfg<NW>::CAP && CAP < 0xffff, "segment capacity: a multiple of the CTA size, at most the default");
+    static_assert((size_t)kResCap * NW * 8 + (size_t)4 * kBins * 2 >= (size_t)4 * (CAP + 1) && (size_t)kResCap * NW * 8 + (size_t)4 * kBins * 2 >= (size_t)4 * 256 * kSWarps,
+                  "the residual records and the bin tables double as scratch of the LSD fallback");
+    extern __shared__ __align__(16) uint64_t sm64[];
+    uint64_t *Abuf = sm64;                                // 2 x CAP*NW: the segment being sorted, the next one arriving
+    uint64_t *R = Abuf + (size_t)2 * CAP * NW;            // kResCap*NW residual slots, grouped by bin
+    uint16_t *rep = reinterpret_cast<uint16_t *>(R + (size_t)kResCap * NW);   // 4 x kBins + kBins+2, see sort_segment
+    uint16_t *rcnt = rep + 5 * kBins + 2;                 // kResCap multiplicity at a key's first slot
+    uint16_t *rbin = rcnt + kResCap;                      // kResCap bin of the slot
+    uint32_t *lsdcnt = reinterpret_cast<uint32_t *>(R);   // fallback only
+    __shared__ uint32_t tot[kSWarps];
+    __shared__ unsigned long long s_claim[2];
+    __shared__ int s_flag;
+    // claims run two segments ahead: s_claim[(it + 1) & 1] holds the segment after the current one when iteration `it` starts,
+    // and thread 0 stores the claim of the one after that into s_claim[it & 1] at the end of the iteration
+    if (threadIdx.x == 0) s_claim[0] = atomicAdd(work_counter, 1ull);
+    __syncthreads();
+    uint64_t si = s_claim[0];
+    if (threadIdx.x == 0) s_claim[1] = atomicAdd(work_counter, 1ull);
+    Seg s = {0, 0, 0, 0};
+    if (si < nsegs) {
+        s = segs[si];
+        prefetch_segment<NW, CAP>(Abuf, ((s.bb & 1) ? buf1 : buf0) + s.start * NW, s.len);
+    }
+    cp_async_commit();
+    for (uint32_t it = 0;; ++it) {
+        cp_async_wait_all();
+        __syncthreads();              // segment si is in A; every thread is done with the other buffer and with s_claim[(it + 1) & 1]'s writer
+        if (si >= nsegs) return;      // claims only grow: no copy was issued after this one
+        uint64_t *A = Abuf + (size_t)(it & 1) * CAP * NW;
+        const uint64_t ni = s_claim[(it + 1) & 1];
+        Seg ns = {0, 0, 0, 0};
+        if (ni < nsegs) {
+            ns = segs[ni];
+            // the next segment's records [start, start+len) are disjoint from this segment's in both buffers, so the sort's
+            // scratch (partner region) and output (source region) below never touch what the copy reads
+            prefetch_segment<NW, CAP>(Abuf + (size_t)((it + 1) & 1) * CAP * NW, ((ns.bb & 1) ? buf1 : buf0) + ns.start * NW, ns.len);
+        }
+        cp_async_commit();
+        unsigned long long claim = 0;
+        if (threadIdx.x == 0) claim = atomicAdd(work_counter, 1ull);
+        sort_segment<NW, kBinBits, CAP>(si, s, A, R, rep, rcnt, rbin, lsdcnt, tot, &s_flag, K, buf0, buf1, ndist, stats);
+        if (threadIdx.x == 0) s_claim[it & 1] = claim;
+        si = ni;
+        s = ns;
     }
 }
 
@@ -1547,9 +1590,7 @@ static void sort_pass(Ctx *ctx, int K, DArr<uint64_t> &X, DArr<uint64_t> &Y, con
             if (grid < 1) grid = 1;
             kernel<<<grid, kSThreads, smem, st>>>(segs.p, nsegs, K, X.p, Y.p, ndist.p, wcounter.p, stats.p);
         };
-        constexpr int bins = 1 << kSortBinBits;
-        launch(local_sort3_k<NW, kSortBinBits, CAP>, (size_t)(CAP + kResCap) * NW * sizeof(uint64_t) + (size_t)3 * bins * sizeof(uint32_t) +
-                                                         ((size_t)2 * bins + 2 + kResCap) * sizeof(uint16_t) + 16);
+        launch(local_sort3_k<NW, kSortBinBits, CAP>, SortSmem<NW, kSortBinBits, CAP>::bytes);
         ctx->launches++;
         SG_CUDA(cudaGetLastError());
     }
