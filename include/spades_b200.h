@@ -49,7 +49,7 @@ extern "C" {
 #endif
 
 typedef struct sgpu_ctx sgpu_ctx;
-typedef struct sgpu_kset sgpu_kset;     /* a counted k-mer set resident in HBM (== KMerDiskStorage contents) */
+typedef struct sgpu_kset sgpu_kset;     /* a counted k-mer set resident in HBM, or in host memory (== KMerDiskStorage contents) */
 typedef struct sgpu_mphf sgpu_mphf;     /* a boomphf-compatible KMerIndex resident in HBM */
 typedef struct sgpu_graph sgpu_graph;   /* masks + coverage + unitigs + link records */
 
@@ -61,6 +61,10 @@ typedef struct sgpu_config {
 } sgpu_config;
 
 enum { SGPU_CANONICAL = 0, SGPU_ALL_WINDOWS = 1 };
+/* OR-ed into the mode of sgpu_count / sgpu_dist_begin: the k-mer set is returned in pinned host memory instead of HBM, so a set
+ * larger than the device can be counted. Each pass's result is copied to the host while the next pass runs; only the pass in
+ * flight keeps its result on the device. */
+#define SGPU_RESULT_ON_HOST 0x100
 
 enum {
     SGPU_OK = 0, SGPU_EINVAL = 2, SGPU_ENODEV = 3, SGPU_ENOMEM = 4, SGPU_ECUDA = 5, SGPU_EINTERNAL = 6, SGPU_EUNSUPPORTED = 7,
@@ -84,6 +88,9 @@ typedef struct sgpu_times {
     uint64_t refine_splits_later;   /* segments the later refinement rounds added */
     uint64_t sort_lsd_fallbacks;    /* local-sort segments that took the exact LSD fallback */
     uint64_t sort_oversize_equal;   /* segments longer than the local-sort capacity whose records are all equal */
+    /* a count with SGPU_RESULT_ON_HOST (last sgpu_count / sgpu_dist_begin .. sgpu_dist_end) */
+    uint64_t result_d2h_bytes;      /* bytes of records and multiplicities copied to host memory */
+    float result_d2h_wait_ms;       /* host time the count spent waiting for those copies */
 } sgpu_times;
 
 int sgpu_create(const sgpu_config *cfg, sgpu_ctx **out);
@@ -152,6 +159,9 @@ int64_t sgpu_text_index_fastx(const char *text, uint64_t text_bytes, uint64_t *s
 /* sgpu_reads_append_packed of a whole batch */
 int sgpu_reads_append_batch(sgpu_ctx *ctx, const sgpu_read_batch *b);
 
+/* mode: SGPU_CANONICAL or SGPU_ALL_WINDOWS, optionally | SGPU_RESULT_ON_HOST. A host set answers every sgpu_kset_* call and
+ * sgpu_mphf_build exactly as a device set does (the index is built chunk by chunk, uploading each chunk while the one before is
+ * placed); sgpu_kmers_from_kpomers and the sgpu_graph_build* calls need their sets in HBM and return SGPU_EUNSUPPORTED for it. */
 int sgpu_count(sgpu_ctx *ctx, int K, int num_buckets, int mode, sgpu_kset **out);
 int sgpu_kmers_from_kpomers(sgpu_ctx *ctx, const sgpu_kset *kpomers, int num_buckets, sgpu_kset **out);
 
@@ -159,6 +169,7 @@ int64_t sgpu_kset_size(const sgpu_kset *s);
 int sgpu_kset_k(const sgpu_kset *s);
 int sgpu_kset_num_buckets(const sgpu_kset *s);
 int sgpu_kset_record_bytes(const sgpu_kset *s);                       /* KMerCounter::kmer_size(): 8*ceil(K/32) */
+int sgpu_kset_on_host(const sgpu_kset *s);                            /* 1: the set lives in host memory, 0: in HBM, -1: NULL */
 int sgpu_kset_bucket_sizes(const sgpu_kset *s, int64_t *out);         /* num_buckets entries */
 /* records [first, first+n) of final_kmers order (KMerDiskStorage::merge, kmer_index_builder.hpp:190-203) to host memory */
 /* order-independent checksums computed on the device: out4 = { number of records, weighted sum of all record words, xor of

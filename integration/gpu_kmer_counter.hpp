@@ -35,8 +35,12 @@ class GpuKMerDiskCounterT : public KMerCounter<Seq> {
     // mode: SGPU_ALL_WINDOWS = every window and its reverse complement (spades-kmercount's splitter, kmercount.cpp:48-122; BayesHammer's
     //                          BufferFiller pushes seq and !seq, hammer/kmer_data.cpp:75-82),
     //       SGPU_CANONICAL   = DeBruijnReadKMerSplitter with the IsMinimal filter (kmer_splitters.hpp:112-136, storing_traits.hpp:92-101)
-    GpuKMerDiskCounterT(fs::TmpDir work_dir, unsigned K, sgpu_ctx *ctx, int mode)
-            : KMerCounter<Seq>(K), work_dir_(work_dir), ctx_(ctx), mode_(mode) { check(sgpu_reads_clear(ctx_)); }
+    // result_on_host: the counted set is kept in pinned host memory (SGPU_RESULT_ON_HOST), so it may be larger than the device; the
+    // bucket files and the GPU index are made from it as from a device set, the graph phases need a device set
+    GpuKMerDiskCounterT(fs::TmpDir work_dir, unsigned K, sgpu_ctx *ctx, int mode, bool result_on_host = false)
+            : KMerCounter<Seq>(K), work_dir_(work_dir), ctx_(ctx), mode_(result_on_host ? (mode | SGPU_RESULT_ON_HOST) : mode) {
+        check(sgpu_reads_clear(ctx_));
+    }
     ~GpuKMerDiskCounterT() override { if (last_) sgpu_kset_free(last_); }
 
     // the payload of the reference's binary read records: Sequence::data(), ceil(size/32) words (sequence.hpp:808-830). Reads are
@@ -125,7 +129,7 @@ class GpuKMerDiskCounterT : public KMerCounter<Seq> {
         return storage;
     }
 
-    const sgpu_kset *device_set() const { return last_; }      // the same set, still resident in HBM, for the GPU index / graph phases
+    const sgpu_kset *device_set() const { return last_; }      // the same set, still resident (HBM or host memory), for the GPU index / graph phases
 
   private:
     void check(int rc) const { if (rc) FATAL_ERROR("spades_b200: " << sgpu_last_error(ctx_)); }          // logger.hpp:185-261 convention

@@ -2,7 +2,10 @@
 // swapped for the GPU adapter: REFERENCE host code (KMerDiskStorage, KMerIndexBuilder, KMerIndex, RtSeq, Sequence, fs::TmpDir,
 // logger -- all unmodified, compiled where they lie) calling hand-written sm_90a CUDA through the C ABI.
 //
-//   spades_kmercount_gpu <reads.txt> <k> <workdir> [num_buckets=16]
+//   spades_kmercount_gpu <reads.txt> <k> <workdir> [num_buckets=16] [--host-result]
+//
+// --host-result: the count's result stays in host memory (SGPU_RESULT_ON_HOST) instead of HBM; the tool needs only final_kmers,
+// so its result may be larger than the device.
 //
 // reads: FASTA / FASTQ, plain or gzip (parsed by the library's ingest with the original tool's semantics: kseq records +
 // LongestValid), or one ACGT read per line (ref_probe's format). Output: <workdir>/final_kmers, byte-identical to the original
@@ -93,7 +96,9 @@ static int hammer_client_check(sgpu_ctx *ctx, const std::vector<std::string> &re
 }
 
 int main(int argc, char **argv) {
-    if (argc < 4) { fprintf(stderr, "usage: %s reads.txt k workdir [num_buckets]\n", argv[0]); return 2; }
+    const bool host_result = argc > 4 && std::string(argv[argc - 1]) == "--host-result";
+    if (host_result) --argc;
+    if (argc < 4) { fprintf(stderr, "usage: %s reads.txt k workdir [num_buckets] [--host-result]\n", argv[0]); return 2; }
     const std::string reads_path = argv[1];
     const unsigned K = (unsigned)atoi(argv[2]);
     const std::filesystem::path workdir = argv[3];
@@ -111,7 +116,7 @@ int main(int argc, char **argv) {
     typedef kmers::KMerIndex<kmers::kmer_index_traits<RtSeq>> Index;
     int bad = 0;
     {
-        kmers::GpuKMerDiskCounter counter(fs::tmp::make_temp_dir(workdir, "kmer_counter"), K, ctx, SGPU_ALL_WINDOWS);
+        kmers::GpuKMerDiskCounter counter(fs::tmp::make_temp_dir(workdir, "kmer_counter"), K, ctx, SGPU_ALL_WINDOWS, host_result);
         std::vector<std::string> plain_reads;                                  // kept for the Seq<21> client check below (K == 21 only)
         {
             std::ifstream is(reads_path, std::ios::binary);
@@ -126,7 +131,7 @@ int main(int argc, char **argv) {
                     if (!line.empty()) { counter.AddRead(Sequence(line)); if (K == 21) plain_reads.push_back(line); }
             }
         }
-        auto storage = counter.Count(B, 1);                         // KMerDiskStorage<RtSeq>, buckets written from HBM
+        auto storage = counter.Count(B, 1);                         // KMerDiskStorage<RtSeq>, buckets written from HBM (or host memory)
         const size_t total = storage.total_kmers();
         if (!storage.is_unique_and_sorted()) { ERROR("GPU-written buckets are not sorted/unique"); ++bad; }
 

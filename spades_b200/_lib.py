@@ -17,7 +17,7 @@ SYMBOLS = [
     "sgpu_read_batch_words", "sgpu_read_batch_offs", "sgpu_read_batch_lens", "sgpu_read_batch_stats", "sgpu_read_batch_error", "sgpu_read_batch_free",
     "sgpu_reads_append_batch",
     "sgpu_count", "sgpu_kmers_from_kpomers",
-    "sgpu_kset_size", "sgpu_kset_k", "sgpu_kset_num_buckets", "sgpu_kset_record_bytes", "sgpu_kset_bucket_sizes",
+    "sgpu_kset_size", "sgpu_kset_k", "sgpu_kset_num_buckets", "sgpu_kset_record_bytes", "sgpu_kset_on_host", "sgpu_kset_bucket_sizes",
     "sgpu_kset_checksum", "sgpu_kset_download_keys", "sgpu_kset_download_counts", "sgpu_kset_write_buckets", "sgpu_kset_write_final", "sgpu_kset_free",
     "sgpu_mphf_build", "sgpu_mphf_serialized_size", "sgpu_mphf_serialize", "sgpu_mphf_lookup", "sgpu_mphf_free",
     "sgpu_graph_build", "sgpu_graph_build_ex", "sgpu_graph_build_opts", "sgpu_graph_at_clipper_stats", "sgpu_graph_tip_clipper_stats", "sgpu_graph_masks", "sgpu_graph_coverage", "sgpu_graph_histogram", "sgpu_graph_num_unitigs",
@@ -45,7 +45,7 @@ class SgpuTimes(C.Structure):
                 ("instances", C.c_uint64), ("passes", C.c_uint64), ("launches", C.c_uint64), ("peak_bytes", C.c_uint64), ("cached_bytes", C.c_uint64),
                 ("level_a_key_bits", C.c_uint64), ("level_a_scatters", C.c_uint64), ("refine_rounds_max", C.c_uint64),
                 ("refine_splits_round0", C.c_uint64), ("refine_splits_later", C.c_uint64), ("sort_lsd_fallbacks", C.c_uint64),
-                ("sort_oversize_equal", C.c_uint64)]
+                ("sort_oversize_equal", C.c_uint64), ("result_d2h_bytes", C.c_uint64), ("result_d2h_wait_ms", C.c_float)]
 
 
 _lib = None
@@ -93,6 +93,7 @@ def load():
     L.sgpu_kset_k.restype = i32; L.sgpu_kset_k.argtypes = [vp]
     L.sgpu_kset_num_buckets.restype = i32; L.sgpu_kset_num_buckets.argtypes = [vp]
     L.sgpu_kset_record_bytes.restype = i32; L.sgpu_kset_record_bytes.argtypes = [vp]
+    L.sgpu_kset_on_host.restype = i32; L.sgpu_kset_on_host.argtypes = [vp]
     L.sgpu_kset_bucket_sizes.restype = i32; L.sgpu_kset_bucket_sizes.argtypes = [vp, vp]
     L.sgpu_kset_checksum.restype = i32; L.sgpu_kset_checksum.argtypes = [vp, vp]
     L.sgpu_kset_download_keys.restype = i32; L.sgpu_kset_download_keys.argtypes = [vp, i64, i64, vp]

@@ -21,6 +21,7 @@ static void ctx_teardown(sgpu_ctx *ctx) {
     cudaSetDevice(ctx->c.device);
     ctx->c.r_words.release(); ctx->c.r_offs.release(); ctx->c.r_lens.release();
     ctx->c.pool_trim();
+    if (ctx->c.copy) cudaStreamDestroy(ctx->c.copy);
     if (ctx->c.stream && ctx->own_stream) cudaStreamDestroy(ctx->c.stream);
     delete ctx;
 }
@@ -84,6 +85,7 @@ int sgpu_get_times(const sgpu_ctx *ctx, sgpu_times *out) {
     out->level_a_key_bits = t.level_a_key_bits; out->level_a_scatters = t.level_a_scatters;
     out->refine_rounds_max = t.refine_rounds_max; out->refine_splits_round0 = t.refine_splits_round0; out->refine_splits_later = t.refine_splits_later;
     out->sort_lsd_fallbacks = t.sort_lsd_fallbacks; out->sort_oversize_equal = t.sort_oversize_equal;
+    out->result_d2h_bytes = t.result_d2h_bytes; out->result_d2h_wait_ms = t.result_d2h_wait;
     return SGPU_OK;
 }
 
@@ -178,9 +180,11 @@ int sgpu_count(sgpu_ctx *ctx, int K, int num_buckets, int mode, sgpu_kset **out)
     *out = nullptr;
     Ctx *c = &ctx->c;
     API_TRY(c, {
+        const bool on_host = (mode & SGPU_RESULT_ON_HOST) != 0;
+        mode &= ~SGPU_RESULT_ON_HOST;
         SG_CHECK(mode == SGPU_CANONICAL || mode == SGPU_ALL_WINDOWS, SGPU_EINVAL, "bad mode");
         SG_CUDA(cudaSetDevice(c->device));
-        KSet *s = count_from_reads(c, K, num_buckets, mode);
+        KSet *s = count_from_reads(c, K, num_buckets, mode, on_host);
         *out = new sgpu_kset{s};
         child_add(c);
     })
@@ -202,6 +206,7 @@ int64_t sgpu_kset_size(const sgpu_kset *s) { return s ? s->s->n : -1; }
 int sgpu_kset_k(const sgpu_kset *s) { return s ? s->s->K : -1; }
 int sgpu_kset_num_buckets(const sgpu_kset *s) { return s ? s->s->B : -1; }
 int sgpu_kset_record_bytes(const sgpu_kset *s) { return s ? 8 * s->s->nw : -1; }
+int sgpu_kset_on_host(const sgpu_kset *s) { return s ? (s->s->on_host ? 1 : 0) : -1; }
 int sgpu_kset_bucket_sizes(const sgpu_kset *s, int64_t *out) {
     if (!s || !out) return SGPU_EINVAL;
     for (int b = 0; b < s->s->B; ++b) out[b] = s->s->bsz[b];
@@ -209,6 +214,10 @@ int sgpu_kset_bucket_sizes(const sgpu_kset *s, int64_t *out) {
 }
 
 }  // extern "C"
+
+// where a chunk's records live: pinned host memory for a host set, HBM otherwise
+static const uint64_t *chunk_keys(const Chunk &ch) { return ch.h_keys.p ? ch.h_keys.p : ch.keys.p; }
+static const uint32_t *chunk_counts(const Chunk &ch) { return ch.h_counts.p ? ch.h_counts.p : ch.counts.p; }
 
 template <class T, class Get>
 static void download_range(const KSet *ks, int64_t first, int64_t n, T *out, size_t per, Get get) {
@@ -219,8 +228,11 @@ static void download_range(const KSet *ks, int64_t first, int64_t n, T *out, siz
     for (const Chunk &ch : ks->chunks) {
         const int64_t lo = std::max(first, ch.first), hi = std::min(first + n, ch.first + ch.n);
         if (lo >= hi) continue;
-        SG_CUDA(cudaMemcpyAsync(out + (size_t)(lo - first) * per, get(ch) + (size_t)(lo - ch.first) * per, (size_t)(hi - lo) * per * sizeof(T),
-                                cudaMemcpyDeviceToHost, c->stream));
+        T *dst = out + (size_t)(lo - first) * per;
+        const T *src = get(ch) + (size_t)(lo - ch.first) * per;
+        const size_t bytes = (size_t)(hi - lo) * per * sizeof(T);
+        if (ks->on_host) memcpy(dst, src, bytes);
+        else SG_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->stream));
         done += hi - lo;
     }
     SG_CUDA(cudaStreamSynchronize(c->stream));
@@ -234,7 +246,7 @@ static void write_range(const KSet *ks, int64_t first, int64_t n, FILE *f) {
     for (int64_t o = 0; o < n; o += step) {
         const int64_t m = std::min(step, n - o);
         buf.resize((size_t)m * W);
-        download_range<uint64_t>(ks, first + o, m, buf.data(), W, [](const Chunk &ch) { return ch.keys.p; });
+        download_range<uint64_t>(ks, first + o, m, buf.data(), W, chunk_keys);
         SG_CHECK(fwrite(buf.data(), 8 * W, (size_t)m, f) == (size_t)m, SGPU_EIO, "short write");
     }
 }
@@ -249,14 +261,14 @@ int sgpu_kset_checksum(const sgpu_kset *s, uint64_t *out4) {
 int sgpu_kset_download_keys(const sgpu_kset *s, int64_t first, int64_t n, uint64_t *out) {
     if (!s || (n && !out)) return SGPU_EINVAL;
     Ctx *c = s->s->ctx;
-    API_TRY(c, { download_range<uint64_t>(s->s, first, n, out, (size_t)s->s->nw, [](const Chunk &ch) { return ch.keys.p; }); })
+    API_TRY(c, { download_range<uint64_t>(s->s, first, n, out, (size_t)s->s->nw, chunk_keys); })
 }
 int sgpu_kset_download_counts(const sgpu_kset *s, int64_t first, int64_t n, uint32_t *out) {
     if (!s || (n && !out)) return SGPU_EINVAL;
     Ctx *c = s->s->ctx;
     API_TRY(c, {
         SG_CHECK(s->s->has_counts, SGPU_EINVAL, "this k-mer set carries no multiplicities");
-        download_range<uint32_t>(s->s, first, n, out, 1, [](const Chunk &ch) { return ch.counts.p; });
+        download_range<uint32_t>(s->s, first, n, out, 1, chunk_counts);
     })
 }
 
@@ -320,12 +332,23 @@ void sgpu_mphf_free(sgpu_mphf *m) {
     delete m;
 }
 
+}  // extern "C"
+
+// the graph kernels read both k-mer sets from HBM
+static void check_device_sets(const sgpu_kset *kpomers, const sgpu_kset *kmers) {
+    SG_CHECK(!kpomers->s->on_host && !kmers->s->on_host, SGPU_EUNSUPPORTED,
+             "the graph is built from k-mer sets in device memory; this one lives in host memory (SGPU_RESULT_ON_HOST)");
+}
+
+extern "C" {
+
 int sgpu_graph_build(sgpu_ctx *ctx, const sgpu_kset *kpomers, const sgpu_kset *kmers, const sgpu_mphf *kmer_index, const sgpu_mphf *kpomer_index,
                      int keep_perfect_loops, sgpu_graph **out) {
     if (!ctx || !kpomers || !kmers || !kmer_index || !out) return SGPU_EINVAL;
     *out = nullptr;
     Ctx *c = &ctx->c;
     API_TRY(c, {
+        check_device_sets(kpomers, kmers);
         SG_CUDA(cudaSetDevice(c->device));
         GraphOptions opt;
         opt.keep_perfect_loops = keep_perfect_loops != 0;
@@ -340,6 +363,7 @@ int sgpu_graph_build_ex(sgpu_ctx *ctx, const sgpu_kset *kpomers, const sgpu_kset
     *out = nullptr;
     Ctx *c = &ctx->c;
     API_TRY(c, {
+        check_device_sets(kpomers, kmers);
         SG_CUDA(cudaSetDevice(c->device));
         GraphOptions opt;
         opt.keep_perfect_loops = keep_perfect_loops != 0;
@@ -356,6 +380,7 @@ int sgpu_graph_build_opts(sgpu_ctx *ctx, const sgpu_kset *kpomers, const sgpu_ks
     Ctx *c = &ctx->c;
     API_TRY(c, {
         SG_CHECK(!o->early_at_clipper || (o->at_ratio > 0.0 && o->at_ratio <= 1.0 && o->at_max_length >= 1), SGPU_EINVAL, "bad A/T clipper parameters");
+        check_device_sets(kpomers, kmers);
         SG_CUDA(cudaSetDevice(c->device));
         GraphOptions opt;
         opt.keep_perfect_loops = o->keep_perfect_loops != 0;
@@ -511,7 +536,8 @@ int sgpu_dist_begin(sgpu_ctx *ctx, int K, int num_buckets, int mode, int world, 
     Ctx *c = &ctx->c;
     API_TRY(c, {
         SG_CUDA(cudaSetDevice(c->device));
-        DistState *d = dist_begin(c, K, num_buckets, mode, world, rank);
+        const bool on_host = (mode & SGPU_RESULT_ON_HOST) != 0;
+        DistState *d = dist_begin(c, K, num_buckets, mode & ~SGPU_RESULT_ON_HOST, world, rank, on_host);
         *out = new sgpu_dist{d, c};
         child_add(c);
     })

@@ -19,6 +19,8 @@
 #include <time.h>
 
 #include <algorithm>
+#include <chrono>
+#include <memory>
 
 #include "sgpu_internal.h"
 
@@ -1515,12 +1517,59 @@ static const int kLevelAMaxParts = 8192;      // partitions one level-A launch c
 // mean segment length the refinement aims for: 3/4 of the local-sort capacity
 template <int NW> static uint32_t sort_target() { return (uint32_t)SortCfg<NW>::CAP * 6 / 8; }
 
+// Copies a count's finished chunks to pinned host memory behind the next pass (SGPU_RESULT_ON_HOST). One chunk is in flight at
+// a time, on the context's copy stream. Its device arrays stay allocated until the copy has completed: the arena is host
+// bookkeeping, so a block released early could be handed to the next pass's buffers while the copy still reads it.
+struct ResultSink {
+    Ctx *ctx;
+    KSet *ks;
+    int inflight = -1;                       // index in ks->chunks of the chunk being copied
+    cudaEvent_t compacted = nullptr, copied = nullptr;
+    ResultSink(Ctx *c, KSet *s) : ctx(c), ks(s) {
+        SG_CUDA(cudaEventCreateWithFlags(&compacted, cudaEventDisableTiming));
+        SG_CUDA(cudaEventCreateWithFlags(&copied, cudaEventDisableTiming));
+    }
+    ~ResultSink() {
+        if (inflight >= 0) cudaEventSynchronize(copied);
+        cudaEventDestroy(compacted); cudaEventDestroy(copied);
+    }
+    ResultSink(const ResultSink &) = delete;
+    ResultSink &operator=(const ResultSink &) = delete;
+    // the last chunk of the set has just been compacted on ctx->stream: start its copy and return
+    void push() {
+        drain();
+        Chunk &ch = ks->chunks.back();
+        const size_t kb = (size_t)ch.n * ks->nw * 8, cb = ks->has_counts ? (size_t)ch.n * 4 : 0;
+        ch.h_keys.alloc((size_t)ch.n * ks->nw);
+        if (ks->has_counts) ch.h_counts.alloc((size_t)ch.n);
+        cudaStream_t cs = ctx->copy_stream();
+        SG_CUDA(cudaEventRecord(compacted, ctx->stream));
+        SG_CUDA(cudaStreamWaitEvent(cs, compacted, 0));
+        if (kb) SG_CUDA(cudaMemcpyAsync(ch.h_keys.p, ch.keys.p, kb, cudaMemcpyDeviceToHost, cs));
+        if (cb) SG_CUDA(cudaMemcpyAsync(ch.h_counts.p, ch.counts.p, cb, cudaMemcpyDeviceToHost, cs));
+        SG_CUDA(cudaEventRecord(copied, cs));
+        ctx->times.result_d2h_bytes += kb + cb;
+        inflight = (int)ks->chunks.size() - 1;
+    }
+    // wait for the chunk in flight, then give its device arrays back
+    void drain() {
+        if (inflight < 0) return;
+        const auto t0 = std::chrono::steady_clock::now();
+        SG_CUDA(cudaEventSynchronize(copied));
+        ctx->times.result_d2h_wait += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+        Chunk &ch = ks->chunks[(size_t)inflight];
+        ch.keys.release(); ch.counts.release();
+        inflight = -1;
+    }
+};
+
 // refinement + local sort + compaction of one pass: X holds the level-A output (CTA-major pieces when `pieces` is given, else
-// partition-major with the given starts/totals), Y is the ping-pong partner of the same size.
+// partition-major with the given starts/totals), Y is the ping-pong partner of the same size. With a sink, the previous pass's
+// chunk is drained just before this pass allocates its own output.
 template <int NW>
 static void sort_pass(Ctx *ctx, int K, DArr<uint64_t> &X, DArr<uint64_t> &Y, const uint64_t *part_start_p, const uint64_t *part_total_p, uint32_t PA,
                       int rA_, uint32_t b_lo, int b_hi, int64_t first, bool want_counts, bool double_selfrc, unsigned long long *d_bsz_p, Chunk &ch_out,
-                      Timer &tm, Trace &tr, const Pieces *pieces = nullptr) {
+                      Timer &tm, Trace &tr, const Pieces *pieces = nullptr, ResultSink *sink = nullptr) {
     constexpr int CAP = SortCfg<NW>::CAP;
     const int total_bits = 2 * K;
     cudaStream_t st = ctx->stream;
@@ -1607,6 +1656,7 @@ static void sort_pass(Ctx *ctx, int K, DArr<uint64_t> &X, DArr<uint64_t> &Y, con
     ctx->times.sort_lsd_fallbacks += h_stats[1];
     ctx->times.sort_oversize_equal += h_stats[2];
     // ---- compaction into the dense chunk
+    if (sink) sink->drain();
     Chunk ch;
     ch.n = (int64_t)D; ch.b_lo = (int)b_lo; ch.b_hi = b_hi; ch.first = first;
     ch.keys.alloc(ctx, (size_t)D * NW + 2, true);
@@ -1802,7 +1852,8 @@ static void levelA_scatter(LevelAJob<NW, Src, BOTH> &job, int b_lo, int b_hi, ui
 static double pass_bytes_needed(uint64_t recs, size_t W) { return (double)recs * W * 2.0 + (double)recs * (W + 4) * 0.6 + (64 << 20); }
 
 template <int NW, bool BOTH, class Src>
-static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, int B, bool want_counts, bool double_selfrc, uint64_t est_records, KSet *out) {
+static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, int B, bool want_counts, bool double_selfrc, uint64_t est_records, KSet *out,
+                      ResultSink *sink = nullptr) {
     const int total_bits = 2 * K;
     const size_t W = 8 * NW;
     cudaStream_t st = ctx->stream;
@@ -1841,16 +1892,18 @@ static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, int B, bool
         uint64_t pass_target = total_records;
         bool capped = false;
         {
-            double lim_sim = (double)current_limit();
+            // a set that goes to host memory keeps only the previous pass's output on the device, while it is copied
+            double lim_sim = (double)current_limit(), inflight = 0;
             int npass_sim = 0, b = job.s_lo;
             while (b < job.s_hi) {
                 uint64_t I = 0; const int b0 = b;
                 while (b < job.s_hi) {
                     const uint64_t ib = job.bucket_records(b);
-                    if (b > b0 && pass_bytes_needed(I + ib, W) > lim_sim) break;
+                    if (b > b0 && pass_bytes_needed(I + ib, W) + inflight > lim_sim) break;
                     I += ib; ++b;
                 }
-                lim_sim -= (double)I * (W + 4) * 0.5;            // this pass's output stays resident
+                if (sink) inflight = (double)I * (W + 4) * 0.5;
+                else lim_sim -= (double)I * (W + 4) * 0.5;     // this pass's output stays resident
                 ++npass_sim;
             }
             capped = npass_sim > share;
@@ -1886,12 +1939,15 @@ static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, int B, bool
             Pieces pcs;
             levelA_scatter(job, b_lo, b_hi, I, total_records, X.p, pbase.p, pcs, tm, tr);
             Chunk ch;
-            sort_pass<NW>(ctx, K, X, Y, part_start.p, part_total.p, PA, rA, (uint32_t)b_lo, b_hi, first, want_counts, double_selfrc, d_bsz.p, ch, tm, tr, &pcs);
+            sort_pass<NW>(ctx, K, X, Y, part_start.p, part_total.p, PA, rA, (uint32_t)b_lo, b_hi, first, want_counts, double_selfrc, d_bsz.p, ch, tm, tr, &pcs,
+                          sink);
             first += ch.n;
             out->chunks.push_back(std::move(ch));
+            if (sink) sink->push();
             b_lo = b_hi;
         }
     }
+    if (sink) sink->drain();
     std::vector<unsigned long long> hb(B);
     SG_CUDA(cudaMemcpyAsync(hb.data(), d_bsz.p, B * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     SG_CUDA(cudaStreamSynchronize(st));
@@ -1932,28 +1988,29 @@ static ReadsSrc reads_source(Ctx *ctx, int K) {
 }
 
 template <int NW>
-static KSet *count_reads_nw(Ctx *ctx, int K, int B, int mode) {
+static KSet *count_reads_nw(Ctx *ctx, int K, int B, int mode, bool on_host) {
     ensure_reads_on_device(ctx);
     KSet *ks = new KSet();
-    ks->ctx = ctx; ks->K = K; ks->nw = NW; ks->B = B; ks->has_counts = (mode == kCanonical);
+    ks->ctx = ctx; ks->K = K; ks->nw = NW; ks->B = B; ks->has_counts = (mode == kCanonical); ks->on_host = on_host;
     try {
+        std::unique_ptr<ResultSink> sink(on_host ? new ResultSink(ctx, ks) : nullptr);   // gone before `ks` is: no copy outlives the set
         const uint64_t wn = count_windows(ctx, K);
         std::vector<ReadsSrc> srcs{reads_source(ctx, K)};
-        if (mode == kAllWindows) run_count<NW, true>(ctx, srcs, K, B, false, false, wn * 2, ks);
-        else run_count<NW, false>(ctx, srcs, K, B, true, K % 2 == 0, wn, ks);
+        if (mode == kAllWindows) run_count<NW, true>(ctx, srcs, K, B, false, false, wn * 2, ks, sink.get());
+        else run_count<NW, false>(ctx, srcs, K, B, true, K % 2 == 0, wn, ks, sink.get());
     } catch (...) { delete ks; throw; }
     return ks;
 }
 
-KSet *count_from_reads(Ctx *ctx, int K, int B, int mode) {
+KSet *count_from_reads(Ctx *ctx, int K, int B, int mode, bool result_on_host) {
     SG_CHECK(K >= 1 && K <= 128, 2, "K must be in [1,128]");
     SG_CHECK(B >= 1 && B <= (1 << 20), 2, "num_buckets must be in [1, 2^20]");
     ctx->times = PhaseTimes();
     switch (nwords_of(K)) {
-        case 1: return count_reads_nw<1>(ctx, K, B, mode);
-        case 2: return count_reads_nw<2>(ctx, K, B, mode);
-        case 3: return count_reads_nw<3>(ctx, K, B, mode);
-        default: return count_reads_nw<4>(ctx, K, B, mode);
+        case 1: return count_reads_nw<1>(ctx, K, B, mode, result_on_host);
+        case 2: return count_reads_nw<2>(ctx, K, B, mode, result_on_host);
+        case 3: return count_reads_nw<3>(ctx, K, B, mode, result_on_host);
+        default: return count_reads_nw<4>(ctx, K, B, mode, result_on_host);
     }
 }
 
@@ -1975,6 +2032,7 @@ static KSet *kmers_from_kpomers_nw(Ctx *ctx, const KSet *kp, int B) {
 
 KSet *kmers_from_kpomers(Ctx *ctx, const KSet *kp, int B) {
     SG_CHECK(kp->K >= 2, 2, "source k-mers too short");
+    SG_CHECK(!kp->on_host, 7, "the (k+1)-mer set lives in host memory: the k-mers of the (k+1)-mers read it from the device");
     SG_CHECK(B >= 1 && B <= (1 << 20), 2, "num_buckets must be in [1, 2^20]");
     SG_CHECK(kp->nw == nwords_of(kp->K), 2, "unsupported k-mer word combination");
     ctx->times = PhaseTimes();
@@ -2010,10 +2068,17 @@ void kset_checksum(const KSet *ks, uint64_t *out4) {
     Ctx *ctx = ks->ctx;
     DArr<unsigned long long> d(ctx, 4);
     SG_CUDA(cudaMemsetAsync(d.p, 0, 32, ctx->stream));
-    for (const Chunk &c : ks->chunks) {
-        if (c.n == 0) continue;
-        kset_checksum_k<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(c.keys.p, ks->has_counts ? c.counts.p : nullptr, (uint64_t)c.n, ks->nw, d.p);
-        ctx->launches++;
+    std::unique_ptr<ChunkStager> stage(ks->on_host ? new ChunkStager(ks, true) : nullptr);     // a host set streams through the device
+    for (size_t i = 0; i < ks->chunks.size(); ++i) {
+        const Chunk &c = ks->chunks[i];
+        const uint64_t *keys = c.keys.p;
+        const uint32_t *counts = ks->has_counts ? c.counts.p : nullptr;
+        if (stage) stage->acquire(i, &keys, &counts);
+        if (c.n) {
+            kset_checksum_k<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(keys, counts, (uint64_t)c.n, ks->nw, d.p);
+            ctx->launches++;
+        }
+        if (stage) stage->release(i);
     }
     SG_CUDA(cudaGetLastError());
     unsigned long long h[4];
@@ -2133,9 +2198,11 @@ struct DistState {
     std::vector<PullSrc> peers;              // world entries (own entry = local pointers)
     DArr<unsigned long long> d_bsz;
     KSet *out = nullptr;
+    std::unique_ptr<ResultSink> sink;        // SGPU_RESULT_ON_HOST: each pass's chunk is copied to host memory behind the next pass
+    bool result_on_host = false;
     int64_t first = 0;
     bool want_counts = false, double_selfrc = false;
-    virtual ~DistState() { delete out; }
+    virtual ~DistState() { sink.reset(); delete out; }
     virtual void begin() = 0;
     virtual void local_counts(uint64_t *h_out) = 0;
     virtual const uint32_t *blk_counts_ptr() = 0;
@@ -2294,14 +2361,17 @@ struct DistStateNW : DistState {
             SG_CUDA(cudaMemcpyAsync(d_start.p, start.data(), (size_t)(PA + 1) * 8, cudaMemcpyHostToDevice, st));
             Timer tm(st);
             Trace tr(st);
-            sort_pass<NW>(ctx, K, xbuf, sbuf, d_start.p, d_tot.p, PA, plan.rA, (uint32_t)my_lo, my_hi, first, want_counts, double_selfrc, d_bsz.p, ch, tm, tr);
+            sort_pass<NW>(ctx, K, xbuf, sbuf, d_start.p, d_tot.p, PA, plan.rA, (uint32_t)my_lo, my_hi, first, want_counts, double_selfrc, d_bsz.p, ch, tm, tr,
+                          nullptr, sink.get());
         } else {
+            if (sink) sink->drain();
             ch.n = 0; ch.b_lo = my_lo; ch.b_hi = my_hi; ch.first = first;
             ch.keys.alloc(ctx, 2, true);
             if (want_counts) ch.counts.alloc(ctx, 1, true);
         }
         first += ch.n;
         out->chunks.push_back(std::move(ch));
+        if (sink) sink->push();
     }
 };
 
@@ -2311,7 +2381,7 @@ static DistState *dist_state_new(int mode) {
     return new DistStateNW<NW, false>();
 }
 
-DistState *dist_begin(Ctx *ctx, int K, int B, int mode, int world, int rank) {
+DistState *dist_begin(Ctx *ctx, int K, int B, int mode, int world, int rank, bool result_on_host) {
     SG_CHECK(K >= 1 && K <= 128, 2, "K must be in [1,128]");
     SG_CHECK(B >= 1 && B <= kLevelAMaxParts, 2, "distributed count: num_buckets must be in [1, 8192]");
     SG_CHECK(world >= 1 && world <= 255 && rank >= 0 && rank < world, 2, "bad world/rank");
@@ -2325,7 +2395,7 @@ DistState *dist_begin(Ctx *ctx, int K, int B, int mode, int world, int rank) {
         case 3: d = dist_state_new<3>(mode); break;
         default: d = dist_state_new<4>(mode); break;
     }
-    d->ctx = ctx; d->K = K; d->B = B; d->mode = mode; d->nw = nwords_of(K);
+    d->ctx = ctx; d->K = K; d->B = B; d->mode = mode; d->nw = nwords_of(K); d->result_on_host = result_on_host;
     d->G = ctx->num_sms * levelA_ctas_per_sm();
     d->want_counts = (mode == kCanonical); d->double_selfrc = (mode == kCanonical) && (K % 2 == 0);
     // every rank must use the same geometry, so it depends on B only. As many level-A partitions as the shared-memory tables allow:
@@ -2350,6 +2420,8 @@ void dist_plan(DistState *d, const uint64_t *cnt_all, uint64_t *total_records) {
     SG_CUDA(cudaMemsetAsync(d->d_bsz.p, 0, (size_t)d->B * 8, ctx->stream));
     d->out = new KSet();
     d->out->ctx = ctx; d->out->K = d->K; d->out->nw = d->nw; d->out->B = d->B; d->out->has_counts = d->want_counts;
+    d->out->on_host = d->result_on_host;
+    if (d->result_on_host) d->sink.reset(new ResultSink(ctx, d->out));
     SG_CUDA(cudaStreamSynchronize(ctx->stream));
     *total_records = d->plan.Tb[d->B];
 }
@@ -2451,6 +2523,7 @@ void dist_sort(DistState *d, int p) {
 KSet *dist_end(DistState *d) {
     Ctx *ctx = d->ctx;
     KSet *ks = d->out;
+    if (d->sink) { d->sink->drain(); d->sink.reset(); }
     const int B = d->B;
     std::vector<unsigned long long> hb(B);
     SG_CUDA(cudaMemcpyAsync(hb.data(), d->d_bsz.p, (size_t)B * 8, cudaMemcpyDeviceToHost, ctx->stream));

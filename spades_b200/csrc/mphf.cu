@@ -232,43 +232,64 @@ static void build_nw(Ctx *ctx, const KSet *ks, Mphf *m) {
     SG_CUDA(cudaMemcpyAsync(m->d_starts.p, m->starts.data(), m->starts.size() * 8, cudaMemcpyHostToDevice, st));
     if (n == 0 || total_words == 0) { SG_CUDA(cudaStreamSynchronize(st)); return; }
 
-    KeyTable t = make_table(ks);
     MphfDev md = mphf_dev(m);
     const uint64_t l0_words = level_start[1] - level_start[0];
     DArr<uint64_t> coll(ctx, l0_words + 8);
     SG_CUDA(cudaMemsetAsync(coll.p, 0, coll.bytes(), st));
     DArr<unsigned long long> d_cnt(ctx, 1);
     DArr<uint64_t> aliveA, aliveB;
-    const uint64_t *alive = nullptr;
-    uint64_t n_alive = n;
-    // level 0 takes every key; afterwards one fused kernel per level tests the previous level's bit and inserts the
-    // survivors into the next level right away (one key load + one XXH3-128 per key and level instead of two)
-    mphf_insert_k<NW><<<div_up((int64_t)n_alive, 256), 256, 0, st>>>(t, alive, n_alive, 0, md, level_start[0], coll.p);
-    mphf_clear_k<<<div_up((int64_t)l0_words, 256), 256, 0, st>>>(m->bits.p + level_start[0], coll.p, l0_words);
-    ctx->launches += 2;
-    for (int l = 0; l < kLevels - 1 && n_alive; ++l) {
-        const bool last = (l == kLevels - 2);              // level 23 has no successor bitset: only count what is left
-        DArr<uint64_t> &next = (l & 1) ? aliveA : aliveB;
-        uint64_t cap = (l == 0) ? n_alive / 2 + 1024 : n_alive;
-        if (next.n < cap) next.alloc(ctx, cap);
-        SG_CUDA(cudaMemsetAsync(d_cnt.p, 0, 8, st));
-        mphf_advance_k<NW><<<div_up((int64_t)n_alive, 256), 256, 0, st>>>(t, alive, n_alive, l, md, next.p, (uint64_t)next.n, d_cnt.p,
-                                                                         last ? 0 : 1, last ? 0 : level_start[l + 1], coll.p);
-        ctx->launches++;
-        if (!last) {
-            const uint64_t lw = level_start[l + 2] - level_start[l + 1];
-            mphf_clear_k<<<div_up((int64_t)lw, 256), 256, 0, st>>>(m->bits.p + level_start[l + 1], coll.p, lw);
+    // places the n keys of table t, all of buckets [b_lo, b_hi), in every level. A key touches only its own bucket's pieces, so
+    // a level's collisions are cleared over the words of those buckets alone, and the bits do not depend on how the set is split.
+    // Level 0 takes every key; afterwards one fused kernel per level tests the previous level's bit and inserts the survivors
+    // into the next level right away (one key load + one XXH3-128 per key and level instead of two)
+    auto place = [&](const KeyTable &t, uint64_t n, int b_lo, int b_hi) {
+        auto clear = [&](int l) {
+            const uint64_t w0 = m->woff[(size_t)l * B + b_lo], nw = m->woff[(size_t)l * B + b_hi] - w0;
+            mphf_clear_k<<<div_up((int64_t)nw, 256), 256, 0, st>>>(m->bits.p + w0, coll.p + (w0 - level_start[l]), nw);
             ctx->launches++;
+        };
+        const uint64_t *alive = nullptr;
+        uint64_t n_alive = n;
+        mphf_insert_k<NW><<<div_up((int64_t)n_alive, 256), 256, 0, st>>>(t, alive, n_alive, 0, md, level_start[0], coll.p);
+        ctx->launches++;
+        clear(0);
+        for (int l = 0; l < kLevels - 1 && n_alive; ++l) {
+            const bool last = (l == kLevels - 2);              // level 23 has no successor bitset: only count what is left
+            DArr<uint64_t> &next = (l & 1) ? aliveA : aliveB;
+            uint64_t cap = (l == 0) ? n_alive / 2 + 1024 : n_alive;
+            if (next.n < cap) next.alloc(ctx, cap);
+            SG_CUDA(cudaMemsetAsync(d_cnt.p, 0, 8, st));
+            mphf_advance_k<NW><<<div_up((int64_t)n_alive, 256), 256, 0, st>>>(t, alive, n_alive, l, md, next.p, (uint64_t)next.n, d_cnt.p,
+                                                                             last ? 0 : 1, last ? 0 : level_start[l + 1], coll.p);
+            ctx->launches++;
+            if (!last) clear(l + 1);
+            SG_CUDA(cudaGetLastError());
+            unsigned long long c = 0;
+            SG_CUDA(cudaMemcpyAsync(&c, d_cnt.p, 8, cudaMemcpyDeviceToHost, st));
+            SG_CUDA(cudaStreamSynchronize(st));
+            SG_CHECK(c <= next.n, 6, "internal: MPHF survivor list overflow");
+            alive = next.p;
+            n_alive = c;
         }
-        SG_CUDA(cudaGetLastError());
-        unsigned long long c = 0;
-        SG_CUDA(cudaMemcpyAsync(&c, d_cnt.p, 8, cudaMemcpyDeviceToHost, st));
-        SG_CUDA(cudaStreamSynchronize(st));
-        SG_CHECK(c <= next.n, 6, "internal: MPHF survivor list overflow");
-        alive = next.p;
-        n_alive = c;
+        SG_CHECK(n_alive == 0, 7, "MPHF: keys fell through all 24 bitset levels (reference would use its order-dependent fallback map); unsupported");
+    };
+    if (!ks->on_host) {
+        place(make_table(ks), n, 0, B);
+    } else {
+        // a host set is placed chunk by chunk (a chunk is a contiguous bucket range), each chunk uploaded while the one before is placed
+        ChunkStager stage(ks, false);
+        for (size_t c = 0; c < ks->chunks.size(); ++c) {
+            const Chunk &ch = ks->chunks[c];
+            const uint64_t *keys = nullptr;
+            stage.acquire(c, &keys, nullptr);
+            if (ch.n) {
+                KeyTable t;
+                t.nchunks = 1; t.first[0] = 0; t.first[1] = ch.n; t.keys[0] = keys;
+                place(t, (uint64_t)ch.n, ch.b_lo, ch.b_hi);
+            }
+            stage.release(c);
+        }
     }
-    SG_CHECK(n_alive == 0, 7, "MPHF: keys fell through all 24 bitset levels (reference would use its order-dependent fallback map); unsupported");
     // ---- ranks
     DArr<uint32_t> pop(ctx, nblocks + 1);
     DArr<uint64_t> gscan(ctx, nblocks + 1), piece_base(ctx, (size_t)kLevels * B), d_last(ctx, B);

@@ -73,11 +73,19 @@ struct PhaseTimes {   // device milliseconds measured with CUDA events on ctx->s
     uint64_t level_a_key_bits = 0, level_a_scatters = 0;
     uint64_t refine_rounds_max = 0, refine_splits_round0 = 0, refine_splits_later = 0;
     uint64_t sort_lsd_fallbacks = 0, sort_oversize_equal = 0;
+    // a count whose result goes to host memory: bytes copied there, and host milliseconds spent waiting for those copies
+    uint64_t result_d2h_bytes = 0;
+    float result_d2h_wait = 0;
 };
 
 struct Ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
+    cudaStream_t copy = nullptr;    // non-blocking stream of the copies between host-resident k-mer sets and the device (created at first use)
+    cudaStream_t copy_stream() {
+        if (!copy) SG_CUDA(cudaStreamCreateWithFlags(&copy, cudaStreamNonBlocking));
+        return copy;
+    }
     int num_sms = 132;
     size_t hbm_budget = 0;       // 0 = use free memory
     size_t allocated = 0, peak = 0;
@@ -229,11 +237,40 @@ void DArr<T>::release() {
     p = nullptr; n = 0; blk = 0;
 }
 
-// A counted k-mer set resident in HBM: what KMerDiskCounter::Count leaves on disk
-// (kmer_index_builder.hpp:306-332), bucket-major, strictly increasing inside a bucket.
+// pinned host memory (cudaHostAlloc): copies to and from it run at the full PCIe rate and asynchronously
+template <class T>
+struct HostArr {
+    T *p = nullptr;
+    size_t n = 0;
+    HostArr() {}
+    HostArr(const HostArr &) = delete;
+    HostArr &operator=(const HostArr &) = delete;
+    HostArr(HostArr &&o) noexcept { p = o.p; n = o.n; o.p = nullptr; o.n = 0; }
+    HostArr &operator=(HostArr &&o) noexcept {
+        if (this != &o) { release(); p = o.p; n = o.n; o.p = nullptr; o.n = 0; }
+        return *this;
+    }
+    ~HostArr() { release(); }
+    void alloc(size_t n_) {
+        release();
+        void *q = nullptr;
+        if (cudaHostAlloc(&q, (n_ ? n_ : 1) * sizeof(T), cudaHostAllocDefault) != cudaSuccess) {
+            cudaGetLastError();
+            throw Error(4, "out of pinned host memory for a host-resident k-mer set");
+        }
+        p = (T *)q; n = n_;
+    }
+    void release() { if (p) cudaFreeHost(p); p = nullptr; n = 0; }
+};
+
+// A counted k-mer set: what KMerDiskCounter::Count leaves on disk (kmer_index_builder.hpp:306-332), bucket-major, strictly
+// increasing inside a bucket. It lives in HBM (keys / counts), or, for a count with SGPU_RESULT_ON_HOST, in pinned host memory
+// (h_keys / h_counts; the device arrays are released once the chunk's copy has completed). A set's chunks all live in one place.
 struct Chunk {
     DArr<uint64_t> keys;     // n * nw words (records of W = 8*nw bytes, the on-disk record format)
     DArr<uint32_t> counts;   // n (canonical mode) or empty
+    HostArr<uint64_t> h_keys;
+    HostArr<uint32_t> h_counts;
     int64_t n = 0;
     int b_lo = 0, b_hi = 0;  // buckets [b_lo, b_hi)
     int64_t first = 0;       // index of its first record in final_kmers order
@@ -246,9 +283,59 @@ struct KSet {
     int K = 0, nw = 0, B = 0;
     int64_t n = 0;
     bool has_counts = false;
+    bool on_host = false;              // chunks in pinned host memory
     std::vector<Chunk> chunks;
     std::vector<int64_t> bsz;          // B
     std::vector<int64_t> bstart;       // B+1 exclusive prefix (final_kmers order)
+};
+
+// Brings a host set's chunks to the device one at a time, double-buffered: chunk c + 1 is copied on the context's copy stream
+// while chunk c is used on its stream. acquire(c) makes chunk c readable by work enqueued next on ctx->stream; release(c) marks
+// the end of that work (the chunk's buffer may then take chunk c + 2). Chunks must be acquired in order.
+struct ChunkStager {
+    Ctx *ctx;
+    const KSet *ks;
+    bool with_counts;
+    DArr<uint64_t> keys[2];
+    DArr<uint32_t> counts[2];
+    cudaEvent_t loaded[2] = {nullptr, nullptr}, used[2] = {nullptr, nullptr};
+    ChunkStager(const KSet *s, bool counts_too) : ctx(s->ctx), ks(s), with_counts(counts_too && s->has_counts) {
+        size_t mx = 1;
+        for (const Chunk &c : ks->chunks) mx = std::max(mx, (size_t)c.n);
+        for (int i = 0; i < 2; ++i) {
+            keys[i].alloc(ctx, mx * ks->nw);
+            if (with_counts) counts[i].alloc(ctx, mx);
+            SG_CUDA(cudaEventCreateWithFlags(&loaded[i], cudaEventDisableTiming));
+            SG_CUDA(cudaEventCreateWithFlags(&used[i], cudaEventDisableTiming));
+        }
+    }
+    ~ChunkStager() {
+        // the buffers go back to the arena: no copy may still be writing them
+        if (ctx->copy) cudaStreamSynchronize(ctx->copy);
+        for (int i = 0; i < 2; ++i) { if (loaded[i]) cudaEventDestroy(loaded[i]); if (used[i]) cudaEventDestroy(used[i]); }
+    }
+    ChunkStager(const ChunkStager &) = delete;
+    ChunkStager &operator=(const ChunkStager &) = delete;
+    void prefetch(size_t c) {
+        const Chunk &ch = ks->chunks[c];
+        const int s = (int)(c & 1);
+        cudaStream_t cs = ctx->copy_stream();
+        SG_CUDA(cudaStreamWaitEvent(cs, used[s], 0));
+        if (ch.n) {
+            SG_CUDA(cudaMemcpyAsync(keys[s].p, ch.h_keys.p, (size_t)ch.n * ks->nw * 8, cudaMemcpyHostToDevice, cs));
+            if (with_counts) SG_CUDA(cudaMemcpyAsync(counts[s].p, ch.h_counts.p, (size_t)ch.n * 4, cudaMemcpyHostToDevice, cs));
+        }
+        SG_CUDA(cudaEventRecord(loaded[s], cs));
+    }
+    void acquire(size_t c, const uint64_t **k, const uint32_t **cnt) {
+        if (c == 0) prefetch(0);
+        const int s = (int)(c & 1);
+        SG_CUDA(cudaStreamWaitEvent(ctx->stream, loaded[s], 0));
+        if (c + 1 < ks->chunks.size()) prefetch(c + 1);
+        *k = keys[s].p;
+        if (cnt) *cnt = with_counts ? counts[s].p : nullptr;
+    }
+    void release(size_t c) { SG_CUDA(cudaEventRecord(used[c & 1], ctx->stream)); }
 };
 
 // boomphf-compatible index resident in HBM (one mphf per bucket, BooPHF.h / kmer_index.hpp)
@@ -281,7 +368,7 @@ void cov_filter(Ctx *ctx, int K, unsigned thr, int apply, uint8_t *keep_out, uin
 
 // count.cu
 enum CountMode { kCanonical = 0, kAllWindows = 1 };
-KSet *count_from_reads(Ctx *ctx, int K, int B, int mode);
+KSet *count_from_reads(Ctx *ctx, int K, int B, int mode, bool result_on_host = false);
 KSet *kmers_from_kpomers(Ctx *ctx, const KSet *kp, int B);
 
 void kset_checksum(const KSet *ks, uint64_t *out4);
@@ -289,7 +376,7 @@ void kset_checksum(const KSet *ks, uint64_t *out4);
 // distributed count (count.cu)
 struct DistState;
 struct DistPlan;
-DistState *dist_begin(Ctx *ctx, int K, int B, int mode, int world, int rank);
+DistState *dist_begin(Ctx *ctx, int K, int B, int mode, int world, int rank, bool result_on_host = false);
 uint32_t dist_num_partitions(const DistState *d);
 void dist_local_counts(DistState *d, uint64_t *h_out);
 void dist_plan(DistState *d, const uint64_t *cnt_all, uint64_t *total_records);

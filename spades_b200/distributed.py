@@ -8,16 +8,17 @@ import ctypes as C
 
 import numpy as np
 
-from .kmer_index import KMerDiskStorage, SGPU_CANONICAL
+from .kmer_index import KMerDiskStorage, SGPU_CANONICAL, SGPU_RESULT_ON_HOST
 
 SGPU_IPC_BYTES = 96
 
 
 class DistributedKMerCounter:
-    """KMerDiskCounter over a read set sharded across the ranks of a torch.distributed process group."""
+    """KMerDiskCounter over a read set sharded across the ranks of a torch.distributed process group. result_on_host: each rank's
+    set goes to its pinned host memory, pass by pass behind the next one."""
 
-    def __init__(self, ctx, K, mode=SGPU_CANONICAL, group=None):
-        self.ctx, self.K, self.mode, self.group = ctx, K, mode, group
+    def __init__(self, ctx, K, mode=SGPU_CANONICAL, group=None, result_on_host=False):
+        self.ctx, self.K, self.mode, self.group, self.result_on_host = ctx, K, mode, group, result_on_host
         self.npass = 0
 
     def close(self):
@@ -30,7 +31,8 @@ class DistributedKMerCounter:
         world, rank = dist.get_world_size(self.group), dist.get_rank(self.group)
         backend_dev = "cuda" if dist.get_backend(self.group) == "nccl" else "cpu"
         h = C.c_void_p()
-        ctx.check(L.sgpu_dist_begin(ctx.h, self.K, num_buckets, self.mode, world, rank, C.byref(h)))
+        mode = self.mode | (SGPU_RESULT_ON_HOST if self.result_on_host else 0)
+        ctx.check(L.sgpu_dist_begin(ctx.h, self.K, num_buckets, mode, world, rank, C.byref(h)))
         try:
             npart = L.sgpu_dist_num_partitions(h)
             local = np.zeros(npart, np.uint64)

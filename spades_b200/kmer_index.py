@@ -14,6 +14,7 @@ import numpy as np
 from . import _lib
 
 SGPU_CANONICAL, SGPU_ALL_WINDOWS = 0, 1
+SGPU_RESULT_ON_HOST = 0x100      # OR-ed into a count's mode: the set is returned in pinned host memory
 
 
 class SpadesGpuError(RuntimeError):
@@ -69,7 +70,8 @@ class Context:
 
 
 class KMerDiskStorage:
-    """Result of a count: B buckets of strictly increasing records, resident in HBM."""
+    """Result of a count: B buckets of strictly increasing records, resident in HBM or, for a count with result_on_host, in pinned
+    host memory (every accessor and KMerIndexBuilder work on both; the graph path needs sets in HBM)."""
 
     def __init__(self, ctx, h):
         self.ctx, self.h = ctx, h
@@ -87,6 +89,9 @@ class KMerDiskStorage:
 
     def total_kmers(self):
         return self._n
+
+    def on_host(self):
+        return self.ctx.L.sgpu_kset_on_host(self.h) == 1
 
     def bucket_sizes(self):
         out = np.zeros(self._B, np.int64)
@@ -159,15 +164,18 @@ class DeBruijnKMerKMerSplitter:
 
 
 class KMerDiskCounter:
-    def __init__(self, ctx: Context, splitter):
-        self.ctx, self.splitter = ctx, splitter
+    """result_on_host: the counted set goes to pinned host memory, pass by pass behind the next one, so it may exceed HBM."""
+
+    def __init__(self, ctx: Context, splitter, result_on_host=False):
+        self.ctx, self.splitter, self.result_on_host = ctx, splitter, result_on_host
 
     def Count(self, num_buckets, num_threads=0):
         h = C.c_void_p()
         if isinstance(self.splitter, DeBruijnKMerKMerSplitter):
             rc = self.ctx.L.sgpu_kmers_from_kpomers(self.ctx.h, self.splitter.source.h, num_buckets, C.byref(h))
         else:
-            rc = self.ctx.L.sgpu_count(self.ctx.h, self.splitter.K, num_buckets, self.splitter.mode, C.byref(h))
+            mode = self.splitter.mode | (SGPU_RESULT_ON_HOST if self.result_on_host else 0)
+            rc = self.ctx.L.sgpu_count(self.ctx.h, self.splitter.K, num_buckets, mode, C.byref(h))
         self.ctx.check(rc)
         return KMerDiskStorage(self.ctx, h)
 
