@@ -91,6 +91,11 @@ typedef struct sgpu_times {
     /* a count with SGPU_RESULT_ON_HOST (last sgpu_count / sgpu_dist_begin .. sgpu_dist_end) */
     uint64_t result_d2h_bytes;      /* bytes of records and multiplicities copied to host memory */
     float result_d2h_wait_ms;       /* host time the count spent waiting for those copies */
+    /* bytes of host-set chunks uploaded to the device since the last sgpu_kmers_from_kpomers_ex, sgpu_mphf_build or graph build
+     * began (0 when its sets live in HBM) */
+    uint64_t stage_h2d_bytes;
+    uint64_t graph_junction_batches; /* junction batches of the last graph build (0 when it had no junctions, e.g. no k-mers or
+                                      * only perfect loops); a batch never spans the junctions of two chunks of the k-mer set */
 } sgpu_times;
 
 int sgpu_create(const sgpu_config *cfg, sgpu_ctx **out);
@@ -161,9 +166,13 @@ int sgpu_reads_append_batch(sgpu_ctx *ctx, const sgpu_read_batch *b);
 
 /* mode: SGPU_CANONICAL or SGPU_ALL_WINDOWS, optionally | SGPU_RESULT_ON_HOST. A host set answers every sgpu_kset_* call and
  * sgpu_mphf_build exactly as a device set does (the index is built chunk by chunk, uploading each chunk while the one before is
- * placed); sgpu_kmers_from_kpomers and the sgpu_graph_build* calls need their sets in HBM and return SGPU_EUNSUPPORTED for it. */
+ * placed), and sgpu_kmers_from_kpomers_ex and sgpu_graph_build_streamed take it. sgpu_kmers_from_kpomers and the older
+ * sgpu_graph_build* calls need their sets in HBM and return SGPU_EUNSUPPORTED for a host set. */
 int sgpu_count(sgpu_ctx *ctx, int K, int num_buckets, int mode, sgpu_kset **out);
 int sgpu_kmers_from_kpomers(sgpu_ctx *ctx, const sgpu_kset *kpomers, int num_buckets, sgpu_kset **out);
+/* the k-mers of a (k+1)-mer set in HBM or in host memory; mode = 0 (result in HBM) or SGPU_RESULT_ON_HOST. A host (k+1)-mer
+ * set is uploaded chunk by chunk, once per histogram super-range and once per pass, the next chunk while the current one is read. */
+int sgpu_kmers_from_kpomers_ex(sgpu_ctx *ctx, const sgpu_kset *kpomers, int num_buckets, int mode, sgpu_kset **out);
 
 int64_t sgpu_kset_size(const sgpu_kset *s);
 int sgpu_kset_k(const sgpu_kset *s);
@@ -214,6 +223,11 @@ typedef struct sgpu_graph_options {
 } sgpu_graph_options;
 int sgpu_graph_build_opts(sgpu_ctx *ctx, const sgpu_kset *kpomers, const sgpu_kset *kmers, const sgpu_mphf *kmer_index,
                           const sgpu_mphf *kpomer_index, const sgpu_graph_options *opts, sgpu_graph **out);
+/* sgpu_graph_build_opts over sets in HBM or host memory, in any combination; the sets are read chunk by chunk (a host set's chunks
+ * are uploaded while the one before is used). The device keeps both indexes, the masks, the coverage and the clippers' flags; the
+ * unbranching paths are extracted in batches of junctions sized from the memory left. Same results as sgpu_graph_build_opts. */
+int sgpu_graph_build_streamed(sgpu_ctx *ctx, const sgpu_kset *kpomers, const sgpu_kset *kmers, const sgpu_mphf *kmer_index,
+                              const sgpu_mphf *kpomer_index, const sgpu_graph_options *opts, sgpu_graph **out);
 /* stats: edges collected (RemoveATEdges' return value), links removed, k-mers removed (RemoveATTips' return value), clipped tips */
 int sgpu_graph_at_clipper_stats(const sgpu_graph *g, uint64_t *out4);
 int sgpu_graph_masks(const sgpu_graph *g, uint8_t *out, int64_t n);           /* n = number of k-mers */

@@ -17,7 +17,10 @@
 // This only works because the GPU's MPHF is bit-identical to the one the reference builds: the mask / coverage arrays are indexed
 // by it. Exit code 0 iff the reference, fed with the GPU's arrays, extracts the GPU's unitigs and writes the GPU's GFA.
 //
-//   spades_gbuilder_gpu <reads (FASTA/FASTQ[.gz] or one read per line)> <k> <workdir> [num_buckets=16] [early_tip_length_bound=0]
+//   spades_gbuilder_gpu <reads (FASTA/FASTQ[.gz] or one read per line)> <k> <workdir> [num_buckets=16] [early_tip_length_bound=0] [--host-result]
+//
+// --host-result: both counts keep their sets in host memory (SGPU_RESULT_ON_HOST), so they may be larger than the device, and the
+// graph comes from sgpu_graph_build_streamed, which reads the sets chunk by chunk. The checks against the reference are the same.
 #include "gpu_kmer_counter.hpp"
 
 #include "kmer_index/ph_map/kmer_maps.hpp"
@@ -50,12 +53,13 @@ static void create_console_logger() {
 // DeBruijnKMerKMerSplitter (kmer_extension_index_builder.hpp:83-96, kmer_splitters.hpp:138-207)
 class GpuKmersFromKpomersCounter : public kmers::KMerCounter<RtSeq> {
   public:
-    GpuKmersFromKpomersCounter(fs::TmpDir work_dir, unsigned k, sgpu_ctx *ctx, const sgpu_kset *kpomers)
-            : kmers::KMerCounter<RtSeq>(k), work_dir_(work_dir), ctx_(ctx), kpomers_(kpomers) {}
+    // mode: 0, or SGPU_RESULT_ON_HOST to keep the k-mer set in host memory
+    GpuKmersFromKpomersCounter(fs::TmpDir work_dir, unsigned k, sgpu_ctx *ctx, const sgpu_kset *kpomers, int mode = 0)
+            : kmers::KMerCounter<RtSeq>(k), work_dir_(work_dir), ctx_(ctx), kpomers_(kpomers), mode_(mode) {}
     ~GpuKmersFromKpomersCounter() override { if (last_) sgpu_kset_free(last_); }
     size_t kmer_size() const override { return RtSeq::GetDataSize(this->k()) * sizeof(RtSeq::DataType); }
     kmers::KMerDiskStorage<RtSeq> Count(unsigned num_buckets, unsigned) override {
-        if (sgpu_kmers_from_kpomers(ctx_, kpomers_, (int)num_buckets, &last_)) FATAL_ERROR("spades_b200: " << sgpu_last_error(ctx_));
+        if (sgpu_kmers_from_kpomers_ex(ctx_, kpomers_, (int)num_buckets, mode_, &last_)) FATAL_ERROR("spades_b200: " << sgpu_last_error(ctx_));
         kmers::KMerDiskStorage<RtSeq> res(work_dir_, this->k(), kmer::KMerSegmentPolicy<RtSeq>(num_buckets));
         std::string prefix;
         for (unsigned i = 0; i < num_buckets; ++i) {
@@ -76,13 +80,16 @@ class GpuKmersFromKpomersCounter : public kmers::KMerCounter<RtSeq> {
     fs::TmpDir work_dir_;
     sgpu_ctx *ctx_;
     const sgpu_kset *kpomers_;
+    int mode_;
     sgpu_kset *last_ = nullptr;
 };
 
 #define CK(call) do { if (int rc_ = (call)) { fprintf(stderr, "spades_b200 error %d: %s\n", rc_, sgpu_last_error(ctx)); return 4; } } while (0)
 
 int main(int argc, char **argv) {
-    if (argc < 4) { fprintf(stderr, "usage: %s reads k workdir [num_buckets] [early_tip_length_bound]\n", argv[0]); return 2; }
+    const bool host_result = argc > 4 && std::string(argv[argc - 1]) == "--host-result";
+    if (host_result) --argc;
+    if (argc < 4) { fprintf(stderr, "usage: %s reads k workdir [num_buckets] [early_tip_length_bound] [--host-result]\n", argv[0]); return 2; }
     const std::string reads_path = argv[1];
     const unsigned k = (unsigned)atoi(argv[2]);
     const std::filesystem::path workdir = argv[3];
@@ -102,7 +109,7 @@ int main(int argc, char **argv) {
     {
         auto tmp = fs::tmp::make_temp_dir(workdir, "construction");
         // ---- (k+1)-mers on the GPU
-        kmers::GpuKMerDiskCounter kpomer_counter(tmp, k + 1, ctx, SGPU_CANONICAL);
+        kmers::GpuKMerDiskCounter kpomer_counter(tmp, k + 1, ctx, SGPU_CANONICAL, host_result);
         {
             std::ifstream is(reads_path, std::ios::binary);
             const int c0 = is.get(), c1 = is.get();
@@ -113,14 +120,19 @@ int main(int argc, char **argv) {
         auto kpomers = kpomer_counter.Count(B, 1);
         // ---- k-mers on the GPU, the extension index's MPHF by the reference's own builder over the GPU-written buckets
         kmers::DeBruijnExtensionIndex<> ext(k);
-        GpuKmersFromKpomersCounter kmer_counter(tmp, k, ctx, kpomer_counter.device_set());
+        GpuKmersFromKpomersCounter kmer_counter(tmp, k, ctx, kpomer_counter.device_set(), host_result ? SGPU_RESULT_ON_HOST : 0);
         kmers::BuildIndex(ext, kmer_counter, B, 1);                  // KeyIteratingIndexBuilder: index + data_ size + kmers_ = final_kmers
         // ---- masks / coverage / unitigs / GFA on the GPU
         sgpu_mphf *mk = nullptr, *mkp = nullptr;
         sgpu_graph *gg = nullptr;
         CK(sgpu_mphf_build(ctx, kmer_counter.device_set(), &mk));
         CK(sgpu_mphf_build(ctx, kpomer_counter.device_set(), &mkp));
-        CK(sgpu_graph_build_ex(ctx, kpomer_counter.device_set(), kmer_counter.device_set(), mk, mkp, /* keep_perfect_loops */ 1, early_tc, &gg));
+        if (host_result) {
+            const sgpu_graph_options o = {/* keep_perfect_loops */ 1, early_tc, 0, 0.8, 10, 200};
+            CK(sgpu_graph_build_streamed(ctx, kpomer_counter.device_set(), kmer_counter.device_set(), mk, mkp, &o, &gg));
+        } else {
+            CK(sgpu_graph_build_ex(ctx, kpomer_counter.device_set(), kmer_counter.device_set(), mk, mkp, /* keep_perfect_loops */ 1, early_tc, &gg));
+        }
         if ((size_t)sgpu_kset_size(kmer_counter.device_set()) != ext.size()) { ERROR("k-mer count differs from the reference index size"); ++bad; }
         // the GPU's mask array straight into the reference's extension index (after the early tip clipper, if requested)
         CK(sgpu_graph_masks(gg, (uint8_t *)ext.raw_data(), (int64_t)ext.raw_size()));

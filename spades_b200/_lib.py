@@ -16,11 +16,11 @@ SYMBOLS = [
     "sgpu_fastx_parse", "sgpu_fastx_parse_threads", "sgpu_seqfile_parse", "sgpu_read_batch_write_seqfile", "sgpu_read_batch_num_reads", "sgpu_read_batch_num_words",
     "sgpu_read_batch_words", "sgpu_read_batch_offs", "sgpu_read_batch_lens", "sgpu_read_batch_stats", "sgpu_read_batch_error", "sgpu_read_batch_free",
     "sgpu_reads_append_batch",
-    "sgpu_count", "sgpu_kmers_from_kpomers",
+    "sgpu_count", "sgpu_kmers_from_kpomers", "sgpu_kmers_from_kpomers_ex",
     "sgpu_kset_size", "sgpu_kset_k", "sgpu_kset_num_buckets", "sgpu_kset_record_bytes", "sgpu_kset_on_host", "sgpu_kset_bucket_sizes",
     "sgpu_kset_checksum", "sgpu_kset_download_keys", "sgpu_kset_download_counts", "sgpu_kset_write_buckets", "sgpu_kset_write_final", "sgpu_kset_free",
     "sgpu_mphf_build", "sgpu_mphf_serialized_size", "sgpu_mphf_serialize", "sgpu_mphf_lookup", "sgpu_mphf_free",
-    "sgpu_graph_build", "sgpu_graph_build_ex", "sgpu_graph_build_opts", "sgpu_graph_at_clipper_stats", "sgpu_graph_tip_clipper_stats", "sgpu_graph_masks", "sgpu_graph_coverage", "sgpu_graph_histogram", "sgpu_graph_num_unitigs",
+    "sgpu_graph_build", "sgpu_graph_build_ex", "sgpu_graph_build_opts", "sgpu_graph_build_streamed", "sgpu_graph_at_clipper_stats", "sgpu_graph_tip_clipper_stats", "sgpu_graph_masks", "sgpu_graph_coverage", "sgpu_graph_histogram", "sgpu_graph_num_unitigs",
     "sgpu_graph_unitig_bases", "sgpu_graph_unitigs", "sgpu_graph_gfa", "sgpu_graph_write_gfa", "sgpu_graph_free",
     "sgpu_edge_index_build", "sgpu_edge_index_k", "sgpu_edge_index_size", "sgpu_edge_index_serialized_size", "sgpu_edge_index_serialize",
     "sgpu_edge_index_values", "sgpu_edge_index_lookup", "sgpu_edge_index_free",
@@ -45,7 +45,8 @@ class SgpuTimes(C.Structure):
                 ("instances", C.c_uint64), ("passes", C.c_uint64), ("launches", C.c_uint64), ("peak_bytes", C.c_uint64), ("cached_bytes", C.c_uint64),
                 ("level_a_key_bits", C.c_uint64), ("level_a_scatters", C.c_uint64), ("refine_rounds_max", C.c_uint64),
                 ("refine_splits_round0", C.c_uint64), ("refine_splits_later", C.c_uint64), ("sort_lsd_fallbacks", C.c_uint64),
-                ("sort_oversize_equal", C.c_uint64), ("result_d2h_bytes", C.c_uint64), ("result_d2h_wait_ms", C.c_float)]
+                ("sort_oversize_equal", C.c_uint64), ("result_d2h_bytes", C.c_uint64), ("result_d2h_wait_ms", C.c_float),
+                ("stage_h2d_bytes", C.c_uint64), ("graph_junction_batches", C.c_uint64)]
 
 
 _lib = None
@@ -89,6 +90,7 @@ def load():
     L.sgpu_reads_append_batch.restype = i32; L.sgpu_reads_append_batch.argtypes = [vp, vp]
     L.sgpu_count.restype = i32; L.sgpu_count.argtypes = [vp, i32, i32, i32, pp]
     L.sgpu_kmers_from_kpomers.restype = i32; L.sgpu_kmers_from_kpomers.argtypes = [vp, vp, i32, pp]
+    L.sgpu_kmers_from_kpomers_ex.restype = i32; L.sgpu_kmers_from_kpomers_ex.argtypes = [vp, vp, i32, i32, pp]
     L.sgpu_kset_size.restype = i64; L.sgpu_kset_size.argtypes = [vp]
     L.sgpu_kset_k.restype = i32; L.sgpu_kset_k.argtypes = [vp]
     L.sgpu_kset_num_buckets.restype = i32; L.sgpu_kset_num_buckets.argtypes = [vp]
@@ -109,6 +111,7 @@ def load():
     L.sgpu_graph_build.restype = i32; L.sgpu_graph_build.argtypes = [vp, vp, vp, vp, vp, i32, pp]
     L.sgpu_graph_build_ex.restype = i32; L.sgpu_graph_build_ex.argtypes = [vp, vp, vp, vp, vp, i32, u64, pp]
     L.sgpu_graph_build_opts.restype = i32; L.sgpu_graph_build_opts.argtypes = [vp, vp, vp, vp, vp, C.POINTER(SgpuGraphOptions), pp]
+    L.sgpu_graph_build_streamed.restype = i32; L.sgpu_graph_build_streamed.argtypes = [vp, vp, vp, vp, vp, C.POINTER(SgpuGraphOptions), pp]
     L.sgpu_graph_at_clipper_stats.restype = i32; L.sgpu_graph_at_clipper_stats.argtypes = [vp, vp]
     L.sgpu_graph_tip_clipper_stats.restype = i32; L.sgpu_graph_tip_clipper_stats.argtypes = [vp, vp]
     L.sgpu_graph_masks.restype = i32; L.sgpu_graph_masks.argtypes = [vp, vp, i64]

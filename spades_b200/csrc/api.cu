@@ -44,6 +44,18 @@ static int fail(Ctx *c, int code, const std::string &msg) {
     catch (const std::bad_alloc &) { return fail((ctxptr), SGPU_ENOMEM, "host allocation failed"); } \
     catch (const std::exception &e) { return fail((ctxptr), SGPU_EINTERNAL, e.what()); }
 
+// the entries that predate host sets (sgpu_kmers_from_kpomers, sgpu_graph_build, _ex, _opts) keep refusing them; their _ex /
+// _streamed successors take either placement
+static void check_device_sets(const sgpu_kset *kpomers, const sgpu_kset *kmers) {
+    SG_CHECK(!kpomers->s->on_host && !kmers->s->on_host, SGPU_EUNSUPPORTED,
+             "the graph is built from k-mer sets in device memory; this one lives in host memory (SGPU_RESULT_ON_HOST)");
+}
+static int device_sets_only(Ctx *c, const sgpu_kset *kpomers, const sgpu_kset *kmers) { API_TRY(c, check_device_sets(kpomers, kmers)); }
+static int device_kpomers_only(Ctx *c, const sgpu_kset *kpomers) {
+    API_TRY(c, SG_CHECK(!kpomers->s->on_host, SGPU_EUNSUPPORTED,
+                        "the (k+1)-mer set lives in host memory: the k-mers of the (k+1)-mers read it from the device"));
+}
+
 extern "C" {
 
 int sgpu_create(const sgpu_config *cfg, sgpu_ctx **out) {
@@ -86,6 +98,7 @@ int sgpu_get_times(const sgpu_ctx *ctx, sgpu_times *out) {
     out->refine_rounds_max = t.refine_rounds_max; out->refine_splits_round0 = t.refine_splits_round0; out->refine_splits_later = t.refine_splits_later;
     out->sort_lsd_fallbacks = t.sort_lsd_fallbacks; out->sort_oversize_equal = t.sort_oversize_equal;
     out->result_d2h_bytes = t.result_d2h_bytes; out->result_d2h_wait_ms = t.result_d2h_wait;
+    out->stage_h2d_bytes = t.stage_h2d_bytes; out->graph_junction_batches = t.graph_junction_batches;
     return SGPU_OK;
 }
 
@@ -190,16 +203,24 @@ int sgpu_count(sgpu_ctx *ctx, int K, int num_buckets, int mode, sgpu_kset **out)
     })
 }
 
-int sgpu_kmers_from_kpomers(sgpu_ctx *ctx, const sgpu_kset *kpomers, int num_buckets, sgpu_kset **out) {
+int sgpu_kmers_from_kpomers_ex(sgpu_ctx *ctx, const sgpu_kset *kpomers, int num_buckets, int mode, sgpu_kset **out) {
     if (!ctx || !kpomers || !out) return SGPU_EINVAL;
     *out = nullptr;
     Ctx *c = &ctx->c;
     API_TRY(c, {
+        SG_CHECK(mode == 0 || mode == SGPU_RESULT_ON_HOST, SGPU_EINVAL, "bad mode");
         SG_CUDA(cudaSetDevice(c->device));
-        KSet *s = kmers_from_kpomers(c, kpomers->s, num_buckets);
+        KSet *s = kmers_from_kpomers(c, kpomers->s, num_buckets, mode == SGPU_RESULT_ON_HOST);
         *out = new sgpu_kset{s};
         child_add(c);
     })
+}
+
+int sgpu_kmers_from_kpomers(sgpu_ctx *ctx, const sgpu_kset *kpomers, int num_buckets, sgpu_kset **out) {
+    if (!ctx || !kpomers || !out) return SGPU_EINVAL;
+    *out = nullptr;
+    const int rc = device_kpomers_only(&ctx->c, kpomers);
+    return rc != SGPU_OK ? rc : sgpu_kmers_from_kpomers_ex(ctx, kpomers, num_buckets, 0, out);
 }
 
 int64_t sgpu_kset_size(const sgpu_kset *s) { return s ? s->s->n : -1; }
@@ -334,53 +355,33 @@ void sgpu_mphf_free(sgpu_mphf *m) {
 
 }  // extern "C"
 
-// the graph kernels read both k-mer sets from HBM
-static void check_device_sets(const sgpu_kset *kpomers, const sgpu_kset *kmers) {
-    SG_CHECK(!kpomers->s->on_host && !kmers->s->on_host, SGPU_EUNSUPPORTED,
-             "the graph is built from k-mer sets in device memory; this one lives in host memory (SGPU_RESULT_ON_HOST)");
-}
 
 extern "C" {
 
 int sgpu_graph_build(sgpu_ctx *ctx, const sgpu_kset *kpomers, const sgpu_kset *kmers, const sgpu_mphf *kmer_index, const sgpu_mphf *kpomer_index,
                      int keep_perfect_loops, sgpu_graph **out) {
-    if (!ctx || !kpomers || !kmers || !kmer_index || !out) return SGPU_EINVAL;
-    *out = nullptr;
-    Ctx *c = &ctx->c;
-    API_TRY(c, {
-        check_device_sets(kpomers, kmers);
-        SG_CUDA(cudaSetDevice(c->device));
-        GraphOptions opt;
-        opt.keep_perfect_loops = keep_perfect_loops != 0;
-        Graph *g = graph_build(c, kpomers->s, kmers->s, kmer_index->m, kpomer_index ? kpomer_index->m : nullptr, opt);
-        *out = new sgpu_graph{g};
-        child_add(c);
-    })
+    const sgpu_graph_options o = {keep_perfect_loops, 0, 0, 0.8, 10, 200};
+    return sgpu_graph_build_opts(ctx, kpomers, kmers, kmer_index, kpomer_index, &o, out);
 }
 int sgpu_graph_build_ex(sgpu_ctx *ctx, const sgpu_kset *kpomers, const sgpu_kset *kmers, const sgpu_mphf *kmer_index, const sgpu_mphf *kpomer_index,
                         int keep_perfect_loops, uint64_t early_tip_length_bound, sgpu_graph **out) {
-    if (!ctx || !kpomers || !kmers || !kmer_index || !out) return SGPU_EINVAL;
-    *out = nullptr;
-    Ctx *c = &ctx->c;
-    API_TRY(c, {
-        check_device_sets(kpomers, kmers);
-        SG_CUDA(cudaSetDevice(c->device));
-        GraphOptions opt;
-        opt.keep_perfect_loops = keep_perfect_loops != 0;
-        opt.early_tip_length_bound = early_tip_length_bound;
-        Graph *g = graph_build(c, kpomers->s, kmers->s, kmer_index->m, kpomer_index ? kpomer_index->m : nullptr, opt);
-        *out = new sgpu_graph{g};
-        child_add(c);
-    })
+    const sgpu_graph_options o = {keep_perfect_loops, early_tip_length_bound, 0, 0.8, 10, 200};
+    return sgpu_graph_build_opts(ctx, kpomers, kmers, kmer_index, kpomer_index, &o, out);
 }
 int sgpu_graph_build_opts(sgpu_ctx *ctx, const sgpu_kset *kpomers, const sgpu_kset *kmers, const sgpu_mphf *kmer_index, const sgpu_mphf *kpomer_index,
                           const sgpu_graph_options *o, sgpu_graph **out) {
     if (!ctx || !kpomers || !kmers || !kmer_index || !o || !out) return SGPU_EINVAL;
     *out = nullptr;
+    const int rc = device_sets_only(&ctx->c, kpomers, kmers);
+    return rc != SGPU_OK ? rc : sgpu_graph_build_streamed(ctx, kpomers, kmers, kmer_index, kpomer_index, o, out);
+}
+int sgpu_graph_build_streamed(sgpu_ctx *ctx, const sgpu_kset *kpomers, const sgpu_kset *kmers, const sgpu_mphf *kmer_index,
+                              const sgpu_mphf *kpomer_index, const sgpu_graph_options *o, sgpu_graph **out) {
+    if (!ctx || !kpomers || !kmers || !kmer_index || !o || !out) return SGPU_EINVAL;
+    *out = nullptr;
     Ctx *c = &ctx->c;
     API_TRY(c, {
         SG_CHECK(!o->early_at_clipper || (o->at_ratio > 0.0 && o->at_ratio <= 1.0 && o->at_max_length >= 1), SGPU_EINVAL, "bad A/T clipper parameters");
-        check_device_sets(kpomers, kmers);
         SG_CUDA(cudaSetDevice(c->device));
         GraphOptions opt;
         opt.keep_perfect_loops = o->keep_perfect_loops != 0;

@@ -1688,6 +1688,17 @@ struct LevelAJob {
     std::vector<DArr<uint64_t>> tile_off; // per source: first id of every tile
     std::vector<DArr<uint16_t>> ids;      // per source: 2-byte partition id per record slot
     std::vector<uint64_t> h_part;         // host copy of part_total_all
+    ChunkStager *stage = nullptr;         // sources are the chunks of a host set: each launch reads the chunk's staged copy
+    // runs launch(src) for every non-empty source, in order; a staged source is uploaded behind the launches of the one before
+    template <class F>
+    void for_each_src(F &&launch) const {
+        for (size_t si = 0; si < srcs.size(); ++si) {
+            Src src = srcs[si];
+            if (stage) stage->acquire(si, &src.words, nullptr);
+            if (src.n) launch(si, src);
+            if (stage) stage->release(si);
+        }
+    }
     uint64_t bucket_records(int b) const {
         uint64_t s = 0;
         for (uint32_t q = 0; q < (1u << rA); ++q) s += h_part[((size_t)(b - s_lo) << rA) + q];
@@ -1772,12 +1783,10 @@ static void levelA_count(LevelAJob<NW, Src, BOTH> &job, Timer &tm, Trace &tr) {
     }
     tm.start();
     SG_CUDA(cudaFuncSetAttribute(levelA_count_roll_k<NW, Src, BOTH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)roll_smem_bytes(PA_all)));
-    for (size_t si = 0; si < job.srcs.size(); ++si) {
-        const Src &src = job.srcs[si];
-        if (src.n == 0) continue;
+    job.for_each_src([&](size_t si, const Src &src) {
         levelA_count_roll_k<NW, Src, BOTH><<<G, kRollThreads, roll_smem_bytes(PA_all), st>>>(src, pa_all, job.blk_counts.p, job.tile_off[si].p, job.ids[si].p);
         ctx->launches++;
-    }
+    });
     SG_CUDA(cudaGetLastError());
     levelA_totals_k<<<div_up(PA_all, 256), 256, 0, st>>>(job.blk_counts.p, PA_all, G, job.part_total_all.p);
     ctx->launches++;
@@ -1832,15 +1841,13 @@ static void levelA_scatter(LevelAJob<NW, Src, BOTH> &job, int b_lo, int b_hi, ui
         const size_t smem = job.use_ids ? levelA_batch_smem<NW, true>(pa_sub.PA, &cap) : levelA_batch_smem<NW, false>(pa_sub.PA, &cap);
         if (job.use_ids) SG_CUDA(cudaFuncSetAttribute(levelA_scatter_plan_k<NW, Src, BOTH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         else SG_CUDA(cudaFuncSetAttribute(levelA_scatter_roll_k<NW, Src, BOTH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        for (size_t si = 0; si < job.srcs.size(); ++si) {
-            const Src &src = job.srcs[si];
-            if (src.n == 0) continue;
+        job.for_each_src([&](size_t si, const Src &src) {
             if (job.use_ids)
                 levelA_scatter_plan_k<NW, Src, BOTH><<<G, kRollThreads, smem, st>>>(src, pa_sub, base.p, X, job.tile_off[si].p, job.ids[si].p, p_lo + q_lo, PA, q_lo, (uint64_t)job.ids[si].n, cap);
             else
                 levelA_scatter_roll_k<NW, Src, BOTH><<<G, kRollThreads, smem, st>>>(src, pa, base.p, X, PA, cap);
             ctx->launches++; ctx->times.level_a_scatters++;
-        }
+        });
     }
     SG_CUDA(cudaGetLastError());
     ctx->times.extract_scatter += tm.stop();       // synchronises: `base` may go out of scope
@@ -1853,7 +1860,7 @@ static double pass_bytes_needed(uint64_t recs, size_t W) { return (double)recs *
 
 template <int NW, bool BOTH, class Src>
 static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, int B, bool want_counts, bool double_selfrc, uint64_t est_records, KSet *out,
-                      ResultSink *sink = nullptr) {
+                      ResultSink *sink = nullptr, ChunkStager *stage = nullptr) {
     const int total_bits = 2 * K;
     const size_t W = 8 * NW;
     cudaStream_t st = ctx->stream;
@@ -1878,7 +1885,7 @@ static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, int B, bool
     for (int s_lo = 0; s_lo < B; s_lo += SR) {
         const int share = (kMaxChunks - (int)out->chunks.size()) / (n_ranges - s_lo / SR);
         LevelAJob<NW, Src, BOTH> job;
-        job.ctx = ctx; job.srcs = srcs; job.K = K; job.B = B; job.rA = rA; job.G = ctx->num_sms * levelA_ctas_per_sm();
+        job.ctx = ctx; job.srcs = srcs; job.K = K; job.B = B; job.rA = rA; job.G = ctx->num_sms * levelA_ctas_per_sm(); job.stage = stage;
         job.s_lo = s_lo; job.s_hi = std::min(B, s_lo + SR);
         job.PA_all = (uint32_t)(job.s_hi - job.s_lo) << rA;
         levelA_count(job, tm, tr);
@@ -2015,32 +2022,35 @@ KSet *count_from_reads(Ctx *ctx, int K, int B, int mode, bool result_on_host) {
 }
 
 template <int NW>
-static KSet *kmers_from_kpomers_nw(Ctx *ctx, const KSet *kp, int B) {
+static KSet *kmers_from_kpomers_nw(Ctx *ctx, const KSet *kp, int B, bool on_host) {
     const int K = kp->K - 1;
     KSet *ks = new KSet();
-    ks->ctx = ctx; ks->K = K; ks->nw = NW; ks->B = B; ks->has_counts = false;
+    ks->ctx = ctx; ks->K = K; ks->nw = NW; ks->B = B; ks->has_counts = false; ks->on_host = on_host;
     try {
+        std::unique_ptr<ResultSink> sink(on_host ? new ResultSink(ctx, ks) : nullptr);
+        // a host (k+1)-mer set: every launch that reads a chunk's words reads its staged copy. Allocated before the passes are
+        // planned, so the planner sees the two staging buffers.
+        std::unique_ptr<ChunkStager> stage(kp->on_host ? new ChunkStager(kp, false) : nullptr);
         std::vector<KmerSetSrc> srcs;
         for (const Chunk &c : kp->chunks) {
             KmerSetSrc s; s.words = c.keys.p; s.n = c.n; s.nwords = (uint64_t)c.n * kp->nw; s.K = K; s.stride = (uint32_t)kp->nw;
             srcs.push_back(s);
         }
-        run_count<NW, false>(ctx, srcs, K, B, false, false, (uint64_t)kp->n * 2, ks);
+        run_count<NW, false>(ctx, srcs, K, B, false, false, (uint64_t)kp->n * 2, ks, sink.get(), stage.get());
     } catch (...) { delete ks; throw; }
     return ks;
 }
 
-KSet *kmers_from_kpomers(Ctx *ctx, const KSet *kp, int B) {
+KSet *kmers_from_kpomers(Ctx *ctx, const KSet *kp, int B, bool result_on_host) {
     SG_CHECK(kp->K >= 2, 2, "source k-mers too short");
-    SG_CHECK(!kp->on_host, 7, "the (k+1)-mer set lives in host memory: the k-mers of the (k+1)-mers read it from the device");
     SG_CHECK(B >= 1 && B <= (1 << 20), 2, "num_buckets must be in [1, 2^20]");
     SG_CHECK(kp->nw == nwords_of(kp->K), 2, "unsupported k-mer word combination");
     ctx->times = PhaseTimes();
     switch (nwords_of(kp->K - 1)) {
-        case 1: return kmers_from_kpomers_nw<1>(ctx, kp, B);
-        case 2: return kmers_from_kpomers_nw<2>(ctx, kp, B);
-        case 3: return kmers_from_kpomers_nw<3>(ctx, kp, B);
-        default: return kmers_from_kpomers_nw<4>(ctx, kp, B);
+        case 1: return kmers_from_kpomers_nw<1>(ctx, kp, B, result_on_host);
+        case 2: return kmers_from_kpomers_nw<2>(ctx, kp, B, result_on_host);
+        case 3: return kmers_from_kpomers_nw<3>(ctx, kp, B, result_on_host);
+        default: return kmers_from_kpomers_nw<4>(ctx, kp, B, result_on_host);
     }
 }
 

@@ -7,6 +7,7 @@
 #include <algorithm>
 
 #include <chrono>
+#include <memory>
 
 #include "graph.h"
 #include "mphf_dev.cuh"
@@ -48,6 +49,15 @@ __device__ __forceinline__ void kmer_shr(Kmer<NW> &k, int K, int c) {
         carry = nc;
     }
     k.w[NW - 1] &= last_word_mask<NW>(K);
+}
+
+// record j of a dense key array (a chunk of a k-mer set, or a compacted list of keys)
+template <int NW>
+__device__ __forceinline__ Kmer<NW> key_at(const uint64_t *__restrict__ keys, int64_t j) {
+    Kmer<NW> k;
+#pragma unroll
+    for (int q = 0; q < NW; ++q) k.w[q] = keys[j * NW + q];
+    return k;
 }
 
 // ---- masks -------------------------------------------------------------------------------------------------------
@@ -97,13 +107,17 @@ __global__ void hist_fill_k(const uint32_t *__restrict__ cov, int64_t n, unsigne
 }
 
 // ---- unbranching paths ---------------------------------------------------------------------------------------------
+// The kernels below that walk the k-mer set run once per chunk: `keys` holds the chunk's n records, and `base` is the position
+// of its first record in final_kmers order, so every thread keeps its global k-mer position.
 template <int NW>
-__global__ void junction_flags_k(KeyTable t, int64_t n, int K, MphfDev mk, const uint8_t *__restrict__ masks, uint32_t *__restrict__ flag) {
+__global__ void junction_flags_k(const uint64_t *__restrict__ keys, int64_t n, int K, MphfDev mk, const uint8_t *__restrict__ masks, uint32_t *__restrict__ flag) {
     int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= n) return;
-    Kmer<NW> k = table_key<NW>(t, j);
+    Kmer<NW> k = key_at<NW>(keys, j);
     const uint8_t m = masks[mphf_lookup_dev<NW>(mk, k)];
-    flag[j] = (uniq4(m & 15) < 0 || uniq4(m >> 4) < 0) ? 1u : 0u;       // IsJunction, :194-200
+    // IsJunction (:194-200). An isolated k-mer (mask 0, e.g. a clipped tip's) is one too, but starts no path: it is left out of
+    // the list, which then costs nothing for the clipped k-mers
+    flag[j] = (m && (uniq4(m & 15) < 0 || uniq4(m >> 4) < 0)) ? 1u : 0u;
 }
 // kept slots -> dense (offset, length) table of the path edges (eidx = rank among the kept slots, eoff = first base)
 __global__ void edge_table_k(const uint32_t *__restrict__ len, const uint64_t *__restrict__ eidx, const uint64_t *__restrict__ eoff, int64_t nslots,
@@ -114,10 +128,14 @@ __global__ void edge_table_k(const uint32_t *__restrict__ len, const uint64_t *_
     out_len[eidx[i]] = len[i];
 }
 
-__global__ void compact_list_k(const uint32_t *__restrict__ flag, const uint64_t *__restrict__ pos, int64_t n, uint64_t *__restrict__ list) {
+// the flagged keys of a chunk, in chunk order
+template <int NW>
+__global__ void compact_keys_k(const uint32_t *__restrict__ flag, const uint64_t *__restrict__ pos, const uint64_t *__restrict__ keys, int64_t n,
+                               uint64_t *__restrict__ list) {
     int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= n) return;
-    if (flag[j]) list[pos[j]] = (uint64_t)j;
+    if (j >= n || !flag[j]) return;
+#pragma unroll
+    for (int q = 0; q < NW; ++q) list[pos[j] * NW + q] = keys[j * NW + q];
 }
 
 void launch_nonzero_flags(Ctx *ctx, const uint32_t *in, uint32_t *out, uint64_t n);
@@ -146,13 +164,13 @@ __device__ __forceinline__ uint32_t walk_right(const MphfDev &mk, const uint8_t 
 
 // probe pass: for junction q and slot s = side*4 + c decide whether the path is emitted and how long it is
 template <int NW>
-__global__ void unitig_probe_k(KeyTable t, const uint64_t *__restrict__ jlist, int64_t njunc, int K, MphfDev mk, const uint8_t *__restrict__ masks,
+__global__ void unitig_probe_k(const uint64_t *__restrict__ jkeys, int64_t njunc, int K, MphfDev mk, const uint8_t *__restrict__ masks,
                                uint64_t nk, uint32_t *__restrict__ len /*[njunc*8] 0 = none*/, uint8_t *__restrict__ selfc) {
     int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (tid >= njunc * 8) return;
     const int64_t q = tid >> 3;
     const int side = (int)(tid >> 2) & 1, c = (int)tid & 3;
-    const Kmer<NW> key = table_key<NW>(t, (int64_t)jlist[q]);
+    const Kmer<NW> key = key_at<NW>(jkeys, q);
     const uint8_t mfw = masks[mphf_lookup_dev<NW>(mk, key)];
     const Kmer<NW> start = side ? kmer_rc<NW>(key, K) : key;          // AddStartDeEdges :214-235
     const uint8_t m = side ? inv_byte(mfw) : mfw;
@@ -208,7 +226,7 @@ __device__ __forceinline__ uint32_t kpomer_cov(const MphfDev &mkp, const uint32_
 __device__ __forceinline__ uint64_t link_value(uint64_t idx, bool is_start, bool is_rc) { return (idx << 2) | (is_rc ? 2ull : 0ull) | (is_start ? 1ull : 0ull); }
 
 template <int NW, int NWS>
-__global__ void unitig_write_k(KeyTable t, const uint64_t *__restrict__ jlist, int64_t njunc, int K, MphfDev mk, const uint8_t *__restrict__ masks,
+__global__ void unitig_write_k(const uint64_t *__restrict__ jkeys, int64_t njunc, int K, MphfDev mk, const uint8_t *__restrict__ masks,
                                uint64_t nk, const uint32_t *__restrict__ len, const uint8_t *__restrict__ selfc, const uint64_t *__restrict__ eidx,
                                const uint64_t *__restrict__ eoff, MphfDev mkp, const uint32_t *__restrict__ cov, EdgeOut o) {
     int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -216,7 +234,7 @@ __global__ void unitig_write_k(KeyTable t, const uint64_t *__restrict__ jlist, i
     if (!len[tid]) return;
     const int64_t q = tid >> 3;
     const int side = (int)(tid >> 2) & 1, c = (int)tid & 3;
-    const Kmer<NW> key = table_key<NW>(t, (int64_t)jlist[q]);
+    const Kmer<NW> key = key_at<NW>(jkeys, q);
     const Kmer<NW> start = side ? kmer_rc<NW>(key, K) : key;
     const uint64_t e = eidx[tid];
     char *out = o.seq + eoff[tid];
@@ -249,7 +267,10 @@ __global__ void unitig_write_k(KeyTable t, const uint64_t *__restrict__ jlist, i
     o.raw_cov[e] = raw;
 }
 
-__global__ void masks_clear_visited_k(uint8_t *__restrict__ masks, const uint8_t *__restrict__ visited, uint64_t n, unsigned long long *__restrict__ remaining) {
+// also marks the remaining slots (unvisited, neither junction nor dead end: the vertices of perfect loops) in rem_bits, one bit per
+// slot: warp w writes word w (the grid covers whole warps)
+__global__ void masks_clear_visited_k(uint8_t *__restrict__ masks, const uint8_t *__restrict__ visited, uint64_t n, unsigned long long *__restrict__ remaining,
+                                      uint32_t *__restrict__ rem_bits) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     bool rem = false;
     if (i < n) {
@@ -258,6 +279,7 @@ __global__ void masks_clear_visited_k(uint8_t *__restrict__ masks, const uint8_t
         rem = m && uniq4(m & 15) >= 0 && uniq4(m >> 4) >= 0;
     }
     const unsigned b = __ballot_sync(0xffffffffu, rem);
+    if ((threadIdx.x & 31) == 0 && i < n) rem_bits[i >> 5] = b;
     if (b && (threadIdx.x & 31) == 0) atomicAdd(remaining, (unsigned long long)__popc(b));
 }
 
@@ -288,11 +310,12 @@ __device__ __forceinline__ uint32_t tc_find_forward(const MphfDev &mk, const uin
     }
 }
 template <int NW>
-__global__ void tc_probe_k(KeyTable t, int64_t n, int K, MphfDev mk, const uint8_t *__restrict__ masks, uint32_t bound, uint8_t *__restrict__ mark,
-                           uint32_t *__restrict__ tipped /*[2n]*/, unsigned long long *__restrict__ stats) {
+__global__ void tc_probe_k(const uint64_t *__restrict__ keys, int64_t base, int64_t n, int K, MphfDev mk, const uint8_t *__restrict__ masks, uint32_t bound,
+                           uint8_t *__restrict__ mark, uint8_t *__restrict__ tipped /*[2 * all k-mers]*/, unsigned long long *__restrict__ stats) {
     const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (tid >= 2 * n) return;
-    const Kmer<NW> key = table_key<NW>(t, tid >> 1);
+    const Kmer<NW> key = key_at<NW>(keys, tid >> 1);
+    tipped += 2 * base;
     const int o = (int)(tid & 1);
     const uint8_t mfw = masks[mphf_lookup_dev<NW>(mk, key)];
     const uint8_t m = o ? inv_byte(mfw) : mfw;
@@ -325,14 +348,14 @@ __global__ void tc_apply_k(uint8_t *__restrict__ masks, const uint8_t *__restric
     if (i < n && mark[i]) masks[i] = 0;
 }
 template <int NW>
-// flags_by_slot = 0: tipped[] is indexed by the thread (table position, orientation), as tc_probe_k writes it; 1: by (MPHF slot, orientation),
+// flags_by_slot = 0: tipped[] is indexed by (k-mer position, orientation), as tc_probe_k writes it; 1: by (MPHF slot, orientation),
 // as at_tips_probe_k marks the roots it reaches by walking
-__global__ void tc_links_k(KeyTable t, int64_t n, int K, MphfDev mk, uint8_t *__restrict__ masks, const uint32_t *__restrict__ tipped,
-                           unsigned long long *__restrict__ stat_clipped, int flags_by_slot) {
+__global__ void tc_links_k(const uint64_t *__restrict__ keys, int64_t base, int64_t n, int K, MphfDev mk, uint8_t *__restrict__ masks,
+                           const uint8_t *__restrict__ tipped, unsigned long long *__restrict__ stat_clipped, int flags_by_slot) {
     const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (tid >= 2 * n) return;
-    if (!flags_by_slot && !tipped[tid]) return;
-    const Kmer<NW> key = table_key<NW>(t, tid >> 1);
+    if (!flags_by_slot && !tipped[2 * base + tid]) return;
+    const Kmer<NW> key = key_at<NW>(keys, tid >> 1);
     const Kmer<NW> kh = (tid & 1) ? kmer_rc<NW>(key, K) : key;
     const CanonIdx<NW> ci = canon_lookup<NW>(mk, kh, K);
     if (flags_by_slot && !tipped[2 * ci.idx + (uint64_t)(tid & 1)]) return;
@@ -379,11 +402,11 @@ __device__ __forceinline__ bool mask_is_junction(uint8_t m) { return uniq4(m & 1
 struct AtParams { double ratio; uint32_t min_len, max_len; };
 
 template <int NW>
-__global__ void at_edges_probe_k(KeyTable t, int64_t n, int K, MphfDev mk, const uint8_t *__restrict__ masks, AtParams ap,
-                                 uint8_t *__restrict__ eflag /*[2n]*/, unsigned long long *__restrict__ stats) {
+__global__ void at_edges_probe_k(const uint64_t *__restrict__ keys, int64_t n, int K, MphfDev mk, const uint8_t *__restrict__ masks, AtParams ap,
+                                 uint8_t *__restrict__ eflag /*[2 * all k-mers]*/, unsigned long long *__restrict__ stats) {
     const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (tid >= 2 * n) return;
-    const Kmer<NW> key = table_key<NW>(t, tid >> 1);
+    const Kmer<NW> key = key_at<NW>(keys, tid >> 1);
     const int o = (int)(tid & 1);
     const uint64_t slot = mphf_lookup_dev<NW>(mk, key);
     const int64_t fid = (int64_t)(2 * slot) + o;                        // flags are indexed by (MPHF slot, orientation), like the masks
@@ -413,11 +436,11 @@ __device__ __forceinline__ void mask_clear_bit(uint8_t *masks, uint64_t idx, uns
     atomicAnd(reinterpret_cast<unsigned *>(masks) + (idx >> 2), ~((1u << bit) << (8 * (idx & 3))));
 }
 template <int NW>
-__global__ void at_edges_apply_k(KeyTable t, int64_t n, int K, MphfDev mk, uint8_t *__restrict__ masks, const uint8_t *__restrict__ eflag,
+__global__ void at_edges_apply_k(const uint64_t *__restrict__ keys, int64_t n, int K, MphfDev mk, uint8_t *__restrict__ masks, const uint8_t *__restrict__ eflag,
                                  unsigned long long *__restrict__ stats) {
     const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (tid >= 2 * n) return;
-    const Kmer<NW> key = table_key<NW>(t, tid >> 1);
+    const Kmer<NW> key = key_at<NW>(keys, tid >> 1);
     const Kmer<NW> kh = (tid & 1) ? kmer_rc<NW>(key, K) : key;
     const CanonIdx<NW> ci = canon_lookup<NW>(mk, kh, K);
     const int64_t fid = (int64_t)(2 * ci.idx) + (tid & 1);               // kh is the table key (minimal form) iff the orientation bit is 0
@@ -439,11 +462,11 @@ __global__ void at_edges_apply_k(KeyTable t, int64_t n, int K, MphfDev mk, uint8
     }
 }
 template <int NW>
-__global__ void at_tips_probe_k(KeyTable t, int64_t n, int K, MphfDev mk, const uint8_t *__restrict__ masks, AtParams ap, uint8_t *__restrict__ mark,
-                                uint32_t *__restrict__ rooted /*[2n]*/, unsigned long long *__restrict__ stats) {
+__global__ void at_tips_probe_k(const uint64_t *__restrict__ keys, int64_t n, int K, MphfDev mk, const uint8_t *__restrict__ masks, AtParams ap,
+                                uint8_t *__restrict__ mark, uint8_t *__restrict__ rooted /*[2 * all k-mers]*/, unsigned long long *__restrict__ stats) {
     const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (tid >= 2 * n) return;
-    const Kmer<NW> key = table_key<NW>(t, tid >> 1);
+    const Kmer<NW> key = key_at<NW>(keys, tid >> 1);
     const int o = (int)(tid & 1);
     const uint64_t idx0 = mphf_lookup_dev<NW>(mk, key);
     const uint8_t mfw = masks[idx0];
@@ -479,31 +502,49 @@ __global__ void at_tips_probe_k(KeyTable t, int64_t n, int K, MphfDev mk, const 
 }
 
 // ---- perfect loops (CollectLoops :359-397). Rare; one thread per candidate / per loop is enough. ---------------------
+// The final_kmers position of each remaining slot, stored densely: pos[rank of the slot among the remaining ones]. rank() is
+// ~0 for a slot that is not remaining. Costs 3/8 B per k-mer plus 8 B per remaining slot.
+struct RemSlots {
+    const uint32_t *bits;      // one bit per MPHF slot
+    const uint64_t *base;      // remaining slots before each 32-slot word (exclusive scan of the words' popcounts)
+    __device__ __forceinline__ uint64_t rank(uint64_t slot) const {
+        const uint32_t w = bits[slot >> 5], bit = 1u << (slot & 31);
+        return (w & bit) ? base[slot >> 5] + (uint64_t)__popc(w & (bit - 1)) : ~0ull;
+    }
+};
+__global__ void popc_words_k(const uint32_t *__restrict__ bits, uint64_t nw, uint32_t *__restrict__ cnt) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < nw) cnt[i] = (uint32_t)__popc(bits[i]);
+}
 template <int NW>
-__global__ void loop_pos_k(KeyTable t, int64_t n, MphfDev mk, uint64_t *__restrict__ pos_of_idx) {
+__global__ void loop_pos_k(const uint64_t *__restrict__ keys, int64_t base, int64_t n, MphfDev mk, RemSlots rs, uint64_t *__restrict__ pos) {
     int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= n) return;
-    pos_of_idx[mphf_lookup_dev<NW>(mk, table_key<NW>(t, j))] = (uint64_t)j;
+    const uint64_t r = rs.rank(mphf_lookup_dev<NW>(mk, key_at<NW>(keys, j)));
+    if (r != ~0ull) pos[r] = (uint64_t)(base + j);
 }
 // leader of a loop = its vertex with the smallest final_kmers position (that is where the serial scan first meets it)
 template <int NW>
-__global__ void loop_leader_k(KeyTable t, int64_t n, int K, MphfDev mk, const uint8_t *__restrict__ masks, const uint64_t *__restrict__ pos_of_idx,
-                              uint32_t *__restrict__ is_leader) {
+// (is_leader: per record of the chunk; nk: all k-mers, the bound of a loop's length)
+__global__ void loop_leader_k(const uint64_t *__restrict__ keys, int64_t base, int64_t n, uint64_t nk, int K, MphfDev mk, const uint8_t *__restrict__ masks,
+                              RemSlots rs, const uint64_t *__restrict__ pos, uint32_t *__restrict__ is_leader) {
     int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= n) return;
     is_leader[j] = 0;
-    const Kmer<NW> key = table_key<NW>(t, j);
+    const Kmer<NW> key = key_at<NW>(keys, j);
     uint64_t idx0;
     uint8_t m = oriented_mask<NW>(mk, masks, key, K, &idx0);
     if (!m || uniq4(m & 15) < 0 || uniq4(m >> 4) < 0) return;
     Kmer<NW> cur = key;
     bool leader = true;
-    for (uint64_t it = 0; it <= (uint64_t)n; ++it) {
+    for (uint64_t it = 0; it <= nk; ++it) {
         kmer_shl<NW>(cur, K, uniq4(m & 15));
         if (kmer_eq<NW>(cur, key)) break;
         uint64_t idx;
         m = oriented_mask<NW>(mk, masks, cur, K, &idx);
-        if (pos_of_idx[idx] < (uint64_t)j) { leader = false; break; }
+        // a loop's vertices are all remaining slots (every other vertex was a junction, a dead end or visited by a path)
+        const uint64_t rk = rs.rank(idx);
+        if (rk != ~0ull && pos[rk] < (uint64_t)(base + j)) { leader = false; break; }
     }
     is_leader[j] = leader ? 1u : 0u;
 }
@@ -511,11 +552,11 @@ __global__ void loop_leader_k(KeyTable t, int64_t n, int K, MphfDev mk, const ui
 // per leader: break point (FindMinimalKMerInLoop :252-262), loop length, self-RC split position (ConstructLoopFromVertex :283-293)
 struct LoopInfo { uint64_t w[4]; uint32_t nverts; int32_t split; };
 template <int NW, int NWS>
-__global__ void loop_probe_k(KeyTable t, const uint64_t *__restrict__ leaders, int64_t nl, int K, MphfDev mk, const uint8_t *__restrict__ masks,
+__global__ void loop_probe_k(const uint64_t *__restrict__ leaders /*keys*/, int64_t nl, int K, MphfDev mk, const uint8_t *__restrict__ masks,
                              LoopInfo *__restrict__ info, uint32_t *__restrict__ len /*[nl*2]*/) {
     int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= nl) return;
-    const Kmer<NW> key = table_key<NW>(t, (int64_t)leaders[q]);
+    const Kmer<NW> key = key_at<NW>(leaders, q);
     Kmer<NW> minimal = key, r = kmer_rc<NW>(key, K);
     if (kmer_nuc_less<NW>(r, minimal)) minimal = r;
     Kmer<NW> cur = key;
@@ -642,6 +683,66 @@ __global__ void loop_write_k(const LoopInfo *__restrict__ info, int64_t nl, int 
 }
 
 // ---- host orchestration ----------------------------------------------------------------------------------------------
+// The chunks of a k-mer set, in order: a device set's own arrays, or a host set's chunks staged through two device buffers (each
+// sweep uploads the set once). Only the sweeps read the sets, so the graph needs the MPHFs, masks and coverage resident, not the sets.
+struct ChunkSource {
+    const KSet *ks;
+    std::unique_ptr<ChunkStager> stage;
+    ChunkSource(const KSet *s, bool counts) : ks(s), stage(s->on_host ? new ChunkStager(s, counts) : nullptr) {}
+    // f(chunk, keys, counts) for every non-empty chunk
+    template <class F>
+    void sweep(F &&f) {
+        for (size_t c = 0; c < ks->chunks.size(); ++c) {
+            const Chunk &ch = ks->chunks[c];
+            const uint64_t *keys = ch.keys.p;
+            const uint32_t *counts = ch.counts.p;
+            if (stage) stage->acquire(c, &keys, &counts);
+            if (ch.n) f(ch, keys, counts);
+            if (stage) stage->release(c);
+        }
+        SG_CUDA(cudaGetLastError());
+    }
+};
+
+// the keys of a sweep's flagged records, in final_kmers order, as one compacted list per chunk that has any (so they are never
+// held twice, as a join would)
+struct KeyParts {
+    std::vector<DArr<uint64_t>> parts;
+    std::vector<uint64_t> sizes;
+    uint64_t total = 0;
+};
+// per chunk: flags -> scan -> compacted keys. flags(ch, keys, flag) fills flag[0, ch.n).
+template <int NW, class Flags>
+static KeyParts collect_keys(Ctx *ctx, ChunkSource &src, Flags &&flags) {
+    cudaStream_t st = ctx->stream;
+    int64_t mx = 1;
+    for (const Chunk &c : src.ks->chunks) mx = std::max(mx, c.n);
+    DArr<uint32_t> flag(ctx, (size_t)mx + 1);
+    DArr<uint64_t> pos(ctx, (size_t)mx + 1);
+    KeyParts kp;
+    src.sweep([&](const Chunk &ch, const uint64_t *keys, const uint32_t *) {
+        SG_CUDA(cudaMemsetAsync(flag.p + ch.n, 0, 4, st));
+        flags(ch, keys, flag.p);
+        exclusive_scan_u32_to_u64(ctx, flag.p, pos.p, (size_t)ch.n + 1);
+        uint64_t m = 0;
+        SG_CUDA(cudaMemcpyAsync(&m, pos.p + ch.n, 8, cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaStreamSynchronize(st));
+        if (!m) return;
+        kp.parts.emplace_back(ctx, (size_t)m * NW);
+        kp.sizes.push_back(m);
+        kp.total += m;
+        compact_keys_k<NW><<<div_up(ch.n, 256), 256, 0, st>>>(flag.p, pos.p, keys, ch.n, kp.parts.back().p);
+        ctx->launches++;
+    });
+    SG_CUDA(cudaStreamSynchronize(st));
+    return kp;
+}
+
+// device bytes a step may still take: what the budget leaves (or 90 % of the arena's free space without one)
+static size_t graph_room(Ctx *ctx) {
+    return ctx->hbm_budget ? (ctx->hbm_budget > ctx->allocated ? ctx->hbm_budget - ctx->allocated : 0) : (size_t)((double)ctx->free_bytes() * 0.90);
+}
+
 template <int NW, int NWS>
 static void graph_build_nw(Ctx *ctx, Graph *g, const GraphOptions &opt) {
     const bool keep_loops = opt.keep_perfect_loops;
@@ -662,48 +763,58 @@ static void graph_build_nw(Ctx *ctx, Graph *g, const GraphOptions &opt) {
     };
     const bool have_cov = g->mkp && kp->has_counts;
     MphfDev mkp = have_cov ? mphf_dev(g->mkp) : MphfDev();
-    // masks
+    // the resident state first, then the staging buffers of the two sets
     g->masks.alloc(ctx, nk + 8, true);
     SG_CUDA(cudaMemsetAsync(g->masks.p, 0, g->masks.bytes(), st));
-    for (const Chunk &c : kp->chunks) {
-        if (!c.n) continue;
-        masks_k<NW, NWS><<<div_up(c.n, 256), 256, 0, st>>>(c.keys.p, c.n, K, mk, reinterpret_cast<unsigned *>(g->masks.p));
-        ctx->launches++;
-    }
-    SG_CUDA(cudaGetLastError());
-    // coverage in MPHF order
     if (have_cov) {
         g->cov.alloc(ctx, (size_t)kp->n + 1, true);
         SG_CUDA(cudaMemsetAsync(g->cov.p, 0, g->cov.bytes(), st));
-        for (const Chunk &c : kp->chunks) {
-            if (!c.n) continue;
-            cov_perm_k<NWS><<<div_up(c.n, 256), 256, 0, st>>>(c.keys.p, c.counts.p, c.n, mkp, g->cov.p);
+    }
+    // masks, and coverage in MPHF order: one sweep over the (k+1)-mers
+    {
+        ChunkSource kps(kp, have_cov);
+        kps.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *counts) {
+            masks_k<NW, NWS><<<div_up(c.n, 256), 256, 0, st>>>(keys, c.n, K, mk, reinterpret_cast<unsigned *>(g->masks.p));
             ctx->launches++;
-        }
-        SG_CUDA(cudaGetLastError());
+            if (have_cov) {
+                cov_perm_k<NWS><<<div_up(c.n, 256), 256, 0, st>>>(keys, counts, c.n, mkp, g->cov.p);
+                ctx->launches++;
+            }
+        });
     }
     SG_CUDA(cudaStreamSynchronize(st));
     trace_mark("masks + coverage");
+    ChunkSource kms(km, false);
     g->tc_stats[0] = g->tc_stats[1] = g->tc_stats[2] = 0;
     for (int i = 0; i < 4; ++i) g->at_stats[i] = 0;
+    // the clippers probe every k-mer on a snapshot of the masks (one whole sweep) before any change is applied
     if (opt.early_at && nk) {
         SG_CHECK(opt.at_min_len <= (uint64_t)K, 2, "early A/T clipper: min_length must not exceed k (the reference indexes kh[k - 1 - i])");
-        KeyTable tt = make_table(km);
         AtParams ap; ap.ratio = opt.at_ratio; ap.min_len = (uint32_t)std::min<uint64_t>(opt.at_min_len, 0x7fffffffu); ap.max_len = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(opt.at_max_len, 1), 0x7fffffffu);
         DArr<uint8_t> eflag(ctx, 2 * nk + 8), mark(ctx, nk + 8);
-        DArr<uint32_t> rooted(ctx, 2 * nk + 1);
+        DArr<uint8_t> rooted(ctx, 2 * nk + 8);
         DArr<unsigned long long> stats(ctx, 4);
         SG_CUDA(cudaMemsetAsync(mark.p, 0, mark.bytes(), st));
         SG_CUDA(cudaMemsetAsync(rooted.p, 0, rooted.bytes(), st));
         SG_CUDA(cudaMemsetAsync(stats.p, 0, 32, st));
-        const int grid2 = div_up((int64_t)(2 * nk), 128);
-        at_edges_probe_k<NW><<<grid2, 128, 0, st>>>(tt, (int64_t)nk, K, mk, g->masks.p, ap, eflag.p, stats.p);
-        at_edges_apply_k<NW><<<grid2, 128, 0, st>>>(tt, (int64_t)nk, K, mk, g->masks.p, eflag.p, stats.p);
-        at_tips_probe_k<NW><<<grid2, 128, 0, st>>>(tt, (int64_t)nk, K, mk, g->masks.p, ap, mark.p, rooted.p, stats.p);
+        kms.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *) {
+            at_edges_probe_k<NW><<<div_up(2 * c.n, 128), 128, 0, st>>>(keys, c.n, K, mk, g->masks.p, ap, eflag.p, stats.p);
+            ctx->launches++;
+        });
+        kms.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *) {
+            at_edges_apply_k<NW><<<div_up(2 * c.n, 128), 128, 0, st>>>(keys, c.n, K, mk, g->masks.p, eflag.p, stats.p);
+            ctx->launches++;
+        });
+        kms.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *) {
+            at_tips_probe_k<NW><<<div_up(2 * c.n, 128), 128, 0, st>>>(keys, c.n, K, mk, g->masks.p, ap, mark.p, rooted.p, stats.p);
+            ctx->launches++;
+        });
         tc_apply_k<<<div_up((int64_t)nk, 256), 256, 0, st>>>(g->masks.p, mark.p, nk);
-        tc_links_k<NW><<<grid2, 128, 0, st>>>(tt, (int64_t)nk, K, mk, g->masks.p, rooted.p, stats.p + 3, 1);
-        ctx->launches += 5;
-        SG_CUDA(cudaGetLastError());
+        ctx->launches++;
+        kms.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *) {
+            tc_links_k<NW><<<div_up(2 * c.n, 128), 128, 0, st>>>(keys, c.first, c.n, K, mk, g->masks.p, rooted.p, stats.p + 3, 1);
+            ctx->launches++;
+        });
         unsigned long long hs[4];
         SG_CUDA(cudaMemcpyAsync(hs, stats.p, 32, cudaMemcpyDeviceToHost, st));
         SG_CUDA(cudaStreamSynchronize(st));
@@ -711,18 +822,22 @@ static void graph_build_nw(Ctx *ctx, Graph *g, const GraphOptions &opt) {
     }
     const uint64_t early_tc_bound = opt.early_tip_length_bound;
     if (early_tc_bound && nk) {
-        KeyTable tt = make_table(km);
         DArr<uint8_t> mark(ctx, nk + 8);
-        DArr<uint32_t> tipped(ctx, 2 * nk + 1);
+        DArr<uint8_t> tipped(ctx, 2 * nk + 8);
         DArr<unsigned long long> stats(ctx, 4);
         SG_CUDA(cudaMemsetAsync(mark.p, 0, mark.bytes(), st));
         SG_CUDA(cudaMemsetAsync(stats.p, 0, 32, st));
         const uint32_t bound = (uint32_t)std::min<uint64_t>(early_tc_bound, 0x7fffffffu);
-        tc_probe_k<NW><<<div_up((int64_t)(2 * nk), 128), 128, 0, st>>>(tt, (int64_t)nk, K, mk, g->masks.p, bound, mark.p, tipped.p, stats.p);
+        kms.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *) {
+            tc_probe_k<NW><<<div_up(2 * c.n, 128), 128, 0, st>>>(keys, c.first, c.n, K, mk, g->masks.p, bound, mark.p, tipped.p, stats.p);
+            ctx->launches++;
+        });
         tc_apply_k<<<div_up((int64_t)nk, 256), 256, 0, st>>>(g->masks.p, mark.p, nk);
-        tc_links_k<NW><<<div_up((int64_t)(2 * nk), 128), 128, 0, st>>>(tt, (int64_t)nk, K, mk, g->masks.p, tipped.p, stats.p + 2, 0);
-        ctx->launches += 3;
-        SG_CUDA(cudaGetLastError());
+        ctx->launches++;
+        kms.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *) {
+            tc_links_k<NW><<<div_up(2 * c.n, 128), 128, 0, st>>>(keys, c.first, c.n, K, mk, g->masks.p, tipped.p, stats.p + 2, 0);
+            ctx->launches++;
+        });
         unsigned long long hs[4];
         SG_CUDA(cudaMemcpyAsync(hs, stats.p, 32, cudaMemcpyDeviceToHost, st));
         SG_CUDA(cudaStreamSynchronize(st));
@@ -733,109 +848,122 @@ static void graph_build_nw(Ctx *ctx, Graph *g, const GraphOptions &opt) {
     if (nk == 0) { SG_CUDA(cudaStreamSynchronize(st)); return; }
 
     trace_mark("early clippers");
-    KeyTable t = make_table(km);
-    // junction list
-    DArr<uint32_t> jflag(ctx, nk + 1);
-    DArr<uint64_t> jpos(ctx, nk + 1);
-    SG_CUDA(cudaMemsetAsync(jflag.p + nk, 0, 4, st));
-    junction_flags_k<NW><<<div_up((int64_t)nk, 256), 256, 0, st>>>(t, (int64_t)nk, K, mk, g->masks.p, jflag.p);
-    ctx->launches++;
-    exclusive_scan_u32_to_u64(ctx, jflag.p, jpos.p, nk + 1);
-    uint64_t njunc = 0;
-    SG_CUDA(cudaMemcpyAsync(&njunc, jpos.p + nk, 8, cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaStreamSynchronize(st));
-    DArr<uint64_t> jlist(ctx, njunc + 1);
-    compact_list_k<<<div_up((int64_t)nk, 256), 256, 0, st>>>(jflag.p, jpos.p, (int64_t)nk, jlist.p);
-    ctx->launches++;
-    jflag.release(); jpos.release();
-    trace_mark("junction list");
-    // probe
-    const uint64_t nslots = njunc * 8;
-    DArr<uint32_t> len(ctx, nslots + 1), keepf(ctx, nslots + 1);
-    DArr<uint8_t> selfc(ctx, nslots + 1);
-    DArr<uint64_t> eidx(ctx, nslots + 1), eoff(ctx, nslots + 1);
-    SG_CUDA(cudaMemsetAsync(len.p, 0, len.bytes(), st));
-    if (nslots) {
-        unitig_probe_k<NW><<<div_up((int64_t)nslots, 128), 128, 0, st>>>(t, jlist.p, (int64_t)njunc, K, mk, g->masks.p, nk, len.p, selfc.p);
+    // junction list: the junctions' keys in final_kmers order, so the unitig kernels never reach into the set
+    KeyParts jk = collect_keys<NW>(ctx, kms, [&](const Chunk &c, const uint64_t *keys, uint32_t *flag) {
+        junction_flags_k<NW><<<div_up(c.n, 256), 256, 0, st>>>(keys, c.n, K, mk, g->masks.p, flag);
         ctx->launches++;
-        SG_CUDA(cudaGetLastError());
-    }
-    exclusive_scan_u32_to_u64(ctx, len.p, eoff.p, nslots + 1);
-    // edge index = rank among kept slots
-    launch_nonzero_flags(ctx, len.p, keepf.p, nslots + 1);
-    exclusive_scan_u32_to_u64(ctx, keepf.p, eidx.p, nslots + 1);
-    uint64_t npaths = 0, nbases = 0;
-    SG_CUDA(cudaMemcpyAsync(&npaths, eidx.p + nslots, 8, cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaMemcpyAsync(&nbases, eoff.p + nslots, 8, cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaStreamSynchronize(st));
-
-    trace_mark("unitig probe + offsets");
-    DArr<char> seq(ctx, nbases + 1);
-    DArr<uint64_t> ls(ctx, npaths + 1), le(ctx, npaths + 1);
-    DArr<uint32_t> rc(ctx, npaths + 1);
+    });
+    trace_mark("junction list");
+    // unbranching paths, in batches of junctions (never across two chunks' lists) sized from the room left: the 8 slots of a
+    // junction cost len + keepf + selfc + eidx + eoff + the compacted (offset, length) = 37 bytes each. The unitig text and link
+    // records of a batch depend on its paths' lengths, not on its junctions: they are reckoned at as much again, a heuristic, and a
+    // batch whose text needs more still runs (blocks beyond the arena come from the driver). Edge numbers and text offsets carry
+    // over from batch to batch.
     DArr<uint8_t> visited(ctx, nk + 8);
     SG_CUDA(cudaMemsetAsync(visited.p, 0, visited.bytes(), st));
-    EdgeOut eo; eo.seq = seq.p; eo.link_start = ls.p; eo.link_end = le.p; eo.raw_cov = rc.p; eo.visited = visited.p;
-    if (nslots) {
-        unitig_write_k<NW, NWS><<<div_up((int64_t)nslots, 128), 128, 0, st>>>(t, jlist.p, (int64_t)njunc, K, mk, g->masks.p, nk, len.p, selfc.p, eidx.p,
+    const uint64_t per_junc = 2 * 8 * 37;
+    const uint64_t jbatch = std::max<uint64_t>(4096, graph_room(ctx) / 2 / per_junc);
+    g->edge_len.clear(); g->edge_off.clear(); g->seq.clear();
+    g->link_start.clear(); g->link_end.clear(); g->raw_cov.clear();
+    uint64_t batches = 0;
+    for (size_t part = 0; part < jk.parts.size(); ++part)
+    for (uint64_t q0 = 0, njunc = jk.sizes[part]; q0 < njunc; q0 += jbatch) {
+        const uint64_t nj = std::min(jbatch, njunc - q0);
+        const uint64_t nslots = nj * 8;
+        ++batches;
+        DArr<uint32_t> len(ctx, nslots + 1), keepf(ctx, nslots + 1);
+        DArr<uint8_t> selfc(ctx, nslots + 1);
+        DArr<uint64_t> eidx(ctx, nslots + 1), eoff(ctx, nslots + 1);
+        SG_CUDA(cudaMemsetAsync(len.p, 0, len.bytes(), st));
+        const uint64_t *bkeys = jk.parts[part].p + q0 * NW;
+        unitig_probe_k<NW><<<div_up((int64_t)nslots, 128), 128, 0, st>>>(bkeys, (int64_t)nj, K, mk, g->masks.p, nk, len.p, selfc.p);
+        ctx->launches++;
+        SG_CUDA(cudaGetLastError());
+        exclusive_scan_u32_to_u64(ctx, len.p, eoff.p, nslots + 1);
+        // edge index = rank among kept slots
+        launch_nonzero_flags(ctx, len.p, keepf.p, nslots + 1);
+        exclusive_scan_u32_to_u64(ctx, keepf.p, eidx.p, nslots + 1);
+        uint64_t npaths = 0, nbases = 0;
+        SG_CUDA(cudaMemcpyAsync(&npaths, eidx.p + nslots, 8, cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaMemcpyAsync(&nbases, eoff.p + nslots, 8, cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaStreamSynchronize(st));
+        trace_mark("unitig probe + offsets");
+        DArr<char> seq(ctx, nbases + 1);
+        DArr<uint64_t> ls(ctx, npaths + 1), le(ctx, npaths + 1);
+        DArr<uint32_t> rc(ctx, npaths + 1);
+        EdgeOut eo; eo.seq = seq.p; eo.link_start = ls.p; eo.link_end = le.p; eo.raw_cov = rc.p; eo.visited = visited.p;
+        unitig_write_k<NW, NWS><<<div_up((int64_t)nslots, 128), 128, 0, st>>>(bkeys, (int64_t)nj, K, mk, g->masks.p, nk, len.p, selfc.p, eidx.p,
                                                                              eoff.p, mkp, have_cov ? g->cov.p : nullptr, eo);
         ctx->launches++;
         SG_CUDA(cudaGetLastError());
-    }
-    trace_mark("unitig write");
-    // download path edges: the (offset, length) table is compacted on the device (8 slots per junction, most of them empty)
-    g->edge_len.assign(npaths, 0); g->edge_off.assign(npaths, 0);
-    DArr<uint64_t> c_off(ctx, npaths + 1);
-    DArr<uint32_t> c_len(ctx, npaths + 1);
-    if (nslots) {
+        trace_mark("unitig write");
+        // download path edges: the (offset, length) table is compacted on the device (8 slots per junction, most of them empty)
+        DArr<uint64_t> c_off(ctx, npaths + 1);
+        DArr<uint32_t> c_len(ctx, npaths + 1);
         edge_table_k<<<div_up((int64_t)nslots, 256), 256, 0, st>>>(len.p, eidx.p, eoff.p, (int64_t)nslots, c_off.p, c_len.p);
         ctx->launches++;
+        const size_t e0 = g->edge_len.size(), b0 = g->seq.size();
+        g->edge_len.resize(e0 + npaths); g->edge_off.resize(e0 + npaths);
+        g->seq.resize(b0 + nbases);
+        g->link_start.resize(e0 + npaths); g->link_end.resize(e0 + npaths); g->raw_cov.resize(e0 + npaths);
+        if (npaths) {
+            SG_CUDA(cudaMemcpyAsync(g->edge_off.data() + e0, c_off.p, npaths * 8, cudaMemcpyDeviceToHost, st));
+            SG_CUDA(cudaMemcpyAsync(g->edge_len.data() + e0, c_len.p, npaths * 4, cudaMemcpyDeviceToHost, st));
+            SG_CUDA(cudaMemcpyAsync(g->link_start.data() + e0, ls.p, npaths * 8, cudaMemcpyDeviceToHost, st));
+            SG_CUDA(cudaMemcpyAsync(g->link_end.data() + e0, le.p, npaths * 8, cudaMemcpyDeviceToHost, st));
+            SG_CUDA(cudaMemcpyAsync(g->raw_cov.data() + e0, rc.p, npaths * 4, cudaMemcpyDeviceToHost, st));
+        }
+        if (nbases) SG_CUDA(cudaMemcpyAsync(&g->seq[b0], seq.p, nbases, cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaStreamSynchronize(st));
+        for (size_t e = e0; e < e0 + npaths; ++e) g->edge_off[e] += b0;
+        if (q0 + nj == njunc) jk.parts[part].release();
+        trace_mark("download + edge table");
     }
-    if (npaths) {
-        SG_CUDA(cudaMemcpyAsync(g->edge_off.data(), c_off.p, npaths * 8, cudaMemcpyDeviceToHost, st));
-        SG_CUDA(cudaMemcpyAsync(g->edge_len.data(), c_len.p, npaths * 4, cudaMemcpyDeviceToHost, st));
-    }
-    g->seq.resize(nbases);
-    g->link_start.resize(npaths); g->link_end.resize(npaths); g->raw_cov.resize(npaths);
-    if (nbases) SG_CUDA(cudaMemcpyAsync(&g->seq[0], seq.p, nbases, cudaMemcpyDeviceToHost, st));
-    if (npaths) {
-        SG_CUDA(cudaMemcpyAsync(g->link_start.data(), ls.p, npaths * 8, cudaMemcpyDeviceToHost, st));
-        SG_CUDA(cudaMemcpyAsync(g->link_end.data(), le.p, npaths * 8, cudaMemcpyDeviceToHost, st));
-        SG_CUDA(cudaMemcpyAsync(g->raw_cov.data(), rc.p, npaths * 4, cudaMemcpyDeviceToHost, st));
-    }
-    SG_CUDA(cudaStreamSynchronize(st));
-    SG_CHECK(g->edge_len.size() == npaths, 6, "internal: path count mismatch");
-    trace_mark("download + edge table");
+    ctx->times.graph_junction_batches = batches;
     if (!keep_loops) return;
     // ---- loops
     DArr<unsigned long long> d_rem(ctx, 1);
     SG_CUDA(cudaMemsetAsync(d_rem.p, 0, 8, st));
-    masks_clear_visited_k<<<div_up((int64_t)nk, 256), 256, 0, st>>>(g->masks.p, visited.p, nk, d_rem.p);
+    const uint64_t nwords = (nk + 31) / 32;
+    DArr<uint32_t> rem_bits(ctx, nwords + 1);
+    masks_clear_visited_k<<<div_up((int64_t)nk, 256), 256, 0, st>>>(g->masks.p, visited.p, nk, d_rem.p, rem_bits.p);
     ctx->launches++;
     unsigned long long rem = 0;
     SG_CUDA(cudaMemcpyAsync(&rem, d_rem.p, 8, cudaMemcpyDeviceToHost, st));
     SG_CUDA(cudaStreamSynchronize(st));
     if (!rem) return;
-    DArr<uint64_t> pos_of_idx(ctx, nk + 1);
-    loop_pos_k<NW><<<div_up((int64_t)nk, 256), 256, 0, st>>>(t, (int64_t)nk, mk, pos_of_idx.p);
-    DArr<uint32_t> lead(ctx, nk + 1);
-    DArr<uint64_t> lpos(ctx, nk + 1);
-    SG_CUDA(cudaMemsetAsync(lead.p + nk, 0, 4, st));
-    loop_leader_k<NW><<<div_up((int64_t)nk, 128), 128, 0, st>>>(t, (int64_t)nk, K, mk, g->masks.p, pos_of_idx.p, lead.p);
-    ctx->launches += 2;
-    exclusive_scan_u32_to_u64(ctx, lead.p, lpos.p, nk + 1);
-    uint64_t nl = 0;
-    SG_CUDA(cudaMemcpyAsync(&nl, lpos.p + nk, 8, cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaStreamSynchronize(st));
+    // final_kmers positions of the remaining slots only (RemSlots): the loop kernels never need 8 B per k-mer
+    DArr<uint64_t> rem_base(ctx, nwords + 1), rem_pos(ctx, rem);
+    {
+        DArr<uint32_t> cnt(ctx, nwords + 1);
+        SG_CUDA(cudaMemsetAsync(cnt.p + nwords, 0, 4, st));
+        popc_words_k<<<div_up((int64_t)nwords, 256), 256, 0, st>>>(rem_bits.p, nwords, cnt.p);
+        ctx->launches++;
+        exclusive_scan_u32_to_u64(ctx, cnt.p, rem_base.p, nwords + 1);
+        SG_CUDA(cudaStreamSynchronize(st));
+    }
+    RemSlots rs; rs.bits = rem_bits.p; rs.base = rem_base.p;
+    kms.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *) {
+        loop_pos_k<NW><<<div_up(c.n, 256), 256, 0, st>>>(keys, c.first, c.n, mk, rs, rem_pos.p);
+        ctx->launches++;
+    });
+    KeyParts lk = collect_keys<NW>(ctx, kms, [&](const Chunk &c, const uint64_t *keys, uint32_t *flag) {
+        loop_leader_k<NW><<<div_up(c.n, 128), 128, 0, st>>>(keys, c.first, c.n, nk, K, mk, g->masks.p, rs, rem_pos.p, flag);
+        ctx->launches++;
+    });
+    rem_pos.release(); rem_base.release(); rem_bits.release();
+    const uint64_t nl = lk.total;
     if (!nl) return;
-    DArr<uint64_t> leaders(ctx, nl + 1);
-    compact_list_k<<<div_up((int64_t)nk, 256), 256, 0, st>>>(lead.p, lpos.p, (int64_t)nk, leaders.p);
+    // the leaders as one list (loops are rare, a few keys)
+    DArr<uint64_t> leaders(ctx, (size_t)nl * NW);
+    for (size_t i = 0, at = 0; i < lk.parts.size(); at += lk.sizes[i], ++i)
+        SG_CUDA(cudaMemcpyAsync(leaders.p + at * NW, lk.parts[i].p, lk.sizes[i] * NW * 8, cudaMemcpyDeviceToDevice, st));
     DArr<LoopInfo> info(ctx, nl);
     DArr<uint32_t> llen(ctx, 2 * nl + 1), lkeep(ctx, 2 * nl + 1), sfull(ctx, nl + 1);
     DArr<uint64_t> leidx(ctx, 2 * nl + 1), leoff(ctx, 2 * nl + 1), soff(ctx, nl + 1);
     SG_CUDA(cudaMemsetAsync(llen.p, 0, llen.bytes(), st));
-    loop_probe_k<NW, NWS><<<div_up((int64_t)nl, 64), 64, 0, st>>>(t, leaders.p, (int64_t)nl, K, mk, g->masks.p, info.p, llen.p);
-    ctx->launches += 2;
+    loop_probe_k<NW, NWS><<<div_up((int64_t)nl, 64), 64, 0, st>>>(leaders.p, (int64_t)nl, K, mk, g->masks.p, info.p, llen.p);
+    ctx->launches++;
     launch_nonzero_flags(ctx, llen.p, lkeep.p, 2 * nl + 1);
     exclusive_scan_u32_to_u64(ctx, llen.p, leoff.p, 2 * nl + 1);
     exclusive_scan_u32_to_u64(ctx, lkeep.p, leidx.p, 2 * nl + 1);
@@ -887,6 +1015,8 @@ Graph *graph_build(Ctx *ctx, const KSet *kp, const KSet *km, const Mphf *mk, con
     SG_CHECK(km->K % 2 == 1, 2, "graph: k must be odd (gbuilder.cpp:125)");
     Graph *g = new Graph();
     g->ctx = ctx; g->k = km->K; g->kp = kp; g->km = km; g->mk = mk; g->mkp = mkp;
+    ctx->times.stage_h2d_bytes = 0;
+    ctx->times.graph_junction_batches = 0;
     try {
         const int nw = km->nw, nws = kp->nw;
         if (nw == 1 && nws == 1) graph_build_nw<1, 1>(ctx, g, opt);

@@ -309,6 +309,7 @@ static void build_nw(Ctx *ctx, const KSet *ks, Mphf *m) {
 Mphf *mphf_build(Ctx *ctx, const KSet *ks) {
     Mphf *m = new Mphf();
     m->ctx = ctx; m->K = ks->K; m->nw = ks->nw; m->B = ks->B; m->n = ks->n;
+    ctx->times.stage_h2d_bytes = 0;
     cudaEvent_t a, b;
     cudaEventCreate(&a); cudaEventCreate(&b);
     cudaEventRecord(a, ctx->stream);

@@ -76,6 +76,10 @@ struct PhaseTimes {   // device milliseconds measured with CUDA events on ctx->s
     // a count whose result goes to host memory: bytes copied there, and host milliseconds spent waiting for those copies
     uint64_t result_d2h_bytes = 0;
     float result_d2h_wait = 0;
+    // host-set chunks uploaded by a ChunkStager (reset by sgpu_kmers_from_kpomers_ex, the MPHF build and the graph builds), and
+    // the junction batches of the last graph build
+    uint64_t stage_h2d_bytes = 0;
+    uint64_t graph_junction_batches = 0;
 };
 
 struct Ctx {
@@ -289,19 +293,23 @@ struct KSet {
     std::vector<int64_t> bstart;       // B+1 exclusive prefix (final_kmers order)
 };
 
-// Brings a host set's chunks to the device one at a time, double-buffered: chunk c + 1 is copied on the context's copy stream
-// while chunk c is used on its stream. acquire(c) makes chunk c readable by work enqueued next on ctx->stream; release(c) marks
-// the end of that work (the chunk's buffer may then take chunk c + 2). Chunks must be acquired in order.
+// Brings a host set's chunks to the device one at a time, double-buffered: chunk c + 1 is copied on the stager's own stream
+// while chunk c is used on the context's stream. acquire(c) makes chunk c readable by work enqueued next on ctx->stream; release(c)
+// marks the end of that work (the chunk's buffer may then take chunk c + 2). Chunks are acquired in order, 0 to the last, and a
+// sweep may start again at chunk 0. The uploads have a stream of their own so that they do not queue behind the result copies of
+// a count that writes to host memory (ResultSink, on ctx->copy).
 struct ChunkStager {
     Ctx *ctx;
     const KSet *ks;
     bool with_counts;
     DArr<uint64_t> keys[2];
     DArr<uint32_t> counts[2];
+    cudaStream_t up = nullptr;
     cudaEvent_t loaded[2] = {nullptr, nullptr}, used[2] = {nullptr, nullptr};
     ChunkStager(const KSet *s, bool counts_too) : ctx(s->ctx), ks(s), with_counts(counts_too && s->has_counts) {
         size_t mx = 1;
         for (const Chunk &c : ks->chunks) mx = std::max(mx, (size_t)c.n);
+        SG_CUDA(cudaStreamCreateWithFlags(&up, cudaStreamNonBlocking));
         for (int i = 0; i < 2; ++i) {
             keys[i].alloc(ctx, mx * ks->nw);
             if (with_counts) counts[i].alloc(ctx, mx);
@@ -311,7 +319,7 @@ struct ChunkStager {
     }
     ~ChunkStager() {
         // the buffers go back to the arena: no copy may still be writing them
-        if (ctx->copy) cudaStreamSynchronize(ctx->copy);
+        if (up) { cudaStreamSynchronize(up); cudaStreamDestroy(up); }
         for (int i = 0; i < 2; ++i) { if (loaded[i]) cudaEventDestroy(loaded[i]); if (used[i]) cudaEventDestroy(used[i]); }
     }
     ChunkStager(const ChunkStager &) = delete;
@@ -319,13 +327,13 @@ struct ChunkStager {
     void prefetch(size_t c) {
         const Chunk &ch = ks->chunks[c];
         const int s = (int)(c & 1);
-        cudaStream_t cs = ctx->copy_stream();
-        SG_CUDA(cudaStreamWaitEvent(cs, used[s], 0));
+        SG_CUDA(cudaStreamWaitEvent(up, used[s], 0));
         if (ch.n) {
-            SG_CUDA(cudaMemcpyAsync(keys[s].p, ch.h_keys.p, (size_t)ch.n * ks->nw * 8, cudaMemcpyHostToDevice, cs));
-            if (with_counts) SG_CUDA(cudaMemcpyAsync(counts[s].p, ch.h_counts.p, (size_t)ch.n * 4, cudaMemcpyHostToDevice, cs));
+            SG_CUDA(cudaMemcpyAsync(keys[s].p, ch.h_keys.p, (size_t)ch.n * ks->nw * 8, cudaMemcpyHostToDevice, up));
+            if (with_counts) SG_CUDA(cudaMemcpyAsync(counts[s].p, ch.h_counts.p, (size_t)ch.n * 4, cudaMemcpyHostToDevice, up));
+            ctx->times.stage_h2d_bytes += (uint64_t)ch.n * ks->nw * 8 + (with_counts ? (uint64_t)ch.n * 4 : 0);
         }
-        SG_CUDA(cudaEventRecord(loaded[s], cs));
+        SG_CUDA(cudaEventRecord(loaded[s], up));
     }
     void acquire(size_t c, const uint64_t **k, const uint32_t **cnt) {
         if (c == 0) prefetch(0);
@@ -369,7 +377,7 @@ void cov_filter(Ctx *ctx, int K, unsigned thr, int apply, uint8_t *keep_out, uin
 // count.cu
 enum CountMode { kCanonical = 0, kAllWindows = 1 };
 KSet *count_from_reads(Ctx *ctx, int K, int B, int mode, bool result_on_host = false);
-KSet *kmers_from_kpomers(Ctx *ctx, const KSet *kp, int B);
+KSet *kmers_from_kpomers(Ctx *ctx, const KSet *kp, int B, bool result_on_host = false);
 
 void kset_checksum(const KSet *ks, uint64_t *out4);
 

@@ -164,7 +164,8 @@ class DeBruijnKMerKMerSplitter:
 
 
 class KMerDiskCounter:
-    """result_on_host: the counted set goes to pinned host memory, pass by pass behind the next one, so it may exceed HBM."""
+    """result_on_host: the counted set goes to pinned host memory, pass by pass behind the next one, so it may exceed HBM. The
+    (k+1)-mers of a DeBruijnKMerKMerSplitter may live in either place."""
 
     def __init__(self, ctx: Context, splitter, result_on_host=False):
         self.ctx, self.splitter, self.result_on_host = ctx, splitter, result_on_host
@@ -172,7 +173,8 @@ class KMerDiskCounter:
     def Count(self, num_buckets, num_threads=0):
         h = C.c_void_p()
         if isinstance(self.splitter, DeBruijnKMerKMerSplitter):
-            rc = self.ctx.L.sgpu_kmers_from_kpomers(self.ctx.h, self.splitter.source.h, num_buckets, C.byref(h))
+            mode = SGPU_RESULT_ON_HOST if self.result_on_host else 0
+            rc = self.ctx.L.sgpu_kmers_from_kpomers_ex(self.ctx.h, self.splitter.source.h, num_buckets, mode, C.byref(h))
         else:
             mode = self.splitter.mode | (SGPU_RESULT_ON_HOST if self.result_on_host else 0)
             rc = self.ctx.L.sgpu_count(self.ctx.h, self.splitter.K, num_buckets, mode, C.byref(h))
