@@ -22,6 +22,7 @@
 #include <chrono>
 #include <memory>
 
+#include "pass_plan.h"
 #include "sgpu_internal.h"
 
 namespace sg {
@@ -1563,13 +1564,56 @@ struct ResultSink {
     }
 };
 
-// refinement + local sort + compaction of one pass: X holds the level-A output (CTA-major pieces when `pieces` is given, else
-// partition-major with the given starts/totals), Y is the ping-pong partner of the same size. With a sink, the previous pass's
-// chunk is drained just before this pass allocates its own output.
+// Puts a counted set together pass by pass: every pass appends one chunk, in bucket order, compact_k adds each bucket's records
+// to d_bsz, and finish() fills in the bucket sizes and hands the set over. With SGPU_RESULT_ON_HOST every chunk is copied to host
+// memory behind the next pass (ResultSink).
+struct KSetBuilder {
+    Ctx *ctx;
+    std::unique_ptr<KSet> ks;                // the set under construction, deleted with the builder unless finish() handed it over
+    DArr<unsigned long long> d_bsz;          // records per bucket
+    int64_t first = 0;                       // records in the chunks appended so far
+    bool double_selfrc;                      // canonical count at even K: a self-RC (k+1)-mer is seen in the read and in its RC
+    std::unique_ptr<ResultSink> sink;        // declared after `ks`, so destroyed first: no copy outlives the set
+    KSetBuilder(Ctx *c, int K, int nw, int B, bool counts, bool double_selfrc_, bool on_host) : ctx(c), ks(new KSet()), double_selfrc(double_selfrc_) {
+        ks->ctx = c; ks->K = K; ks->nw = nw; ks->B = B; ks->has_counts = counts; ks->on_host = on_host;
+        if (on_host) sink.reset(new ResultSink(c, ks.get()));
+        d_bsz.alloc(c, (size_t)B);
+        SG_CUDA(cudaMemsetAsync(d_bsz.p, 0, (size_t)B * 8, c->stream));
+    }
+    // the chunk of the next pass, n records of buckets [b_lo, b_hi); the previous chunk's copy is drained first
+    Chunk &open(int b_lo, int b_hi, uint64_t n) {
+        if (sink) sink->drain();
+        ks->chunks.emplace_back();
+        Chunk &ch = ks->chunks.back();
+        ch.n = (int64_t)n; ch.b_lo = b_lo; ch.b_hi = b_hi; ch.first = first;
+        ch.keys.alloc(ctx, (size_t)n * ks->nw + 2, true);
+        if (ks->has_counts) ch.counts.alloc(ctx, (size_t)n + 1, true);
+        return ch;
+    }
+    // the chunk open() returned has been compacted on ctx->stream
+    void close() {
+        first += ks->chunks.back().n;
+        if (sink) sink->push();
+    }
+    KSet *finish() {
+        if (sink) { sink->drain(); sink.reset(); }
+        const int B = ks->B;
+        std::vector<unsigned long long> hb(B);
+        SG_CUDA(cudaMemcpyAsync(hb.data(), d_bsz.p, (size_t)B * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        SG_CUDA(cudaStreamSynchronize(ctx->stream));
+        ks->bsz.assign(B, 0); ks->bstart.assign(B + 1, 0);
+        for (int b = 0; b < B; ++b) { ks->bsz[b] = (int64_t)hb[b]; ks->bstart[b + 1] = ks->bstart[b] + ks->bsz[b]; }
+        ks->n = first;
+        SG_CHECK(ks->bstart[B] == ks->n, 6, "internal: bucket sizes do not add up");
+        return ks.release();
+    }
+};
+
+// refinement + local sort + compaction of one pass into the next chunk of `set`: X holds the level-A output (CTA-major pieces when
+// `pieces` is given, else partition-major with the given starts/totals), Y is the ping-pong partner of the same size
 template <int NW>
 static void sort_pass(Ctx *ctx, int K, DArr<uint64_t> &X, DArr<uint64_t> &Y, const uint64_t *part_start_p, const uint64_t *part_total_p, uint32_t PA,
-                      int rA_, uint32_t b_lo, int b_hi, int64_t first, bool want_counts, bool double_selfrc, unsigned long long *d_bsz_p, Chunk &ch_out,
-                      Timer &tm, Trace &tr, const Pieces *pieces = nullptr, ResultSink *sink = nullptr) {
+                      int rA_, uint32_t b_lo, int b_hi, KSetBuilder &set, Timer &tm, Trace &tr, const Pieces *pieces = nullptr) {
     constexpr int CAP = SortCfg<NW>::CAP;
     const int total_bits = 2 * K;
     cudaStream_t st = ctx->stream;
@@ -1656,21 +1700,17 @@ static void sort_pass(Ctx *ctx, int K, DArr<uint64_t> &X, DArr<uint64_t> &Y, con
     ctx->times.sort_lsd_fallbacks += h_stats[1];
     ctx->times.sort_oversize_equal += h_stats[2];
     // ---- compaction into the dense chunk
-    if (sink) sink->drain();
-    Chunk ch;
-    ch.n = (int64_t)D; ch.b_lo = (int)b_lo; ch.b_hi = b_hi; ch.first = first;
-    ch.keys.alloc(ctx, (size_t)D * NW + 2, true);
-    if (want_counts) ch.counts.alloc(ctx, (size_t)D + 1, true);
+    Chunk &ch = set.open((int)b_lo, b_hi, D);
     tm.start();
     if (nsegs) {
-        compact_k<NW><<<div_up((int64_t)nsegs * 32, 256), 256, 0, st>>>(segs.p, nsegs, ndist.p, dbase.p, X.p, Y.p, K, want_counts ? 1 : 0,
-                                                                     double_selfrc ? 1 : 0, ch.keys.p, ch.counts.p, d_bsz_p);
+        compact_k<NW><<<div_up((int64_t)nsegs * 32, 256), 256, 0, st>>>(segs.p, nsegs, ndist.p, dbase.p, X.p, Y.p, K, set.ks->has_counts ? 1 : 0,
+                                                                     set.double_selfrc ? 1 : 0, ch.keys.p, ch.counts.p, set.d_bsz.p);
         ctx->launches++;
         SG_CUDA(cudaGetLastError());
     }
     ctx->times.compact += tm.stop();
     tr.mark("compact");
-    ch_out = std::move(ch);
+    set.close();
 }
 
 // ---- level A as a job: one histogram (+ partition id) pass over the source, then one scatter per bucket-group pass -----------
@@ -1859,17 +1899,12 @@ static void levelA_scatter(LevelAJob<NW, Src, BOTH> &job, int b_lo, int b_hi, ui
 static double pass_bytes_needed(uint64_t recs, size_t W) { return (double)recs * W * 2.0 + (double)recs * (W + 4) * 0.6 + (64 << 20); }
 
 template <int NW, bool BOTH, class Src>
-static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, int B, bool want_counts, bool double_selfrc, uint64_t est_records, KSet *out,
-                      ResultSink *sink = nullptr, ChunkStager *stage = nullptr) {
-    const int total_bits = 2 * K;
+static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, uint64_t est_records, KSetBuilder &set, ChunkStager *stage = nullptr) {
+    const int total_bits = 2 * K, B = set.ks->B;
     const size_t W = 8 * NW;
     cudaStream_t st = ctx->stream;
     Timer tm(st);
     Trace tr(st);
-
-    out->bsz.assign(B, 0);
-    DArr<unsigned long long> d_bsz(ctx, B);
-    SG_CUDA(cudaMemsetAsync(d_bsz.p, 0, B * sizeof(unsigned long long), st));
 
     // ---- level-A geometry for the whole job. Partition id = (bucket, top rA key bits). ONE histogram pass over the
     // source serves every bucket-group pass (the groups are contiguous partition ranges), so a multi-pass job hashes
@@ -1881,58 +1916,25 @@ static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, int B, bool
     // share of the chunks still free. There are at most 128 super-ranges (B <= 2^20 with SR = 8192 when rA = 0, a single one
     // when rA > 0), so every share is at least one pass.
     const int n_ranges = (B + SR - 1) / SR;
-    int64_t first = 0;
     for (int s_lo = 0; s_lo < B; s_lo += SR) {
-        const int share = (kMaxChunks - (int)out->chunks.size()) / (n_ranges - s_lo / SR);
+        const int share = (kMaxChunks - (int)set.ks->chunks.size()) / (n_ranges - s_lo / SR);
         LevelAJob<NW, Src, BOTH> job;
         job.ctx = ctx; job.srcs = srcs; job.K = K; job.B = B; job.rA = rA; job.G = ctx->num_sms * levelA_ctas_per_sm(); job.stage = stage;
         job.s_lo = s_lo; job.s_hi = std::min(B, s_lo + SR);
         job.PA_all = (uint32_t)(job.s_hi - job.s_lo) << rA;
         levelA_count(job, tm, tr);
-        // bucket-group passes: simulate the greedy "as many whole buckets as fit" plan to learn how many passes are needed, then
-        // aim for equally sized passes (a tiny last pass still costs a full scan of the source), at most `share` of them
-        auto current_limit = [&]() {
-            return ctx->hbm_budget ? (ctx->hbm_budget > ctx->allocated ? ctx->hbm_budget - ctx->allocated : 0) : (size_t)(ctx->free_bytes() * 0.90);
-        };
-        uint64_t total_records = 0;
-        for (int b = job.s_lo; b < job.s_hi; ++b) total_records += job.bucket_records(b);
-        uint64_t pass_target = total_records;
-        bool capped = false;
-        {
-            // a set that goes to host memory keeps only the previous pass's output on the device, while it is copied
-            double lim_sim = (double)current_limit(), inflight = 0;
-            int npass_sim = 0, b = job.s_lo;
-            while (b < job.s_hi) {
-                uint64_t I = 0; const int b0 = b;
-                while (b < job.s_hi) {
-                    const uint64_t ib = job.bucket_records(b);
-                    if (b > b0 && pass_bytes_needed(I + ib, W) + inflight > lim_sim) break;
-                    I += ib; ++b;
-                }
-                if (sink) inflight = (double)I * (W + 4) * 0.5;
-                else lim_sim -= (double)I * (W + 4) * 0.5;     // this pass's output stays resident
-                ++npass_sim;
-            }
-            capped = npass_sim > share;
-            pass_target = total_records / (uint64_t)std::min(npass_sim, share) + total_records / 64 + 1;
-        }
-        int b_lo = job.s_lo, npass = 0;
-        while (b_lo < job.s_hi) {
-            // ---- plan this pass: whole buckets that fit next to what is already resident (X + Y + its own output). When the
-            // budget would need more passes than the range's share of chunks (or this is the share's last pass), the pass takes
-            // at least an even split of the buckets left, above the budget if need be: the budget is a planning target (blocks
-            // beyond the arena come from the driver), a device that really lacks the memory fails with SGPU_ENOMEM.
-            const int left = share - npass;
-            const int min_b = (capped || left == 1) ? div_up(job.s_hi - b_lo, left) : 1;
-            const size_t lim = current_limit();
-            int b_hi = b_lo;
-            uint64_t I = 0;
-            while (b_hi < job.s_hi) {
-                const uint64_t ib = job.bucket_records(b_hi);
-                if (b_hi - b_lo >= min_b && (pass_bytes_needed(I + ib, W) > (double)lim || I + ib > pass_target)) break;
-                I += ib; ++b_hi;
-            }
-            ++npass;
+        // bucket-group passes against what the budget leaves now. Blocks beyond the arena come from the driver, so a pass may go
+        // above the budget; a device that really lacks the memory fails with SGPU_ENOMEM.
+        std::vector<uint64_t> before(job.s_hi - job.s_lo + 1, 0);
+        for (int b = job.s_lo; b < job.s_hi; ++b) before[b - job.s_lo + 1] = before[b - job.s_lo] + job.bucket_records(b);
+        PassPlan plan(job.s_lo, job.s_hi, share, std::move(before));
+        const uint64_t total_records = plan.records(job.s_lo, job.s_hi);
+        auto need = [&](int a, int b) { return pass_bytes_needed(plan.records(a, b), W); };
+        // a set that goes to host memory keeps only the previous pass's output on the device, while it is copied
+        plan.aim((double)ctx->budget_left(), set.sink != nullptr, need, [&](int a, int b) { return (double)plan.records(a, b) * (W + 4) * 0.5; });
+        while (!plan.done()) {
+            const int b_lo = plan.bounds.back(), b_hi = plan.next((double)ctx->budget_left(), need);
+            const uint64_t I = plan.records(b_lo, b_hi);
             const uint32_t p_lo = (uint32_t)(b_lo - job.s_lo) << rA;
             const uint32_t PA = (uint32_t)(b_hi - b_lo) << rA;
             DArr<uint64_t> part_total(ctx, PA + 1), part_start(ctx, PA + 1);
@@ -1945,23 +1947,9 @@ static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, int B, bool
             DArr<uint64_t> pbase(ctx, (size_t)job.G * PA);
             Pieces pcs;
             levelA_scatter(job, b_lo, b_hi, I, total_records, X.p, pbase.p, pcs, tm, tr);
-            Chunk ch;
-            sort_pass<NW>(ctx, K, X, Y, part_start.p, part_total.p, PA, rA, (uint32_t)b_lo, b_hi, first, want_counts, double_selfrc, d_bsz.p, ch, tm, tr, &pcs,
-                          sink);
-            first += ch.n;
-            out->chunks.push_back(std::move(ch));
-            if (sink) sink->push();
-            b_lo = b_hi;
+            sort_pass<NW>(ctx, K, X, Y, part_start.p, part_total.p, PA, rA, (uint32_t)b_lo, b_hi, set, tm, tr, &pcs);
         }
     }
-    if (sink) sink->drain();
-    std::vector<unsigned long long> hb(B);
-    SG_CUDA(cudaMemcpyAsync(hb.data(), d_bsz.p, B * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaStreamSynchronize(st));
-    out->bstart.assign(B + 1, 0);
-    for (int b = 0; b < B; ++b) { out->bsz[b] = (int64_t)hb[b]; out->bstart[b + 1] = out->bstart[b] + out->bsz[b]; }
-    out->n = first;
-    SG_CHECK(out->bstart[B] == out->n, 6, "internal: bucket sizes do not add up");
 }
 
 __global__ void count_windows_k(const uint32_t *__restrict__ lens, int64_t n, int K, unsigned long long *__restrict__ out) {
@@ -1997,16 +1985,13 @@ static ReadsSrc reads_source(Ctx *ctx, int K) {
 template <int NW>
 static KSet *count_reads_nw(Ctx *ctx, int K, int B, int mode, bool on_host) {
     ensure_reads_on_device(ctx);
-    KSet *ks = new KSet();
-    ks->ctx = ctx; ks->K = K; ks->nw = NW; ks->B = B; ks->has_counts = (mode == kCanonical); ks->on_host = on_host;
-    try {
-        std::unique_ptr<ResultSink> sink(on_host ? new ResultSink(ctx, ks) : nullptr);   // gone before `ks` is: no copy outlives the set
-        const uint64_t wn = count_windows(ctx, K);
-        std::vector<ReadsSrc> srcs{reads_source(ctx, K)};
-        if (mode == kAllWindows) run_count<NW, true>(ctx, srcs, K, B, false, false, wn * 2, ks, sink.get());
-        else run_count<NW, false>(ctx, srcs, K, B, true, K % 2 == 0, wn, ks, sink.get());
-    } catch (...) { delete ks; throw; }
-    return ks;
+    const uint64_t wn = count_windows(ctx, K);
+    std::vector<ReadsSrc> srcs{reads_source(ctx, K)};
+    const bool canonical = mode == kCanonical;
+    KSetBuilder set(ctx, K, NW, B, canonical, canonical && K % 2 == 0, on_host);
+    if (canonical) run_count<NW, false>(ctx, srcs, K, wn, set);
+    else run_count<NW, true>(ctx, srcs, K, wn * 2, set);
+    return set.finish();
 }
 
 KSet *count_from_reads(Ctx *ctx, int K, int B, int mode, bool result_on_host) {
@@ -2024,21 +2009,17 @@ KSet *count_from_reads(Ctx *ctx, int K, int B, int mode, bool result_on_host) {
 template <int NW>
 static KSet *kmers_from_kpomers_nw(Ctx *ctx, const KSet *kp, int B, bool on_host) {
     const int K = kp->K - 1;
-    KSet *ks = new KSet();
-    ks->ctx = ctx; ks->K = K; ks->nw = NW; ks->B = B; ks->has_counts = false; ks->on_host = on_host;
-    try {
-        std::unique_ptr<ResultSink> sink(on_host ? new ResultSink(ctx, ks) : nullptr);
-        // a host (k+1)-mer set: every launch that reads a chunk's words reads its staged copy. Allocated before the passes are
-        // planned, so the planner sees the two staging buffers.
-        std::unique_ptr<ChunkStager> stage(kp->on_host ? new ChunkStager(kp, false) : nullptr);
-        std::vector<KmerSetSrc> srcs;
-        for (const Chunk &c : kp->chunks) {
-            KmerSetSrc s; s.words = c.keys.p; s.n = c.n; s.nwords = (uint64_t)c.n * kp->nw; s.K = K; s.stride = (uint32_t)kp->nw;
-            srcs.push_back(s);
-        }
-        run_count<NW, false>(ctx, srcs, K, B, false, false, (uint64_t)kp->n * 2, ks, sink.get(), stage.get());
-    } catch (...) { delete ks; throw; }
-    return ks;
+    // a host (k+1)-mer set: every launch that reads a chunk's words reads its staged copy. Allocated before the passes are
+    // planned, so the planner sees the two staging buffers.
+    std::unique_ptr<ChunkStager> stage(kp->on_host ? new ChunkStager(kp, false) : nullptr);
+    std::vector<KmerSetSrc> srcs;
+    for (const Chunk &c : kp->chunks) {
+        KmerSetSrc s; s.words = c.keys.p; s.n = c.n; s.nwords = (uint64_t)c.n * kp->nw; s.K = K; s.stride = (uint32_t)kp->nw;
+        srcs.push_back(s);
+    }
+    KSetBuilder set(ctx, K, NW, B, false, false, on_host);
+    run_count<NW, false>(ctx, srcs, K, (uint64_t)kp->n * 2, set, stage.get());
+    return set.finish();
 }
 
 KSet *kmers_from_kpomers(Ctx *ctx, const KSet *kp, int B, bool result_on_host) {
@@ -2112,14 +2093,14 @@ void kset_checksum(const KSet *ks, uint64_t *out4) {
 struct DistPlan {
     int world = 1, rank = 0, B = 0, rA = 0;
     uint32_t PA_all = 0;
-    std::vector<int> pass_b;                   // bucket boundaries of the passes planned so far (starts as {0})
+    PassPlan passes;                           // over all B buckets
     std::vector<uint64_t> tot;                 // PA_all: records per partition summed over ranks
     std::vector<uint64_t> Tb;                  // B+1: records in buckets < b, all ranks
     std::vector<uint64_t> Ps;                  // world x (B+1): records of rank s in buckets < b
-    uint64_t pass_target = 0;                  // records per pass aimed for (equal passes: a tiny last pass still costs a full id sweep)
-    int npass() const { return (int)pass_b.size() - 1; }
+    int npass() const { return passes.npass(); }
+    int pass_lo(int p) const { return passes.bounds[p]; }
     static int own_lo_of(int b_lo, int b_hi, int world, int g) { return b_lo + (int)((int64_t)(b_hi - b_lo) * g / world); }
-    int own_lo(int p, int g) const { return own_lo_of(pass_b[p], pass_b[p + 1], world, g); }
+    int own_lo(int p, int g) const { return own_lo_of(pass_lo(p), pass_lo(p + 1), world, g); }
     // largest number of records an owner receives / a rank sends if [b_lo, b_hi) is one pass
     void maxima(int b_lo, int b_hi, uint64_t *mx, uint64_t *ms) const {
         *mx = 0; *ms = 0;
@@ -2138,6 +2119,7 @@ static double dist_pass_bytes(uint64_t mx, uint64_t ms, size_t W, uint64_t fixed
 
 // pure host functions (also exported for the CPU/gloo tests): identical on every rank given the same inputs
 void dist_plan_tables(DistPlan &pl, int world, int rank, int B, int rA, const uint64_t *cnt_all) {
+    SG_CHECK(rA >= 0 && ((uint64_t)B << rA) <= (uint64_t)kLevelAMaxParts, 2, "distributed count: more level-A partitions than one launch can address");
     pl.world = world; pl.rank = rank; pl.B = B; pl.rA = rA; pl.PA_all = (uint32_t)B << rA;
     pl.tot.assign(pl.PA_all, 0);
     pl.Tb.assign((size_t)B + 1, 0);
@@ -2155,43 +2137,17 @@ void dist_plan_tables(DistPlan &pl, int world, int rank, int B, int rA, const ui
         for (int s = 0; s < world; ++s) t += pl.Ps[(size_t)s * (B + 1) + b];
         pl.Tb[b] = t;
     }
-    pl.pass_b.assign(1, 0);
-    pl.pass_target = 0;
-}
-// the greedy "as many whole buckets as fit" step shared by the simulation and the real planning: returns b_hi > b_lo
-static int dist_greedy_pass(const DistPlan &pl, int b_lo, double budget, size_t W, uint64_t fixed_bytes, uint64_t target) {
-    int b_hi = b_lo;
-    while (b_hi < pl.B) {
-        uint64_t mx, ms;
-        pl.maxima(b_lo, b_hi + 1, &mx, &ms);
-        const uint64_t recs = pl.Tb[b_hi + 1] - pl.Tb[b_lo];
-        if (b_hi > b_lo && (dist_pass_bytes(mx, ms, W, fixed_bytes) > budget || (target && recs > target) ||
-                            ((size_t)(b_hi + 1 - b_lo) << pl.rA) > (size_t)kLevelAMaxParts)) break;
-        ++b_hi;
-    }
-    return b_hi;
+    pl.passes = PassPlan(0, B, kMaxChunks, pl.Tb);
 }
 // plan the next pass against `budget_bytes` = what every rank can allocate NOW (minimum over ranks). Returns false when all
 // buckets are done. The first call also fixes the pass size aimed for by simulating the whole job (outputs of earlier passes
 // stay resident: ~half a record's bytes per record, as measured on read sets with errors).
 bool dist_next_pass(DistPlan &pl, uint64_t budget_bytes, size_t W, uint64_t fixed_bytes, uint64_t *mx_out, uint64_t *ms_out) {
-    const int b_lo = pl.pass_b.back();
-    if (b_lo >= pl.B) return false;
-    if (pl.pass_target == 0) {
-        double lim = (double)budget_bytes;
-        int np = 0, b = 0;
-        while (b < pl.B) {
-            const int e = dist_greedy_pass(pl, b, lim, W, fixed_bytes, 0);
-            uint64_t mx, ms;
-            pl.maxima(b, e, &mx, &ms);
-            lim -= (double)mx * (W + 4) * 0.5;
-            b = e; ++np;
-        }
-        const uint64_t total = pl.Tb[pl.B];
-        pl.pass_target = total / (uint64_t)np + total / 64 + 1;
-    }
-    const int b_hi = dist_greedy_pass(pl, b_lo, (double)budget_bytes, W, fixed_bytes, pl.pass_target);
-    pl.pass_b.push_back(b_hi);
+    if (pl.passes.done()) return false;
+    auto need = [&](int a, int b) { uint64_t mx, ms; pl.maxima(a, b, &mx, &ms); return dist_pass_bytes(mx, ms, W, fixed_bytes); };
+    if (pl.npass() == 0)
+        pl.passes.aim((double)budget_bytes, false, need, [&](int a, int b) { uint64_t mx, ms; pl.maxima(a, b, &mx, &ms); return (double)mx * (W + 4) * 0.5; });
+    const int b_lo = pl.passes.bounds.back(), b_hi = pl.passes.next((double)budget_bytes, need);
     pl.maxima(b_lo, b_hi, mx_out, ms_out);
     return true;
 }
@@ -2206,13 +2162,8 @@ struct DistState {
     DArr<uint64_t> sbuf, xbuf;               // staging buffer (peers read it; later the ping-pong partner) and the merged buffer
     DArr<uint64_t> pbase;                    // [G][max partitions of a pass]: piece starts of the current pass (peers read it)
     std::vector<PullSrc> peers;              // world entries (own entry = local pointers)
-    DArr<unsigned long long> d_bsz;
-    KSet *out = nullptr;
-    std::unique_ptr<ResultSink> sink;        // SGPU_RESULT_ON_HOST: each pass's chunk is copied to host memory behind the next pass
-    bool result_on_host = false;
-    int64_t first = 0;
-    bool want_counts = false, double_selfrc = false;
-    virtual ~DistState() { sink.reset(); delete out; }
+    std::unique_ptr<KSetBuilder> set;        // this rank's buckets, until sgpu_dist_end hands them over
+    virtual ~DistState() = default;
     virtual void begin() = 0;
     virtual void local_counts(uint64_t *h_out) = 0;
     virtual const uint32_t *blk_counts_ptr() = 0;
@@ -2308,7 +2259,7 @@ struct DistStateNW : DistState {
         // local partition of this rank's shard for the pass's buckets into the staging buffer (CTA-major pieces)
         Timer tm(ctx->stream);
         Trace tr(ctx->stream);
-        const int b_lo = plan.pass_b[p], b_hi = plan.pass_b[p + 1];
+        const int b_lo = plan.pass_lo(p), b_hi = plan.pass_lo(p + 1);
         uint64_t I = 0, total = 0;
         for (uint32_t q = 0; q < plan.PA_all; ++q) {
             const uint64_t c = h_cnt_all[(size_t)plan.rank * plan.PA_all + q];
@@ -2324,8 +2275,8 @@ struct DistStateNW : DistState {
     void pull(int p) override {
         cudaStream_t st = ctx->stream;
         const int world = plan.world;
-        const uint32_t pq0 = (uint32_t)plan.pass_b[p] << plan.rA;
-        const uint32_t PAp = (uint32_t)(plan.pass_b[p + 1] - plan.pass_b[p]) << plan.rA;
+        const uint32_t pq0 = (uint32_t)plan.pass_lo(p) << plan.rA;
+        const uint32_t PAp = (uint32_t)(plan.pass_lo(p + 1) - plan.pass_lo(p)) << plan.rA;
         const uint32_t q0 = (uint32_t)plan.own_lo(p, plan.rank) << plan.rA, q1 = (uint32_t)plan.own_lo(p, plan.rank + 1) << plan.rA;
         const uint32_t nq = q1 - q0;
         if (nq == 0) return;
@@ -2364,24 +2315,17 @@ struct DistStateNW : DistState {
         for (uint32_t q = 0; q < PA; ++q) { tot[q] = plan.tot[Q0 + q]; start[q + 1] = start[q] + tot[q]; }
         ctx->times.passes++;
         ctx->times.instances += start[PA];
-        Chunk ch;
         if (PA && start[PA]) {
             DArr<uint64_t> d_tot(ctx, PA + 1), d_start(ctx, PA + 1);
             SG_CUDA(cudaMemcpyAsync(d_tot.p, tot.data(), (size_t)(PA + 1) * 8, cudaMemcpyHostToDevice, st));
             SG_CUDA(cudaMemcpyAsync(d_start.p, start.data(), (size_t)(PA + 1) * 8, cudaMemcpyHostToDevice, st));
             Timer tm(st);
             Trace tr(st);
-            sort_pass<NW>(ctx, K, xbuf, sbuf, d_start.p, d_tot.p, PA, plan.rA, (uint32_t)my_lo, my_hi, first, want_counts, double_selfrc, d_bsz.p, ch, tm, tr,
-                          nullptr, sink.get());
+            sort_pass<NW>(ctx, K, xbuf, sbuf, d_start.p, d_tot.p, PA, plan.rA, (uint32_t)my_lo, my_hi, *set, tm, tr);
         } else {
-            if (sink) sink->drain();
-            ch.n = 0; ch.b_lo = my_lo; ch.b_hi = my_hi; ch.first = first;
-            ch.keys.alloc(ctx, 2, true);
-            if (want_counts) ch.counts.alloc(ctx, 1, true);
+            set->open(my_lo, my_hi, 0);          // nothing arrived: the pass still has its (empty) chunk
+            set->close();
         }
-        first += ch.n;
-        out->chunks.push_back(std::move(ch));
-        if (sink) sink->push();
     }
 };
 
@@ -2405,16 +2349,18 @@ DistState *dist_begin(Ctx *ctx, int K, int B, int mode, int world, int rank, boo
         case 3: d = dist_state_new<3>(mode); break;
         default: d = dist_state_new<4>(mode); break;
     }
-    d->ctx = ctx; d->K = K; d->B = B; d->mode = mode; d->nw = nwords_of(K); d->result_on_host = result_on_host;
+    d->ctx = ctx; d->K = K; d->B = B; d->mode = mode; d->nw = nwords_of(K);
     d->G = ctx->num_sms * levelA_ctas_per_sm();
-    d->want_counts = (mode == kCanonical); d->double_selfrc = (mode == kCanonical) && (K % 2 == 0);
     // every rank must use the same geometry, so it depends on B only. As many level-A partitions as the shared-memory tables allow:
     // an owner's segment is the union of all ranks' records of a partition, so finer partitions keep refinement at one round
     int rA = 0;
     while (rA < 8 && ((uint64_t)B << (rA + 1)) <= (uint64_t)kLevelAMaxParts && rA + 1 <= 2 * K) ++rA;
     d->plan.world = world; d->plan.rank = rank; d->plan.B = B; d->plan.rA = rA; d->plan.PA_all = (uint32_t)B << rA;
     ctx->times.level_a_key_bits = (uint64_t)rA;
-    try { d->begin(); } catch (...) { delete d; throw; }
+    try {
+        d->set.reset(new KSetBuilder(ctx, K, d->nw, B, mode == kCanonical, mode == kCanonical && K % 2 == 0, result_on_host));
+        d->begin();
+    } catch (...) { delete d; throw; }
     return d;
 }
 uint32_t dist_num_partitions(const DistState *d) { return d->plan.PA_all; }
@@ -2423,16 +2369,8 @@ void dist_local_counts(DistState *d, uint64_t *h_out) { d->local_counts(h_out); 
 static const uint64_t kDistFixedBytes = (uint64_t)192 << 20;      // per-pass tables (segments, work lists, scans) next to the big buffers
 
 void dist_plan(DistState *d, const uint64_t *cnt_all, uint64_t *total_records) {
-    Ctx *ctx = d->ctx;
     dist_plan_tables(d->plan, d->plan.world, d->plan.rank, d->B, d->plan.rA, cnt_all);
     d->h_cnt_all.assign(cnt_all, cnt_all + (size_t)d->plan.world * d->plan.PA_all);
-    d->d_bsz.alloc(ctx, (size_t)d->B);
-    SG_CUDA(cudaMemsetAsync(d->d_bsz.p, 0, (size_t)d->B * 8, ctx->stream));
-    d->out = new KSet();
-    d->out->ctx = ctx; d->out->K = d->K; d->out->nw = d->nw; d->out->B = d->B; d->out->has_counts = d->want_counts;
-    d->out->on_host = d->result_on_host;
-    if (d->result_on_host) d->sink.reset(new ResultSink(ctx, d->out));
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));
     *total_records = d->plan.Tb[d->B];
 }
 
@@ -2452,7 +2390,7 @@ int dist_next_pass(DistState *d, uint64_t budget_bytes) {
     if (!dist_next_pass(d->plan, budget_bytes, W, kDistFixedBytes, &mx, &ms)) return -1;
     const int p = d->plan.npass() - 1;
     // buffers the peers read must live inside the arena (one driver allocation, mapped by the peers as a whole)
-    const uint32_t pa = (uint32_t)(d->plan.pass_b[p + 1] - d->plan.pass_b[p]) << d->plan.rA;
+    const uint32_t pa = (uint32_t)(d->plan.pass_lo(p + 1) - d->plan.pass_lo(p)) << d->plan.rA;
     d->sbuf.alloc(ctx, (size_t)((double)std::max(mx, ms) * kDistHeadroom) * d->nw + 16);
     d->xbuf.alloc(ctx, (size_t)((double)mx * kDistHeadroom) * d->nw + 16);
     d->pbase.alloc(ctx, (size_t)d->G * pa);
@@ -2531,18 +2469,9 @@ void dist_sort(DistState *d, int p) {
     SG_CUDA(cudaStreamSynchronize(d->ctx->stream));
 }
 KSet *dist_end(DistState *d) {
-    Ctx *ctx = d->ctx;
-    KSet *ks = d->out;
-    if (d->sink) { d->sink->drain(); d->sink.reset(); }
-    const int B = d->B;
-    std::vector<unsigned long long> hb(B);
-    SG_CUDA(cudaMemcpyAsync(hb.data(), d->d_bsz.p, (size_t)B * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    SG_CUDA(cudaStreamSynchronize(ctx->stream));
-    ks->bsz.assign(B, 0); ks->bstart.assign(B + 1, 0);
-    for (int b = 0; b < B; ++b) { ks->bsz[b] = (int64_t)hb[b]; ks->bstart[b + 1] = ks->bstart[b] + ks->bsz[b]; }
-    ks->n = d->first;
-    SG_CHECK(ks->bstart[B] == ks->n, 6, "internal: distributed bucket sizes do not add up");
-    d->out = nullptr;
+    SG_CHECK(d->set, 2, "sgpu_dist_end has already run");
+    KSet *ks = d->set->finish();
+    d->set.reset();
     return ks;
 }
 void dist_free(DistState *d) { delete d; }
@@ -2558,7 +2487,7 @@ int dist_plan_host(int world, int B, int rA, const uint64_t *cnt_all, uint64_t b
         worst = std::max(worst, mx);
         lim -= (double)mx * (record_bytes + 4) * 0.5;
     }
-    for (int p = 0; p <= pl.npass(); ++p) pass_b[p] = pl.pass_b[p];
+    for (int p = 0; p <= pl.npass(); ++p) pass_b[p] = pl.pass_lo(p);
     *max_recv = worst;
     return pl.npass();
 }

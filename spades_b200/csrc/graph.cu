@@ -738,11 +738,6 @@ static KeyParts collect_keys(Ctx *ctx, ChunkSource &src, Flags &&flags) {
     return kp;
 }
 
-// device bytes a step may still take: what the budget leaves (or 90 % of the arena's free space without one)
-static size_t graph_room(Ctx *ctx) {
-    return ctx->hbm_budget ? (ctx->hbm_budget > ctx->allocated ? ctx->hbm_budget - ctx->allocated : 0) : (size_t)((double)ctx->free_bytes() * 0.90);
-}
-
 template <int NW, int NWS>
 static void graph_build_nw(Ctx *ctx, Graph *g, const GraphOptions &opt) {
     const bool keep_loops = opt.keep_perfect_loops;
@@ -862,7 +857,7 @@ static void graph_build_nw(Ctx *ctx, Graph *g, const GraphOptions &opt) {
     DArr<uint8_t> visited(ctx, nk + 8);
     SG_CUDA(cudaMemsetAsync(visited.p, 0, visited.bytes(), st));
     const uint64_t per_junc = 2 * 8 * 37;
-    const uint64_t jbatch = std::max<uint64_t>(4096, graph_room(ctx) / 2 / per_junc);
+    const uint64_t jbatch = std::max<uint64_t>(4096, ctx->budget_left() / 2 / per_junc);
     g->edge_len.clear(); g->edge_off.clear(); g->seq.clear();
     g->link_start.clear(); g->link_end.clear(); g->raw_cov.clear();
     uint64_t batches = 0;

@@ -132,6 +132,10 @@ struct Ctx {
     void pool_release(void *p, size_t blk);
     void pool_trim();
     size_t free_bytes();                                     // allocatable bytes (arena free list)
+    // device bytes a pass or step may still plan with: what the HBM budget leaves, or 90 % of the arena's free bytes without one
+    size_t budget_left() {
+        return hbm_budget ? (hbm_budget > allocated ? hbm_budget - allocated : 0) : (size_t)((double)free_bytes() * 0.90);
+    }
 };
 
 inline void Ctx::arena_init() {

@@ -31,6 +31,19 @@ def test_exchange_plan_world2_gloo():
     assert all(out.get(r) for r in range(world)), dict(out)
 
 
+def test_plan_keeps_a_set_within_128_chunks():
+    """a budget that fits one bucket per pass: the distributed count still makes at most 128 passes (the chunks a set may hold),
+    each an even split of the buckets"""
+    import numpy as np
+    from spades_b200.distributed import plan_host
+    world, B, rA = 2, 300, 2
+    counts = np.random.default_rng(3).integers(1, 5000, size=(world, B << rA)).astype(np.uint64)
+    npass, bounds, _ = plan_host(world, B, rA, counts, 1, 16)
+    assert npass == 128
+    assert bounds[0] == 0 and bounds[-1] == B
+    assert set(np.diff(bounds).tolist()) == {2, 3}
+
+
 def _check_lines(lines, world):
     from dist_worker import CASES
     assert len(lines) == len(CASES), "%d result lines for %d cases" % (len(lines), len(CASES))
