@@ -294,6 +294,32 @@ void sgpu_dist_free(sgpu_dist *d);
 int sgpu_dist_plan_host(int world, int num_buckets, int key_bits_in_partition, const uint64_t *all_counts, uint64_t budget_bytes,
                         int record_bytes, int *pass_bounds, uint64_t *max_recv);
 
+/* ---- multi-GPU coverage pre-filter (one process per GPU). sgpu_reads_cov_filter over a read set sharded across ranks: the result
+ * is what one GPU computes over the union of the shards (concatenated in rank order): the same cardinality bound and key width on
+ * every rank, the same verdict for every read, the distinct keys summed over the ranks. The HLL registers of the union are the
+ * element-wise maximum of the ranks' registers; the counting table is split into one slice per rank, and a key lives in the slice of
+ * its owner (a hash of the key, independent of the slot inside the slice). Ranks insert into and look up in the owners' slices
+ * through cudaIpc mappings of the peers' memory arenas (the same mappings as sgpu_dist_*). The host language moves the two
+ * descriptors and provides the barriers:
+ *   begin -> ipc_handle -> [all_gather descriptors] -> open_peers -> bound -> ipc_handle -> [all_gather descriptors] -> open_peers ->
+ *   fill [barrier] filter [barrier] free
+ * begin: HLL registers of this rank's shard (K = k + 1). bound: the union's bound and key width, and this rank's empty slice.
+ * fill: every window of this rank's reads into its owner's slice, counts stopping at the threshold. filter: the verdicts of this
+ * rank's reads; keep_out, apply and stats as sgpu_reads_cov_filter, except stats[2] = distinct keys in THIS rank's slice (the
+ * union's number is the sum over the ranks) and stats[3] = reads kept on this rank. A slice that fills up fails the filter on
+ * every rank (SGPU error 6). */
+typedef struct sgpu_dist_cov sgpu_dist_cov;
+int sgpu_dist_cov_begin(sgpu_ctx *ctx, int K, unsigned threshold, int world, int rank, sgpu_dist_cov **out);
+int sgpu_dist_cov_ipc_handle(sgpu_dist_cov *d, uint8_t *out /* SGPU_IPC_BYTES */);
+int sgpu_dist_cov_open_peers(sgpu_dist_cov *d, const uint8_t *descriptors /* world x SGPU_IPC_BYTES, rank-major */);
+int sgpu_dist_cov_bound(sgpu_dist_cov *d);
+int sgpu_dist_cov_fill(sgpu_dist_cov *d);
+int sgpu_dist_cov_filter(sgpu_dist_cov *d, int apply, uint8_t *keep_out, uint64_t *stats);
+void sgpu_dist_cov_free(sgpu_dist_cov *d);
+/* the layout alone (pure host arithmetic, no GPU): the owner rank of each masked key, and the capacity of a rank's slice (entries)
+ * for a cardinality bound */
+int sgpu_dist_cov_layout_host(int world, uint64_t cardinality_bound, const uint64_t *keys, int64_t n, uint32_t *owners, uint64_t *slice_capacity);
+
 /* self tests of the shared host/device arithmetic (tests only): op 0 = xxh3_64, 1 = xxh3_128 lo, 2 = xxh3_128 hi, 3 = bucket(arg),
  * 4 = is_minimal, 5.. = rc word j. keys: n records of ceil(K/32) words. on_device != 0 runs the same code in a kernel. */
 int sgpu_selftest(sgpu_ctx *ctx, int on_device, int op, int K, uint64_t arg, const uint64_t *keys, int64_t n, uint64_t *out);

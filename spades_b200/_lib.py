@@ -26,6 +26,8 @@ SYMBOLS = [
     "sgpu_edge_index_values", "sgpu_edge_index_lookup", "sgpu_edge_index_free",
     "sgpu_dist_begin", "sgpu_dist_num_partitions", "sgpu_dist_local_counts", "sgpu_dist_plan", "sgpu_dist_free_bytes", "sgpu_dist_next_pass", "sgpu_dist_ipc_handle",
     "sgpu_dist_open_peers", "sgpu_dist_scatter", "sgpu_dist_exchange", "sgpu_dist_sort", "sgpu_dist_end", "sgpu_dist_free", "sgpu_dist_plan_host",
+    "sgpu_dist_cov_begin", "sgpu_dist_cov_ipc_handle", "sgpu_dist_cov_open_peers", "sgpu_dist_cov_bound", "sgpu_dist_cov_fill", "sgpu_dist_cov_filter",
+    "sgpu_dist_cov_free", "sgpu_dist_cov_layout_host",
     "sgpu_selftest",
 ]
 
@@ -145,6 +147,14 @@ def load():
     L.sgpu_dist_end.restype = i32; L.sgpu_dist_end.argtypes = [vp, pp]
     L.sgpu_dist_free.restype = None; L.sgpu_dist_free.argtypes = [vp]
     L.sgpu_dist_plan_host.restype = i32; L.sgpu_dist_plan_host.argtypes = [i32, i32, i32, vp, u64, i32, vp, C.POINTER(u64)]
+    L.sgpu_dist_cov_begin.restype = i32; L.sgpu_dist_cov_begin.argtypes = [vp, i32, C.c_uint, i32, i32, pp]
+    L.sgpu_dist_cov_ipc_handle.restype = i32; L.sgpu_dist_cov_ipc_handle.argtypes = [vp, vp]
+    L.sgpu_dist_cov_open_peers.restype = i32; L.sgpu_dist_cov_open_peers.argtypes = [vp, vp]
+    L.sgpu_dist_cov_bound.restype = i32; L.sgpu_dist_cov_bound.argtypes = [vp]
+    L.sgpu_dist_cov_fill.restype = i32; L.sgpu_dist_cov_fill.argtypes = [vp]
+    L.sgpu_dist_cov_filter.restype = i32; L.sgpu_dist_cov_filter.argtypes = [vp, i32, vp, vp]
+    L.sgpu_dist_cov_free.restype = None; L.sgpu_dist_cov_free.argtypes = [vp]
+    L.sgpu_dist_cov_layout_host.restype = i32; L.sgpu_dist_cov_layout_host.argtypes = [i32, u64, vp, i64, vp, C.POINTER(u64)]
     L.sgpu_selftest.restype = i32; L.sgpu_selftest.argtypes = [vp, i32, i32, i32, u64, vp, i64, vp]
     _lib = L
     return L

@@ -602,6 +602,55 @@ int sgpu_dist_plan_host(int world, int num_buckets, int key_bits_in_partition, c
 }
 }  // extern "C"
 
+struct sgpu_dist_cov { CovDist *d; Ctx *c; };
+extern "C" {
+int sgpu_dist_cov_begin(sgpu_ctx *ctx, int K, unsigned threshold, int world, int rank, sgpu_dist_cov **out) {
+    if (!ctx || !out) return SGPU_EINVAL;
+    *out = nullptr;
+    Ctx *c = &ctx->c;
+    API_TRY(c, {
+        SG_CUDA(cudaSetDevice(c->device));
+        CovDist *d = dist_cov_begin(c, K, threshold, world, rank);
+        *out = new sgpu_dist_cov{d, c};
+        child_add(c);
+    })
+}
+int sgpu_dist_cov_ipc_handle(sgpu_dist_cov *d, uint8_t *out) {
+    if (!d || !out) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dist_cov_ipc_handle(d->d, out); })
+}
+int sgpu_dist_cov_open_peers(sgpu_dist_cov *d, const uint8_t *descriptors) {
+    if (!d || !descriptors) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dist_cov_open_peers(d->d, descriptors); })
+}
+int sgpu_dist_cov_bound(sgpu_dist_cov *d) {
+    if (!d) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dist_cov_bound(d->d); })
+}
+int sgpu_dist_cov_fill(sgpu_dist_cov *d) {
+    if (!d) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dist_cov_fill(d->d); })
+}
+int sgpu_dist_cov_filter(sgpu_dist_cov *d, int apply, uint8_t *keep_out, uint64_t *stats) {
+    if (!d) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dist_cov_filter(d->d, apply, keep_out, stats); })
+}
+void sgpu_dist_cov_free(sgpu_dist_cov *d) {
+    if (!d) return;
+    Ctx *c = d->c;
+    cudaSetDevice(c->device);
+    dist_cov_free(d->d);
+    delete d;
+    child_release(c);
+}
+int sgpu_dist_cov_layout_host(int world, uint64_t cardinality_bound, const uint64_t *keys, int64_t n, uint32_t *owners, uint64_t *slice_capacity) {
+    if (world < 1 || n < 0 || (n && (!keys || !owners)) || !slice_capacity) return SGPU_EINVAL;
+    for (int64_t i = 0; i < n; ++i) owners[i] = cov_owner_host(keys[i], world);
+    *slice_capacity = cov_slice_capacity(cardinality_bound, world);
+    return SGPU_OK;
+}
+}  // extern "C"
+
 // ---- self test of kmer_dev.cuh on host and device -----------------------------------------------------------------------
 template <int NW>
 __host__ __device__ uint64_t selftest_one(int op, int K, uint64_t arg, const uint64_t *key) {

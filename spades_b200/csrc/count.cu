@@ -2407,16 +2407,11 @@ static_assert(sizeof(cudaIpcMemHandle_t) == 64 && sizeof(DistDesc) == 96, "descr
 
 void dist_ipc_handle(DistState *d, uint8_t *out96) {
     Ctx *ctx = d->ctx;
-    auto off_of = [&](const void *p, const char *what) {
-        const char *c = (const char *)p;
-        SG_CHECK(ctx->arena && c >= ctx->arena && c < ctx->arena + ctx->arena_size, 4, what);
-        return (uint64_t)(c - ctx->arena);
-    };
     DistDesc ds;
     memset(&ds, 0, sizeof ds);
-    ds.off_sbuf = off_of(d->sbuf.p, "distributed count: the staging buffer did not fit the device memory arena");
-    ds.off_pbase = off_of(d->pbase.p, "distributed count: the piece table did not fit the device memory arena");
-    ds.off_blk = off_of(d->blk_counts_ptr(), "distributed count: the level-A count table did not fit the device memory arena");
+    ds.off_sbuf = ctx->arena_offset(d->sbuf.p, "distributed count: the staging buffer did not fit the device memory arena");
+    ds.off_pbase = ctx->arena_offset(d->pbase.p, "distributed count: the piece table did not fit the device memory arena");
+    ds.off_blk = ctx->arena_offset(d->blk_counts_ptr(), "distributed count: the level-A count table did not fit the device memory arena");
     ds.arena_size = ctx->arena_size;
     if (d->plan.world > 1) SG_CUDA(cudaIpcGetMemHandle(&ds.arena, ctx->arena));
     memcpy(out96, &ds, sizeof ds);
@@ -2426,27 +2421,10 @@ void dist_open_peers(DistState *d, const uint8_t *descs) {
     Ctx *ctx = d->ctx;
     const int world = d->plan.world;
     d->peers.assign(world, PullSrc{nullptr, nullptr, nullptr});
-    if ((int)ctx->peer_arena.size() != world) { ctx->peer_close(); ctx->peer_arena.assign(world, nullptr); ctx->peer_handle.assign((size_t)world * 64, 0); }
     for (int g = 0; g < world; ++g) {
         DistDesc ds;
         memcpy(&ds, descs + (size_t)g * sizeof(DistDesc), sizeof ds);
-        char *base = nullptr;
-        if (g == d->plan.rank) {
-            base = ctx->arena;
-        } else {
-            // a peer's arena is mapped once per process; a different handle under the same rank (its context was re-created) remaps
-            if (ctx->peer_arena[g] && memcmp(&ctx->peer_handle[(size_t)g * 64], &ds.arena, 64) != 0) {
-                cudaIpcCloseMemHandle(ctx->peer_arena[g]);
-                ctx->peer_arena[g] = nullptr;
-            }
-            if (!ctx->peer_arena[g]) {
-                void *p = nullptr;
-                SG_CUDA(cudaIpcOpenMemHandle(&p, ds.arena, cudaIpcMemLazyEnablePeerAccess));
-                ctx->peer_arena[g] = (char *)p;
-                memcpy(&ctx->peer_handle[(size_t)g * 64], &ds.arena, 64);
-            }
-            base = ctx->peer_arena[g];
-        }
+        char *base = ctx->peer_map(world, d->plan.rank, g, &ds.arena);
         SG_CHECK(ds.off_sbuf < ds.arena_size && ds.off_pbase < ds.arena_size && ds.off_blk < ds.arena_size, 2, "bad peer descriptor");
         d->peers[g] = PullSrc{(const uint64_t *)(base + ds.off_sbuf), (const uint64_t *)(base + ds.off_pbase), (const uint32_t *)(base + ds.off_blk)};
     }

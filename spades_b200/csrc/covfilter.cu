@@ -22,6 +22,7 @@
 // the hash instead of materialising 8 bytes per window.
 #include "sgpu_internal.h"
 #include <cmath>
+#include <memory>
 
 namespace sg {
 
@@ -190,6 +191,99 @@ __global__ void cov_distinct_k(const unsigned long long *__restrict__ e, uint64_
     if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, (unsigned long long)c);
 }
 
+// ---- the distributed filter: the table is split into one slice per rank, a key lives in its owner's slice ----------------------------
+// The owner is the high word of a second multiplicative hash of the masked key scaled by the world size, so it does not depend on
+// the slot function inside a slice (which takes the high word of key * 0x9E37...).
+__host__ __device__ __forceinline__ uint32_t cov_owner(uint64_t key, uint32_t world) {
+    const uint64_t h = key * 0xC2B2AE3D27D4EB4FULL;
+#ifdef __CUDA_ARCH__
+    return (uint32_t)__umul64hi(h, world);
+#else
+    return (uint32_t)(((unsigned __int128)h * world) >> 64);
+#endif
+}
+
+// HLL registers of the union = element-wise max of the ranks' registers (read through the peers' mapped arenas)
+__global__ void cov_hll_merge_k(const uint4 *const *__restrict__ regs, int world, uint4 *__restrict__ out, uint32_t n4) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n4) return;
+    uint4 m = regs[0][i];
+    for (int g = 1; g < world; ++g) {
+        const uint4 r = regs[g][i];
+        m.x = max(m.x, r.x); m.y = max(m.y, r.y); m.z = max(m.z, r.z); m.w = max(m.w, r.w);
+    }
+    out[i] = m;
+}
+
+// CovTable::add with system-scope CAS: ranks on other GPUs insert into the same slice at the same time
+__device__ __forceinline__ void cov_add_system(const CovTable &t, uint64_t key, unsigned thr) {
+    const unsigned long long tag = (key + 1) << 16;
+    uint64_t s = t.slot_of(key);
+    for (uint64_t probes = 0;; ++probes) {
+        if (probes > t.cap) { atomicExch_system(t.overflow, 1u); return; }
+        unsigned long long cur = t.e[s];
+        if (cur == 0) {
+            const unsigned long long old = atomicCAS_system(&t.e[s], 0ull, tag | 1ull);
+            if (old == 0) return;
+            cur = old;
+        }
+        if ((cur & ~0xffffull) == tag) {
+            while ((cur & 0xffffull) < thr) {
+                const unsigned long long old = atomicCAS_system(&t.e[s], cur, cur + 1);
+                if (old == cur) return;
+                cur = old;
+            }
+            return;
+        }
+        if (++s == t.cap) s = 0;
+    }
+}
+
+// pass 2 over this rank's reads: every window's key goes to its owner's slice
+__global__ void cov_fill_dist_k(const uint64_t *__restrict__ words, const uint64_t *__restrict__ offs, const uint32_t *__restrict__ lens, int64_t n,
+                                int K, const CovTable *__restrict__ slices, uint32_t world, uint64_t key_mask, unsigned thr) {
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const int L = (int)lens[r];
+    if (L < K) return;
+    const uint64_t *seq = words + offs[r];
+    CycHash h = cyc_init(seq, K);
+    for (int j = 0;; ++j) {
+        const uint64_t key = h.value() & key_mask;
+        const CovTable &t = slices[cov_owner(key, world)];
+        cov_add_system(t, key, thr);
+        if ((K & 1) == 0 && h.fwd == h.rvs && window_self_rc(seq, j, K)) cov_add_system(t, key, thr);
+        if (j + K >= L) break;
+        cyc_roll(h, base_at(seq, j), base_at(seq, j + K), K);
+    }
+}
+
+// pass 3 over this rank's reads: the same verdict as cov_filter_k, each window's count read from its owner's slice
+__global__ void cov_filter_dist_k(const uint64_t *__restrict__ words, const uint64_t *__restrict__ offs, const uint32_t *__restrict__ lens, int64_t n,
+                                  int K, const CovTable *__restrict__ slices, uint32_t world, uint64_t key_mask, unsigned thr,
+                                  uint8_t *__restrict__ keep, uint32_t *__restrict__ keep_words) {
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const int L = (int)lens[r];
+    bool k = false;
+    if (L < K) {
+        k = thr == 0;
+    } else {
+        const uint64_t *seq = words + offs[r];
+        CycHash h = cyc_init(seq, K);
+        uint32_t below = 0;
+        for (int j = 0;; ++j) {
+            const uint64_t key = h.value() & key_mask;
+            below += slices[cov_owner(key, world)].count(key) < thr;
+            if (j + K >= L) break;
+            cyc_roll(h, base_at(seq, j), base_at(seq, j + K), K);
+        }
+        k = below <= (uint32_t)(L - K + 1) / 2;
+    }
+    keep[r] = k ? 1 : 0;
+    keep_words[r] = k ? (uint32_t)((L + 31) >> 5) : 0u;
+}
+
 }  // namespace
 
 // hll<24>::cardinality / upper_bound_cardinality (adt/hll.hpp:50-68): same operations in the same order
@@ -204,6 +298,53 @@ static double hll_upper_bound(const std::vector<uint32_t> &reg) {
     if (res <= 5.0 * (double)m / 2 && zeros > 0) res = (double)m * (std::log((double)m) - std::log((double)zeros));
     return 1.1 * res;
 }
+
+// qf::cqf(maxn) geometry (cqf.hpp:28-37): key bits of the filter for a cardinality bound
+static unsigned cov_key_bits(size_t maxn) {
+    const unsigned lg = maxn > 1 ? (unsigned)std::ceil(std::log2((double)maxn)) : 0u;     // (no reads: the reference's log2(0) is undefined)
+    const unsigned qbits = std::max(7u, lg) + 1;
+    const unsigned key_bits = qbits + 8;
+    SG_CHECK(key_bits <= 47, 2, "coverage filter: more than 2^38 distinct k-mers estimated");
+    return key_bits;
+}
+
+// What follows the verdict kernel, in both entry points: where each survivor and its words go (order kept), the number kept,
+// the flags for the caller and, with apply, the survivors as the context's read set (what CovFilteringWrap does to the streams).
+struct CovVerdicts {
+    Ctx *ctx;
+    int64_t n;
+    DArr<uint8_t> keep;
+    DArr<uint32_t> keep_words, flag;
+    DArr<uint64_t> new_off, new_idx;
+    uint64_t kept = 0, kept_words = 0;
+    explicit CovVerdicts(Ctx *c) : ctx(c), n(c->n_reads), keep(c, (size_t)c->n_reads + 1), keep_words(c, (size_t)c->n_reads + 1), flag(c, (size_t)c->n_reads + 1) {}
+    // after the verdict kernel: enqueues the scans and the copies of the totals and of keep_out (the caller synchronises)
+    void scan(uint8_t *keep_out) {
+        cudaStream_t st = ctx->stream;
+        if (n) { cov_keep_count_k<<<div_up(n, 256), 256, 0, st>>>(keep.p, n, flag.p); ctx->launches++; }
+        SG_CUDA(cudaMemsetAsync(keep_words.p + n, 0, 4, st));
+        SG_CUDA(cudaMemsetAsync(flag.p + n, 0, 4, st));
+        new_off.alloc(ctx, (size_t)n + 1); new_idx.alloc(ctx, (size_t)n + 1);
+        exclusive_scan_u32_to_u64(ctx, keep_words.p, new_off.p, (size_t)n + 1);
+        exclusive_scan_u32_to_u64(ctx, flag.p, new_idx.p, (size_t)n + 1);
+        SG_CUDA(cudaMemcpyAsync(&kept, new_idx.p + n, 8, cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaMemcpyAsync(&kept_words, new_off.p + n, 8, cudaMemcpyDeviceToHost, st));
+        if (keep_out && n) SG_CUDA(cudaMemcpyAsync(keep_out, keep.p, (size_t)n, cudaMemcpyDeviceToHost, st));
+    }
+    void apply() {
+        cudaStream_t st = ctx->stream;
+        DArr<uint64_t> nw(ctx, kept_words + 4, true), no(ctx, kept + 1, true);
+        DArr<uint32_t> nl(ctx, kept + 1, true);
+        SG_CUDA(cudaMemsetAsync(nw.p + kept_words, 0, 4 * 8, st));
+        if (n) { cov_compact_k<<<div_up(n, 128), 128, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, keep.p, new_idx.p, new_off.p, n, nw.p, no.p, nl.p); ctx->launches++; }
+        SG_CUDA(cudaGetLastError());
+        SG_CUDA(cudaStreamSynchronize(st));
+        ctx->h_words.clear(); ctx->h_offs.clear(); ctx->h_lens.clear(); ctx->staged_dirty = false;
+        ctx->r_words = std::move(nw); ctx->r_offs = std::move(no); ctx->r_lens = std::move(nl);
+        ctx->d_words = ctx->r_words.p; ctx->d_offs = ctx->r_offs.p; ctx->d_lens = ctx->r_lens.p;
+        ctx->n_reads = (int64_t)kept; ctx->n_words = kept_words;
+    }
+};
 
 void cov_filter(Ctx *ctx, int K, unsigned thr, int apply, uint8_t *keep_out, uint64_t *stats) {
     SG_CHECK(K >= 1 && K <= 128, 2, "K must be in [1,128]");
@@ -222,19 +363,15 @@ void cov_filter(Ctx *ctx, int K, unsigned thr, int apply, uint8_t *keep_out, uin
         SG_CUDA(cudaStreamSynchronize(st));
     }
     const size_t maxn = (size_t)hll_upper_bound(h_reg);
-    // 2. qf::cqf(maxn) geometry (cqf.hpp:28-37)
-    const unsigned lg = maxn > 1 ? (unsigned)std::ceil(std::log2((double)maxn)) : 0u;     // (no reads: the reference's log2(0) is undefined)
-    const unsigned qbits = std::max(7u, lg) + 1;
-    const unsigned key_bits = qbits + 8;
-    SG_CHECK(key_bits <= 47, 2, "coverage filter: more than 2^38 distinct k-mers estimated");
+    // 2. the table
+    const unsigned key_bits = cov_key_bits(maxn);
     CovTable t;
     t.cap = std::max<uint64_t>(1024, (uint64_t)maxn + (uint64_t)maxn / 2);
     t.key_mask = (1ull << key_bits) - 1;
     DArr<unsigned long long> table(ctx, t.cap);
     t.e = table.p;
     SG_CUDA(cudaMemsetAsync(table.p, 0, table.bytes(), st));
-    DArr<uint8_t> keep(ctx, (size_t)n + 1);
-    DArr<uint32_t> keep_words(ctx, (size_t)n + 1), flag(ctx, (size_t)n + 1);
+    CovVerdicts v(ctx);
     DArr<unsigned long long> d_cnt(ctx, 1);
     DArr<unsigned> d_ovf(ctx, 1);
     SG_CUDA(cudaMemsetAsync(d_cnt.p, 0, 8, st));
@@ -242,41 +379,180 @@ void cov_filter(Ctx *ctx, int K, unsigned thr, int apply, uint8_t *keep_out, uin
     t.overflow = d_ovf.p;
     if (n) {
         cov_fill_k<<<div_up(n, T), T, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, t, thr);
-        cov_filter_k<<<div_up(n, T), T, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, t, thr, keep.p, keep_words.p);
-        cov_keep_count_k<<<div_up(n, 256), 256, 0, st>>>(keep.p, n, flag.p);
-        ctx->launches += 3;
+        cov_filter_k<<<div_up(n, T), T, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, t, thr, v.keep.p, v.keep_words.p);
+        ctx->launches += 2;
     }
     cov_distinct_k<<<ctx->num_sms * 4, 256, 0, st>>>(table.p, t.cap, d_cnt.p);
     ctx->launches++;
-    SG_CUDA(cudaMemsetAsync(keep_words.p + n, 0, 4, st));
-    SG_CUDA(cudaMemsetAsync(flag.p + n, 0, 4, st));
-    DArr<uint64_t> new_off(ctx, (size_t)n + 1), new_idx(ctx, (size_t)n + 1);
-    exclusive_scan_u32_to_u64(ctx, keep_words.p, new_off.p, (size_t)n + 1);
-    exclusive_scan_u32_to_u64(ctx, flag.p, new_idx.p, (size_t)n + 1);
-    uint64_t kept = 0, kept_words = 0;
+    v.scan(keep_out);
     unsigned long long distinct = 0;
-    SG_CUDA(cudaMemcpyAsync(&kept, new_idx.p + n, 8, cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaMemcpyAsync(&kept_words, new_off.p + n, 8, cudaMemcpyDeviceToHost, st));
     SG_CUDA(cudaMemcpyAsync(&distinct, d_cnt.p, 8, cudaMemcpyDeviceToHost, st));
     unsigned overflow = 0;
     SG_CUDA(cudaMemcpyAsync(&overflow, d_ovf.p, 4, cudaMemcpyDeviceToHost, st));
-    if (keep_out && n) SG_CUDA(cudaMemcpyAsync(keep_out, keep.p, (size_t)n, cudaMemcpyDeviceToHost, st));
     SG_CUDA(cudaGetLastError());
     SG_CUDA(cudaStreamSynchronize(st));
     SG_CHECK(!overflow, 6, "coverage filter: more distinct keys than the cardinality bound allows (table full)");
-    if (stats) { stats[0] = maxn; stats[1] = key_bits; stats[2] = distinct; stats[3] = kept; }
-    if (!apply) return;
-    // 3. the surviving reads become the context's read set (what CovFilteringWrap does to the streams)
-    DArr<uint64_t> nw(ctx, kept_words + 4, true), no(ctx, kept + 1, true);
-    DArr<uint32_t> nl(ctx, kept + 1, true);
-    SG_CUDA(cudaMemsetAsync(nw.p + kept_words, 0, 4 * 8, st));
-    if (n) { cov_compact_k<<<div_up(n, 128), 128, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, keep.p, new_idx.p, new_off.p, n, nw.p, no.p, nl.p); ctx->launches++; }
-    SG_CUDA(cudaGetLastError());
-    SG_CUDA(cudaStreamSynchronize(st));
-    ctx->h_words.clear(); ctx->h_offs.clear(); ctx->h_lens.clear(); ctx->staged_dirty = false;
-    ctx->r_words = std::move(nw); ctx->r_offs = std::move(no); ctx->r_lens = std::move(nl);
-    ctx->d_words = ctx->r_words.p; ctx->d_offs = ctx->r_offs.p; ctx->d_lens = ctx->r_lens.p;
-    ctx->n_reads = (int64_t)kept; ctx->n_words = kept_words;
+    if (stats) { stats[0] = maxn; stats[1] = key_bits; stats[2] = distinct; stats[3] = v.kept; }
+    if (apply) v.apply();
 }
+
+// ---- distributed filter (sgpu_dist_cov_*): every rank holds a shard of the reads; the result equals cov_filter over the union --------
+// Slice capacity: 1.5 x an even share of the bound, like the single-GPU table, plus 8 standard deviations of a binomial owner load
+// (at most sqrt(share)) for the unevenness of the owner hash. A slice overflows only when its distinct keys exceed the capacity.
+uint64_t cov_slice_capacity(uint64_t maxn, int world) {
+    const uint64_t share = (maxn + (uint64_t)world - 1) / (uint64_t)world;
+    return std::max<uint64_t>(1024, share + share / 2 + 8 * (uint64_t)std::ceil(std::sqrt((double)share)));
+}
+uint32_t cov_owner_host(uint64_t key, int world) { return cov_owner(key, (uint32_t)world); }
+
+struct CovDist {
+    Ctx *ctx = nullptr;
+    int K = 0, world = 1, rank = 0;
+    unsigned thr = 0;
+    DArr<uint32_t> reg;                      // this rank's HLL registers (peers read them in bound)
+    DArr<unsigned long long> slice;          // this rank's slice: cap entries, then the overflow flag (peers write both in fill)
+    uint64_t maxn = 0, cap = 0;
+    unsigned key_bits = 0;
+    std::vector<const uint32_t *> peer_reg;  // rank-indexed, as this process sees them
+    std::vector<CovTable> peer_slice;
+    bool filled = false;
+};
+
+// descriptor a rank publishes (all_gather) after begin and again after bound: arena handle + where its registers and slice are
+struct CovDesc {
+    cudaIpcMemHandle_t arena;
+    uint64_t arena_size, off_reg, off_slice, slice_cap;     // slice_cap = 0: no slice yet
+};
+static_assert(sizeof(CovDesc) == 96, "descriptor layout (SGPU_IPC_BYTES)");
+
+CovDist *dist_cov_begin(Ctx *ctx, int K, unsigned thr, int world, int rank) {
+    SG_CHECK(K >= 1 && K <= 128, 2, "K must be in [1,128]");
+    SG_CHECK(thr <= 60000u, 2, "coverage threshold must be at most 60000");
+    SG_CHECK(world >= 1 && rank >= 0 && rank < world, 2, "bad world / rank");
+    ensure_reads_on_device(ctx);
+    std::unique_ptr<CovDist> d(new CovDist);
+    d->ctx = ctx; d->K = K; d->thr = thr; d->world = world; d->rank = rank;
+    cudaStream_t st = ctx->stream;
+    const int64_t n = ctx->n_reads;
+    d->reg.alloc(ctx, (size_t)1 << 24);
+    SG_CUDA(cudaMemsetAsync(d->reg.p, 0, d->reg.bytes(), st));
+    if (n) { cov_hll_k<<<div_up(n, 128), 128, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, d->reg.p); ctx->launches++; }
+    SG_CUDA(cudaGetLastError());
+    SG_CUDA(cudaStreamSynchronize(st));                 // the registers are complete before they are published
+    return d.release();
+}
+
+void dist_cov_ipc_handle(CovDist *d, uint8_t *out96) {
+    Ctx *ctx = d->ctx;
+    CovDesc ds;
+    memset(&ds, 0, sizeof ds);
+    ds.arena_size = ctx->arena_size;
+    if (d->reg.p) ds.off_reg = ctx->arena_offset(d->reg.p, "distributed coverage filter: the HLL registers did not fit the device memory arena");
+    if (d->slice.p) {
+        ds.off_slice = ctx->arena_offset(d->slice.p, "distributed coverage filter: the table slice did not fit the device memory arena");
+        ds.slice_cap = d->cap;
+    }
+    if (d->world > 1) SG_CUDA(cudaIpcGetMemHandle(&ds.arena, ctx->arena));
+    memcpy(out96, &ds, sizeof ds);
+}
+
+void dist_cov_open_peers(CovDist *d, const uint8_t *descs) {
+    Ctx *ctx = d->ctx;
+    d->peer_reg.assign(d->world, nullptr);
+    d->peer_slice.assign(d->world, CovTable{});
+    for (int g = 0; g < d->world; ++g) {
+        CovDesc ds;
+        memcpy(&ds, descs + (size_t)g * sizeof(CovDesc), sizeof ds);
+        char *base = ctx->peer_map(d->world, d->rank, g, &ds.arena);
+        SG_CHECK(ds.off_reg + ((uint64_t)4 << 24) <= ds.arena_size && ds.off_slice + (ds.slice_cap + 1) * 8 <= ds.arena_size, 2, "bad peer descriptor");
+        d->peer_reg[g] = (const uint32_t *)(base + ds.off_reg);
+        if (ds.slice_cap) {
+            CovTable &t = d->peer_slice[g];
+            t.e = (unsigned long long *)(base + ds.off_slice);
+            t.cap = ds.slice_cap;
+            t.key_mask = (1ull << d->key_bits) - 1;
+            t.overflow = (unsigned *)(t.e + t.cap);
+        }
+    }
+}
+
+void dist_cov_bound(CovDist *d) {
+    Ctx *ctx = d->ctx;
+    SG_CHECK(d->reg.p && (int)d->peer_reg.size() == d->world && !d->slice.p, 2,
+             "sgpu_dist_cov_bound runs once, after sgpu_dist_cov_open_peers with the descriptors of sgpu_dist_cov_begin");
+    cudaStream_t st = ctx->stream;
+    std::vector<uint32_t> h_reg((size_t)1 << 24);
+    {
+        DArr<uint32_t> merged(ctx, (size_t)1 << 24);
+        DArr<uint64_t> regs(ctx, (size_t)d->world);
+        SG_CUDA(cudaMemcpyAsync(regs.p, d->peer_reg.data(), (size_t)d->world * 8, cudaMemcpyHostToDevice, st));
+        const uint32_t n4 = (1u << 24) / 4;
+        cov_hll_merge_k<<<div_up(n4, 256), 256, 0, st>>>((const uint4 *const *)regs.p, d->world, (uint4 *)merged.p, n4);
+        ctx->launches++;
+        SG_CUDA(cudaMemcpyAsync(h_reg.data(), merged.p, merged.bytes(), cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaGetLastError());
+        SG_CUDA(cudaStreamSynchronize(st));
+    }
+    d->maxn = (uint64_t)(size_t)hll_upper_bound(h_reg);
+    d->key_bits = cov_key_bits((size_t)d->maxn);
+    d->cap = cov_slice_capacity(d->maxn, d->world);
+    d->slice.alloc(ctx, d->cap + 1);
+    SG_CUDA(cudaMemsetAsync(d->slice.p, 0, d->slice.bytes(), st));
+    SG_CUDA(cudaStreamSynchronize(st));                 // the slice is empty before it is published
+}
+
+void dist_cov_fill(CovDist *d) {
+    Ctx *ctx = d->ctx;
+    SG_CHECK(d->slice.p && (int)d->peer_slice.size() == d->world && d->peer_slice[d->rank].e == d->slice.p && !d->filled, 2,
+             "sgpu_dist_cov_fill runs once, after sgpu_dist_cov_open_peers with the descriptors of sgpu_dist_cov_bound");
+    for (const CovTable &t : d->peer_slice) SG_CHECK(t.e, 2, "a peer descriptor carries no table slice");
+    d->reg.release();                                   // every rank has finished its bound before it published its slice
+    cudaStream_t st = ctx->stream;
+    const int64_t n = ctx->n_reads;
+    DArr<CovTable> slices(ctx, (size_t)d->world);
+    SG_CUDA(cudaMemcpyAsync(slices.p, d->peer_slice.data(), (size_t)d->world * sizeof(CovTable), cudaMemcpyHostToDevice, st));
+    if (n) {
+        cov_fill_dist_k<<<div_up(n, 128), 128, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, d->K, slices.p, (uint32_t)d->world,
+                                                        (1ull << d->key_bits) - 1, d->thr);
+        ctx->launches++;
+    }
+    SG_CUDA(cudaGetLastError());
+    SG_CUDA(cudaStreamSynchronize(st));                 // this rank inserts nothing more; peers may read after the next barrier
+    d->filled = true;
+}
+
+void dist_cov_filter(CovDist *d, int apply, uint8_t *keep_out, uint64_t *stats) {
+    Ctx *ctx = d->ctx;
+    SG_CHECK(d->filled, 2, "sgpu_dist_cov_filter runs after sgpu_dist_cov_fill and a barrier");
+    cudaStream_t st = ctx->stream;
+    // every rank checks every slice's overflow flag, so all of them fail together
+    for (const CovTable &t : d->peer_slice) {
+        unsigned overflow = 0;
+        SG_CUDA(cudaMemcpy(&overflow, t.overflow, 4, cudaMemcpyDefault));
+        SG_CHECK(!overflow, 6, "distributed coverage filter: more distinct keys in a slice than its capacity (table full)");
+    }
+    const int64_t n = ctx->n_reads;
+    DArr<CovTable> slices(ctx, (size_t)d->world);
+    SG_CUDA(cudaMemcpyAsync(slices.p, d->peer_slice.data(), (size_t)d->world * sizeof(CovTable), cudaMemcpyHostToDevice, st));
+    CovVerdicts v(ctx);
+    DArr<unsigned long long> d_cnt(ctx, 1);
+    SG_CUDA(cudaMemsetAsync(d_cnt.p, 0, 8, st));
+    if (n) {
+        cov_filter_dist_k<<<div_up(n, 128), 128, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, d->K, slices.p, (uint32_t)d->world,
+                                                          (1ull << d->key_bits) - 1, d->thr, v.keep.p, v.keep_words.p);
+        ctx->launches++;
+    }
+    cov_distinct_k<<<ctx->num_sms * 4, 256, 0, st>>>(d->slice.p, d->cap, d_cnt.p);
+    ctx->launches++;
+    v.scan(keep_out);
+    unsigned long long distinct = 0;
+    SG_CUDA(cudaMemcpyAsync(&distinct, d_cnt.p, 8, cudaMemcpyDeviceToHost, st));
+    SG_CUDA(cudaGetLastError());
+    SG_CUDA(cudaStreamSynchronize(st));                 // this rank reads no slice any more
+    if (stats) { stats[0] = d->maxn; stats[1] = d->key_bits; stats[2] = distinct; stats[3] = v.kept; }
+    if (apply) v.apply();
+}
+
+void dist_cov_free(CovDist *d) { delete d; }
 
 }  // namespace sg

@@ -118,6 +118,10 @@ struct Ctx {
     std::vector<char *> peer_arena;
     std::vector<uint8_t> peer_handle;        // 64 bytes per rank: the handle a mapping was opened from
     void peer_close();
+    // the arena of rank g (of `world`) as this process sees it: its own arena, or the peer's opened from `handle` (64 bytes)
+    char *peer_map(int world, int rank, int g, const void *handle);
+    // offset of a block inside the arena (what a peer adds to its mapping); `what` is the error when the block lies outside it
+    uint64_t arena_offset(const void *p, const char *what) const;
     // device memory: one arena reserved from the driver at first use and sub-allocated with a coalescing free list.
     // cudaMalloc/cudaFree of tens of GB cost 100s of ms and a 100 M-read step turns over ~300 GB of buffers; inside the
     // arena an allocation is a map lookup. Short-lived buffers (X/Y ping-pong, scratch) grow from the bottom, long-lived
@@ -160,6 +164,29 @@ inline void Ctx::arena_init() {
 inline void Ctx::peer_close() {
     for (char *p : peer_arena) if (p) cudaIpcCloseMemHandle(p);
     peer_arena.clear(); peer_handle.clear();
+}
+inline char *Ctx::peer_map(int world, int rank, int g, const void *handle) {
+    if (g == rank) return arena;
+    if ((int)peer_arena.size() != world) { peer_close(); peer_arena.assign(world, nullptr); peer_handle.assign((size_t)world * 64, 0); }
+    // a peer's arena is mapped once per process; a different handle under the same rank (its context was re-created) remaps
+    if (peer_arena[g] && memcmp(&peer_handle[(size_t)g * 64], handle, 64) != 0) {
+        cudaIpcCloseMemHandle(peer_arena[g]);
+        peer_arena[g] = nullptr;
+    }
+    if (!peer_arena[g]) {
+        cudaIpcMemHandle_t h;
+        memcpy(&h, handle, sizeof h);
+        void *p = nullptr;
+        SG_CUDA(cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
+        peer_arena[g] = (char *)p;
+        memcpy(&peer_handle[(size_t)g * 64], handle, 64);
+    }
+    return peer_arena[g];
+}
+inline uint64_t Ctx::arena_offset(const void *p, const char *what) const {
+    const char *c = (const char *)p;
+    SG_CHECK(arena && c >= arena && c < arena + arena_size, 4, what);
+    return (uint64_t)(c - arena);
 }
 inline void Ctx::pool_trim() {
     peer_close();
@@ -377,6 +404,18 @@ void ensure_reads_on_device(Ctx *ctx);
 void reads_pack_text(Ctx *ctx, const char *text, uint64_t text_bytes, const uint64_t *seq_off, const uint32_t *seq_len, int64_t n, int longest_valid);
 void reads_download(Ctx *ctx, uint64_t *words, uint64_t *offs, uint32_t *lens);
 void cov_filter(Ctx *ctx, int K, unsigned thr, int apply, uint8_t *keep_out, uint64_t *stats);   // covfilter.cu
+// distributed coverage filter (covfilter.cu)
+struct CovDist;
+CovDist *dist_cov_begin(Ctx *ctx, int K, unsigned thr, int world, int rank);
+void dist_cov_ipc_handle(CovDist *d, uint8_t *out96);
+void dist_cov_open_peers(CovDist *d, const uint8_t *descs);
+void dist_cov_bound(CovDist *d);
+void dist_cov_fill(CovDist *d);
+void dist_cov_filter(CovDist *d, int apply, uint8_t *keep_out, uint64_t *stats);
+void dist_cov_free(CovDist *d);
+// pure host arithmetic (exported for CPU tests): a key's owner rank and the capacity of a rank's slice
+uint32_t cov_owner_host(uint64_t key, int world);
+uint64_t cov_slice_capacity(uint64_t maxn, int world);
 
 // count.cu
 enum CountMode { kCanonical = 0, kAllWindows = 1 };

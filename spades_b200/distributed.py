@@ -81,6 +81,61 @@ class DistributedKMerCounter:
             L.sgpu_dist_free(h)
 
 
+def distributed_cov_filter(ctx, k_plus_one, threshold, group=None, apply=True, phase_done=None):
+    """reads_io.CovFilteringWrap over a read set sharded across the ranks of a torch.distributed process group: the verdicts, bound
+    and key width are those of one GPU over the union of the shards (in rank order). Returns (keep flags of this rank's reads as
+    they were, {"cardinality_upper_bound", "key_bits", "distinct_keys" (the union's), "distinct_keys_rank" (this rank's slice),
+    "kept" (this rank's reads)}); with apply the survivors become this rank's read set, ready for DistributedKMerCounter.
+    phase_done(name), if given, is called as each of "hll", "merge", "fill", "filter" ends (scripts/bench_dist_covfilter.py)."""
+    done = phase_done or (lambda name: None)
+    import torch
+    import torch.distributed as dist
+    L = ctx.L
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    backend_dev = "cuda" if dist.get_backend(group) == "nccl" else "cpu"
+    n, nw = C.c_int64(), C.c_uint64()
+    ctx.check(L.sgpu_reads_info(ctx.h, C.byref(n), C.byref(nw)))
+    keep = np.zeros(max(n.value, 1), np.uint8)
+    stats = np.zeros(4, np.uint64)
+    h = C.c_void_p()
+    ctx.check(L.sgpu_dist_cov_begin(ctx.h, int(k_plus_one), int(threshold), world, rank, C.byref(h)))
+    try:
+        done("hll")
+        desc = np.zeros(SGPU_IPC_BYTES, np.uint8)
+        for name, step in (("merge", L.sgpu_dist_cov_bound), ("fill", L.sgpu_dist_cov_fill)):
+            # descriptors of the registers, then of the table slices; the all_gather also orders the steps across the ranks
+            ctx.check(L.sgpu_dist_cov_ipc_handle(h, desc.ctypes.data_as(C.c_void_p)))
+            t_h = torch.from_numpy(desc).to(backend_dev)
+            hs = [torch.empty_like(t_h) for _ in range(world)]
+            dist.all_gather(hs, t_h, group=group)
+            descs = np.ascontiguousarray(torch.stack(hs).cpu().numpy())
+            ctx.check(L.sgpu_dist_cov_open_peers(h, descs.ctypes.data_as(C.c_void_p)))
+            ctx.check(step(h))
+            done(name)
+        dist.barrier(group=group)                     # every rank's windows are in the owners' slices
+        ctx.check(L.sgpu_dist_cov_filter(h, 1 if apply else 0, keep.ctypes.data_as(C.c_void_p), stats.ctypes.data_as(C.c_void_p)))
+        done("filter")
+        dist.barrier(group=group)                     # nobody reads my slice any more
+    finally:
+        L.sgpu_dist_cov_free(h)
+    tot = torch.tensor([int(stats[2])], dtype=torch.int64, device=backend_dev)
+    dist.all_reduce(tot, group=group)
+    return keep[: n.value], {"cardinality_upper_bound": int(stats[0]), "key_bits": int(stats[1]), "distinct_keys": int(tot.item()),
+                             "distinct_keys_rank": int(stats[2]), "kept": int(stats[3])}
+
+
+def cov_layout_host(world, cardinality_bound, keys):
+    """the distributed filter's layout alone (pure host arithmetic): (owner rank of each masked key, entries of a rank's slice)"""
+    from . import _lib
+    L = _lib.load()
+    keys = np.ascontiguousarray(keys, np.uint64)
+    owners = np.zeros(max(len(keys), 1), np.uint32)
+    cap = C.c_uint64()
+    if L.sgpu_dist_cov_layout_host(world, cardinality_bound, keys.ctypes.data_as(C.c_void_p), len(keys), owners.ctypes.data_as(C.c_void_p), C.byref(cap)):
+        raise ValueError("bad world size or arguments")
+    return owners[: len(keys)], int(cap.value)
+
+
 def plan_host(world, num_buckets, key_bits, all_counts, budget_bytes, record_bytes):
     """The pass / ownership planning alone (pure host arithmetic; used by the CPU gloo tests)."""
     from . import _lib
