@@ -96,6 +96,9 @@ typedef struct sgpu_times {
     uint64_t stage_h2d_bytes;
     uint64_t graph_junction_batches; /* junction batches of the last graph build (0 when it had no junctions, e.g. no k-mers or
                                       * only perfect loops); a batch never spans the junctions of two chunks of the k-mer set */
+    /* the last sgpu_reads_cov_filter / sgpu_reads_cov_filter_ex */
+    uint64_t cov_filter_passes;      /* key-range passes of the counting table (1 = one table) */
+    uint64_t cov_filter_table_bytes; /* device bytes of one pass's table */
 } sgpu_times;
 
 int sgpu_create(const sgpu_config *cfg, sgpu_ctx **out);
@@ -130,8 +133,20 @@ int sgpu_reads_download(sgpu_ctx *ctx, uint64_t *words, uint64_t *offs, uint32_t
  * (3) io::CovFilteringWrap (io/reads/coverage_filtering_read_wrapper.hpp): a read survives iff the median multiplicity of its K-mers is >=
  * threshold. keep_out (may be NULL): one byte per read of the CURRENT read set, 1 = survives. apply != 0: the survivors (order kept) become
  * the context's read set, as the wrapper does to the pipeline's streams. stats (may be NULL): [0] cardinality upper bound, [1] key bits of
- * the filter (qbits + 8), [2] distinct keys counted, [3] reads kept. */
+ * the filter (qbits + 8), [2] distinct keys counted, [3] reads kept.
+ * The counting table takes 12 bytes per key of the bound in one piece (1.5 x the bound, 8-byte entries). When it does not fit the
+ * device memory left (the context's hbm_budget_bytes minus what it holds, or 90 % of the arena's free bytes), the key space is split
+ * into P ranges and the reads, which stay on the device, are rolled twice per range (fill, then lookup) against a table of about
+ * 1/P of the size: the smallest P that fits, at most 256, else SGPU_ENOMEM. The outputs are the same for every P. */
 int sgpu_reads_cov_filter(sgpu_ctx *ctx, int K, unsigned threshold, int apply, uint8_t *keep_out, uint64_t *stats);
+/* the same with the passes chosen by the caller: 0 = planned as above, 1 = one table whatever the memory left, 2 .. 256 = that many
+ * key ranges */
+int sgpu_reads_cov_filter_ex(sgpu_ctx *ctx, int K, unsigned threshold, int apply, int passes, uint8_t *keep_out, uint64_t *stats);
+/* the pass plan alone (pure host arithmetic, no GPU): for a cardinality bound, n reads and the device bytes left after the bound,
+ * the key-range passes and the entries of one pass's table. budget_bytes also covers the filter's four per-read arrays (n + 1
+ * entries, 13 bytes per entry in all, each array in 512-byte blocks) and two 512-byte blocks. SGPU_ENOMEM (passes = 0) when 256
+ * passes do not fit. */
+int sgpu_cov_pass_plan_host(uint64_t cardinality_bound, int64_t nreads, uint64_t budget_bytes, int *passes, uint64_t *pass_capacity);
 /* use a read set that already lives in device memory (not copied, must stay valid while the context uses it) */
 int sgpu_reads_adopt_device(sgpu_ctx *ctx, const uint64_t *d_words, uint64_t nwords, const uint64_t *d_offs, const uint32_t *d_lens, int64_t nreads);
 

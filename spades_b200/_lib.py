@@ -12,7 +12,7 @@ LIB_PATH = os.path.join(_HERE, "libspades_b200.so")
 SYMBOLS = [
     "sgpu_create", "sgpu_destroy", "sgpu_last_error", "sgpu_get_times",
     "sgpu_reads_clear", "sgpu_reads_append_packed", "sgpu_reads_upload", "sgpu_reads_adopt_device", "sgpu_reads_pack_text", "sgpu_reads_info",
-    "sgpu_reads_download", "sgpu_text_index_fastx", "sgpu_reads_cov_filter",
+    "sgpu_reads_download", "sgpu_text_index_fastx", "sgpu_reads_cov_filter", "sgpu_reads_cov_filter_ex", "sgpu_cov_pass_plan_host",
     "sgpu_fastx_parse", "sgpu_fastx_parse_threads", "sgpu_seqfile_parse", "sgpu_read_batch_write_seqfile", "sgpu_read_batch_num_reads", "sgpu_read_batch_num_words",
     "sgpu_read_batch_words", "sgpu_read_batch_offs", "sgpu_read_batch_lens", "sgpu_read_batch_stats", "sgpu_read_batch_error", "sgpu_read_batch_free",
     "sgpu_reads_append_batch",
@@ -48,7 +48,8 @@ class SgpuTimes(C.Structure):
                 ("level_a_key_bits", C.c_uint64), ("level_a_scatters", C.c_uint64), ("refine_rounds_max", C.c_uint64),
                 ("refine_splits_round0", C.c_uint64), ("refine_splits_later", C.c_uint64), ("sort_lsd_fallbacks", C.c_uint64),
                 ("sort_oversize_equal", C.c_uint64), ("result_d2h_bytes", C.c_uint64), ("result_d2h_wait_ms", C.c_float),
-                ("stage_h2d_bytes", C.c_uint64), ("graph_junction_batches", C.c_uint64)]
+                ("stage_h2d_bytes", C.c_uint64), ("graph_junction_batches", C.c_uint64),
+                ("cov_filter_passes", C.c_uint64), ("cov_filter_table_bytes", C.c_uint64)]
 
 
 _lib = None
@@ -75,6 +76,8 @@ def load():
     L.sgpu_reads_info.restype = i32; L.sgpu_reads_info.argtypes = [vp, C.POINTER(i64), C.POINTER(u64)]
     L.sgpu_reads_download.restype = i32; L.sgpu_reads_download.argtypes = [vp, vp, vp, vp]
     L.sgpu_reads_cov_filter.restype = i32; L.sgpu_reads_cov_filter.argtypes = [vp, i32, C.c_uint, i32, vp, vp]
+    L.sgpu_reads_cov_filter_ex.restype = i32; L.sgpu_reads_cov_filter_ex.argtypes = [vp, i32, C.c_uint, i32, i32, vp, vp]
+    L.sgpu_cov_pass_plan_host.restype = i32; L.sgpu_cov_pass_plan_host.argtypes = [u64, i64, u64, C.POINTER(i32), C.POINTER(u64)]
     L.sgpu_text_index_fastx.restype = i64; L.sgpu_text_index_fastx.argtypes = [vp, u64, vp, vp, i64]
     L.sgpu_reads_adopt_device.restype = i32; L.sgpu_reads_adopt_device.argtypes = [vp, vp, u64, vp, vp, i64]
     L.sgpu_fastx_parse.restype = i32; L.sgpu_fastx_parse.argtypes = [C.c_char_p, i32, pp]

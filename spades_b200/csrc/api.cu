@@ -99,6 +99,7 @@ int sgpu_get_times(const sgpu_ctx *ctx, sgpu_times *out) {
     out->sort_lsd_fallbacks = t.sort_lsd_fallbacks; out->sort_oversize_equal = t.sort_oversize_equal;
     out->result_d2h_bytes = t.result_d2h_bytes; out->result_d2h_wait_ms = t.result_d2h_wait;
     out->stage_h2d_bytes = t.stage_h2d_bytes; out->graph_junction_batches = t.graph_junction_batches;
+    out->cov_filter_passes = t.cov_filter_passes; out->cov_filter_table_bytes = t.cov_filter_table_bytes;
     return SGPU_OK;
 }
 
@@ -165,7 +166,19 @@ int sgpu_reads_pack_text(sgpu_ctx *ctx, const char *text, uint64_t text_bytes, c
 int sgpu_reads_cov_filter(sgpu_ctx *ctx, int K, unsigned threshold, int apply, uint8_t *keep_out, uint64_t *stats) {
     if (!ctx) return SGPU_EINVAL;
     Ctx *c = &ctx->c;
-    API_TRY(c, { SG_CUDA(cudaSetDevice(c->device)); cov_filter(c, K, threshold, apply, keep_out, stats); })
+    API_TRY(c, { SG_CUDA(cudaSetDevice(c->device)); cov_filter(c, K, threshold, apply, 0, keep_out, stats); })
+}
+int sgpu_reads_cov_filter_ex(sgpu_ctx *ctx, int K, unsigned threshold, int apply, int passes, uint8_t *keep_out, uint64_t *stats) {
+    if (!ctx || passes < 0 || passes > kCovMaxPasses) return SGPU_EINVAL;
+    Ctx *c = &ctx->c;
+    API_TRY(c, { SG_CUDA(cudaSetDevice(c->device)); cov_filter(c, K, threshold, apply, passes, keep_out, stats); })
+}
+int sgpu_cov_pass_plan_host(uint64_t cardinality_bound, int64_t nreads, uint64_t budget_bytes, int *passes, uint64_t *pass_capacity) {
+    if (nreads < 0 || !passes || !pass_capacity) return SGPU_EINVAL;
+    const CovPassPlan pl = cov_pass_plan(cardinality_bound, nreads, budget_bytes);
+    *passes = pl.passes;
+    *pass_capacity = pl.cap;
+    return pl.passes ? SGPU_OK : SGPU_ENOMEM;
 }
 int sgpu_reads_info(sgpu_ctx *ctx, int64_t *nreads, uint64_t *nwords) {
     if (!ctx || !nreads || !nwords) return SGPU_EINVAL;

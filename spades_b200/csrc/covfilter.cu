@@ -284,6 +284,61 @@ __global__ void cov_filter_dist_k(const uint64_t *__restrict__ words, const uint
     keep_words[r] = k ? (uint32_t)((L + 31) >> 5) : 0u;
 }
 
+// ---- key-range passes: a table too large for the device is built and read in P passes over the resident reads ----------------------
+// Pass p holds the keys with cov_owner(key, P) == p in a table of cov_slice_capacity(bound, P) entries. Every key lands in exactly one
+// pass with all of its windows, so its count, each read's number of windows below the threshold and the distinct keys summed over the
+// passes are those of the single table. The pass hash composes with the rank owner: floor(h*W*P / 2^64) / P == floor(h*W / 2^64), so
+// cov_owner(key, W*P) / P == cov_owner(key, W) and a distributed filter with passes can take id = cov_owner(key, W*P), owner = id / P,
+// pass = id % P without changing which rank owns a key.
+
+// cov_fill_k restricted to the keys of pass `pass`
+__global__ void cov_fill_pass_k(const uint64_t *__restrict__ words, const uint64_t *__restrict__ offs, const uint32_t *__restrict__ lens, int64_t n,
+                                int K, CovTable t, unsigned thr, uint32_t passes, uint32_t pass) {
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const int L = (int)lens[r];
+    if (L < K) return;
+    const uint64_t *seq = words + offs[r];
+    CycHash h = cyc_init(seq, K);
+    for (int j = 0;; ++j) {
+        const uint64_t key = h.value() & t.key_mask;
+        if (cov_owner(key, passes) == pass) {
+            t.add(key, thr);
+            if ((K & 1) == 0 && h.fwd == h.rvs && window_self_rc(seq, j, K)) t.add(key, thr);
+        }
+        if (j + K >= L) break;
+        cyc_roll(h, base_at(seq, j), base_at(seq, j + K), K);
+    }
+}
+
+// cov_filter_k over pass `pass`: the read's windows of this pass below the threshold are added to below[r] (one thread per read, no
+// atomics); the last pass gives the verdict from the sum
+__global__ void cov_filter_pass_k(const uint64_t *__restrict__ words, const uint64_t *__restrict__ offs, const uint32_t *__restrict__ lens, int64_t n,
+                                  int K, CovTable t, unsigned thr, uint32_t passes, uint32_t pass, uint32_t *__restrict__ below,
+                                  uint8_t *__restrict__ keep, uint32_t *__restrict__ keep_words) {
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const bool last = pass + 1 == passes;
+    const int L = (int)lens[r];
+    bool k = thr == 0;                                         // CountMedianMlt returns 0 for a read shorter than K
+    if (L >= K) {
+        const uint64_t *seq = words + offs[r];
+        CycHash h = cyc_init(seq, K);
+        uint32_t b = pass ? below[r] : 0u;
+        for (int j = 0;; ++j) {
+            const uint64_t key = h.value() & t.key_mask;
+            if (cov_owner(key, passes) == pass) b += t.count(key) < thr;
+            if (j + K >= L) break;
+            cyc_roll(h, base_at(seq, j), base_at(seq, j + K), K);
+        }
+        if (!last) { below[r] = b; return; }
+        k = b <= (uint32_t)(L - K + 1) / 2;
+    }
+    if (!last) return;
+    keep[r] = k ? 1 : 0;
+    keep_words[r] = k ? (uint32_t)((L + 31) >> 5) : 0u;
+}
+
 }  // namespace
 
 // hll<24>::cardinality / upper_bound_cardinality (adt/hll.hpp:50-68): same operations in the same order
@@ -346,9 +401,10 @@ struct CovVerdicts {
     }
 };
 
-void cov_filter(Ctx *ctx, int K, unsigned thr, int apply, uint8_t *keep_out, uint64_t *stats) {
+void cov_filter(Ctx *ctx, int K, unsigned thr, int apply, int passes, uint8_t *keep_out, uint64_t *stats) {
     SG_CHECK(K >= 1 && K <= 128, 2, "K must be in [1,128]");
     SG_CHECK(thr <= 60000u, 2, "coverage threshold must be at most 60000");
+    SG_CHECK(passes >= 0 && passes <= kCovMaxPasses, 2, "coverage filter: passes must be in [0, 256] (0 = planned)");
     ensure_reads_on_device(ctx);
     cudaStream_t st = ctx->stream;
     const int64_t n = ctx->n_reads;
@@ -363,27 +419,63 @@ void cov_filter(Ctx *ctx, int K, unsigned thr, int apply, uint8_t *keep_out, uin
         SG_CUDA(cudaStreamSynchronize(st));
     }
     const size_t maxn = (size_t)hll_upper_bound(h_reg);
-    // 2. the table
+    // 2. the table: one, or one per key range when one table does not fit next to the per-read arrays (cov_plan.h)
     const unsigned key_bits = cov_key_bits(maxn);
-    CovTable t;
-    t.cap = std::max<uint64_t>(1024, (uint64_t)maxn + (uint64_t)maxn / 2);
-    t.key_mask = (1ull << key_bits) - 1;
-    DArr<unsigned long long> table(ctx, t.cap);
-    t.e = table.p;
-    SG_CUDA(cudaMemsetAsync(table.p, 0, table.bytes(), st));
+    const uint64_t budget = ctx->budget_left();
+    const CovPassPlan plan = cov_pass_plan(maxn, n, budget);
+    if (!passes) {
+        if (!plan.passes) {
+            char m[256];
+            snprintf(m, sizeof m, "coverage filter: %llu device bytes needed with %d key-range passes (cardinality bound %zu), %llu left",
+                     (unsigned long long)plan.need, kCovMaxPasses, maxn, (unsigned long long)budget);
+            throw Error(4, m);
+        }
+        passes = plan.passes;
+    }
     CovVerdicts v(ctx);
     DArr<unsigned long long> d_cnt(ctx, 1);
     DArr<unsigned> d_ovf(ctx, 1);
+    DArr<uint32_t> below;
+    if (passes > 1) below.alloc(ctx, (size_t)n + 1);
+    CovTable t;
+    t.cap = cov_pass_capacity(maxn, passes);
+    t.key_mask = (1ull << key_bits) - 1;
+    DArr<unsigned long long> table(ctx, t.cap);
+    t.e = table.p;
+    ctx->times.cov_filter_passes = (uint64_t)passes;
+    ctx->times.cov_filter_table_bytes = table.bytes();
     SG_CUDA(cudaMemsetAsync(d_cnt.p, 0, 8, st));
     SG_CUDA(cudaMemsetAsync(d_ovf.p, 0, 4, st));
     t.overflow = d_ovf.p;
-    if (n) {
-        cov_fill_k<<<div_up(n, T), T, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, t, thr);
-        cov_filter_k<<<div_up(n, T), T, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, t, thr, v.keep.p, v.keep_words.p);
-        ctx->launches += 2;
+    if (passes == 1) {
+        SG_CUDA(cudaMemsetAsync(table.p, 0, table.bytes(), st));
+        if (n) {
+            cov_fill_k<<<div_up(n, T), T, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, t, thr);
+            cov_filter_k<<<div_up(n, T), T, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, t, thr, v.keep.p, v.keep_words.p);
+            ctx->launches += 2;
+        }
+        cov_distinct_k<<<ctx->num_sms * 4, 256, 0, st>>>(table.p, t.cap, d_cnt.p);
+        ctx->launches++;
+    } else {
+        for (int p = 0; p < passes; ++p) {
+            SG_CUDA(cudaMemsetAsync(table.p, 0, table.bytes(), st));
+            if (n) {
+                cov_fill_pass_k<<<div_up(n, T), T, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, t, thr, (uint32_t)passes, (uint32_t)p);
+                cov_filter_pass_k<<<div_up(n, T), T, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, t, thr, (uint32_t)passes, (uint32_t)p,
+                                                             below.p, v.keep.p, v.keep_words.p);
+                ctx->launches += 2;
+            }
+            cov_distinct_k<<<ctx->num_sms * 4, 256, 0, st>>>(table.p, t.cap, d_cnt.p);       // adds to the count of the passes before
+            ctx->launches++;
+            unsigned overflow = 0;
+            SG_CUDA(cudaMemcpyAsync(&overflow, d_ovf.p, 4, cudaMemcpyDeviceToHost, st));
+            SG_CUDA(cudaGetLastError());
+            SG_CUDA(cudaStreamSynchronize(st));
+            SG_CHECK(!overflow, 6, "coverage filter: more distinct keys than the cardinality bound allows (table full)");
+        }
     }
-    cov_distinct_k<<<ctx->num_sms * 4, 256, 0, st>>>(table.p, t.cap, d_cnt.p);
-    ctx->launches++;
+    table.release();                                   // the scans and the compaction below take its place (same stream)
+    below.release();
     v.scan(keep_out);
     unsigned long long distinct = 0;
     SG_CUDA(cudaMemcpyAsync(&distinct, d_cnt.p, 8, cudaMemcpyDeviceToHost, st));
@@ -397,12 +489,7 @@ void cov_filter(Ctx *ctx, int K, unsigned thr, int apply, uint8_t *keep_out, uin
 }
 
 // ---- distributed filter (sgpu_dist_cov_*): every rank holds a shard of the reads; the result equals cov_filter over the union --------
-// Slice capacity: 1.5 x an even share of the bound, like the single-GPU table, plus 8 standard deviations of a binomial owner load
-// (at most sqrt(share)) for the unevenness of the owner hash. A slice overflows only when its distinct keys exceed the capacity.
-uint64_t cov_slice_capacity(uint64_t maxn, int world) {
-    const uint64_t share = (maxn + (uint64_t)world - 1) / (uint64_t)world;
-    return std::max<uint64_t>(1024, share + share / 2 + 8 * (uint64_t)std::ceil(std::sqrt((double)share)));
-}
+// A rank's slice holds cov_slice_capacity(bound, world) entries (cov_plan.h).
 uint32_t cov_owner_host(uint64_t key, int world) { return cov_owner(key, (uint32_t)world); }
 
 struct CovDist {

@@ -13,6 +13,7 @@
 #include <string>
 #include <vector>
 
+#include "cov_plan.h"
 #include "kmer_dev.cuh"
 
 namespace sg {
@@ -80,6 +81,8 @@ struct PhaseTimes {   // device milliseconds measured with CUDA events on ctx->s
     // the junction batches of the last graph build
     uint64_t stage_h2d_bytes = 0;
     uint64_t graph_junction_batches = 0;
+    // the last single-GPU coverage pre-filter: key-range passes, and the bytes of one pass's table
+    uint64_t cov_filter_passes = 0, cov_filter_table_bytes = 0;
 };
 
 struct Ctx {
@@ -403,7 +406,8 @@ void ensure_reads_on_device(Ctx *ctx);
 // ingest_gpu.cu
 void reads_pack_text(Ctx *ctx, const char *text, uint64_t text_bytes, const uint64_t *seq_off, const uint32_t *seq_len, int64_t n, int longest_valid);
 void reads_download(Ctx *ctx, uint64_t *words, uint64_t *offs, uint32_t *lens);
-void cov_filter(Ctx *ctx, int K, unsigned thr, int apply, uint8_t *keep_out, uint64_t *stats);   // covfilter.cu
+// covfilter.cu; passes = 0: planned against the context's device budget (cov_plan.h), 1: one table, >= 2: that many key-range passes
+void cov_filter(Ctx *ctx, int K, unsigned thr, int apply, int passes, uint8_t *keep_out, uint64_t *stats);
 // distributed coverage filter (covfilter.cu)
 struct CovDist;
 CovDist *dist_cov_begin(Ctx *ctx, int K, unsigned thr, int world, int rank);
@@ -413,9 +417,8 @@ void dist_cov_bound(CovDist *d);
 void dist_cov_fill(CovDist *d);
 void dist_cov_filter(CovDist *d, int apply, uint8_t *keep_out, uint64_t *stats);
 void dist_cov_free(CovDist *d);
-// pure host arithmetic (exported for CPU tests): a key's owner rank and the capacity of a rank's slice
+// pure host arithmetic (exported for CPU tests): a key's owner rank; table capacities and the pass plan are in cov_plan.h
 uint32_t cov_owner_host(uint64_t key, int world);
-uint64_t cov_slice_capacity(uint64_t maxn, int world);
 
 // count.cu
 enum CountMode { kCanonical = 0, kAllWindows = 1 };

@@ -136,6 +136,20 @@ def cov_layout_host(world, cardinality_bound, keys):
     return owners[: len(keys)], int(cap.value)
 
 
+def cov_pass_plan_host(cardinality_bound, nreads, budget_bytes):
+    """the single-GPU filter's key-range pass plan alone (pure host arithmetic): (passes, entries of one pass's table) for the device
+    bytes left after the cardinality bound; raises MemoryError when 256 passes do not fit"""
+    from . import _lib
+    L = _lib.load()
+    passes, cap = C.c_int(), C.c_uint64()
+    rc = L.sgpu_cov_pass_plan_host(cardinality_bound, nreads, budget_bytes, C.byref(passes), C.byref(cap))
+    if rc == 4:
+        raise MemoryError("the coverage filter's table does not fit %d bytes in 256 key-range passes" % budget_bytes)
+    if rc:
+        raise ValueError("bad arguments")
+    return passes.value, int(cap.value)
+
+
 def plan_host(world, num_buckets, key_bits, all_counts, budget_bytes, record_bytes):
     """The pass / ownership planning alone (pure host arithmetic; used by the CPU gloo tests)."""
     from . import _lib

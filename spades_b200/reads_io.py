@@ -108,15 +108,21 @@ def download_reads(ctx):
     return words[: nw.value], offs[: n.value], lens[: n.value]
 
 
-def CovFilteringWrap(ctx, k_plus_one, threshold, apply=True):
+def CovFilteringWrap(ctx, k_plus_one, threshold, apply=True, passes=0):
     """The construction stage's coverage pre-filter (stages/construction.cpp:167-198: EstimateCardinalityUpperBound -> qf::cqf ->
     FillCoverageHistogram -> io::CovFilteringWrap, io/reads/coverage_filtering_read_wrapper.hpp:100-122) on the context's read set:
     a read survives iff the median multiplicity of its (k+1)-mers reaches `threshold`. Returns (keep flags of the reads as they were,
-    {"cardinality_upper_bound", "key_bits", "distinct_keys", "kept"}); with apply the survivors become the context's read set."""
+    {"cardinality_upper_bound", "key_bits", "distinct_keys", "kept"}); with apply the survivors become the context's read set.
+    passes: 0 = one counting table, or key-range passes when it does not fit the device memory left; 1 = one table; 2 .. 256 = that
+    many key-range passes. The result is the same for every value; Context.times() reports the passes taken."""
     n, nw = C.c_int64(), C.c_uint64()
     ctx.check(ctx.L.sgpu_reads_info(ctx.h, C.byref(n), C.byref(nw)))
     keep = np.zeros(max(n.value, 1), np.uint8)
     stats = np.zeros(4, np.uint64)
-    ctx.check(ctx.L.sgpu_reads_cov_filter(ctx.h, int(k_plus_one), int(threshold), 1 if apply else 0, keep.ctypes.data_as(C.c_void_p),
-                                          stats.ctypes.data_as(C.c_void_p)))
+    args = (int(k_plus_one), int(threshold), 1 if apply else 0)
+    out = (keep.ctypes.data_as(C.c_void_p), stats.ctypes.data_as(C.c_void_p))
+    if passes == 0:
+        ctx.check(ctx.L.sgpu_reads_cov_filter(ctx.h, *args, *out))
+    else:
+        ctx.check(ctx.L.sgpu_reads_cov_filter_ex(ctx.h, *args, int(passes), *out))
     return keep[: n.value], {"cardinality_upper_bound": int(stats[0]), "key_bits": int(stats[1]), "distinct_keys": int(stats[2]), "kept": int(stats[3])}
