@@ -204,12 +204,22 @@ int sgpu_kset_download_keys(const sgpu_kset *s, int64_t first, int64_t n, uint64
 int sgpu_kset_download_counts(const sgpu_kset *s, int64_t first, int64_t n, uint32_t *out);   /* SGPU_CANONICAL sets only */
 /* writes <prefix>.<b> for every bucket in the reference's bucket file format (raw W-byte records) */
 int sgpu_kset_write_buckets(const sgpu_kset *s, const char *prefix);
+/* the buckets a set holds (flags: num_buckets bytes, 1 = owned): every bucket for a single-GPU set, this rank's share of every pass
+ * for a set from sgpu_dist_end. sgpu_kset_write_owned_buckets writes <prefix>.<b> for the owned buckets only, so the ranks of a
+ * distributed count writing into one directory leave each bucket file once: together the complete set of bucket files. */
+int sgpu_kset_owned_buckets(const sgpu_kset *s, uint8_t *flags);
+int sgpu_kset_write_owned_buckets(const sgpu_kset *s, const char *prefix);
 int sgpu_kset_write_final(const sgpu_kset *s, const char *path);      /* final_kmers */
 void sgpu_kset_free(sgpu_kset *s);
 
 int sgpu_mphf_build(sgpu_ctx *ctx, const sgpu_kset *s, sgpu_mphf **out);
 int64_t sgpu_mphf_serialized_size(const sgpu_mphf *m);
 int sgpu_mphf_serialize(const sgpu_mphf *m, uint8_t *out, int64_t cap);
+/* the serialized buckets [b_lo, b_hi) alone: the bytes sgpu_mphf_serialize writes for them between num_segments and segment_starts.
+ * A bucket's bytes depend on its own keys only, so the index of a distributed k-mer set is assembled from its owners' buckets.
+ * The size is -1 for a bad range. */
+int64_t sgpu_mphf_serialized_size_buckets(const sgpu_mphf *m, int b_lo, int b_hi);
+int sgpu_mphf_serialize_buckets(const sgpu_mphf *m, int b_lo, int b_hi, uint8_t *out, int64_t cap);
 int sgpu_mphf_lookup(const sgpu_mphf *m, const uint64_t *keys, int64_t n, uint64_t *out_idx);   /* host keys, stored (minimal) form */
 void sgpu_mphf_free(sgpu_mphf *m);
 
@@ -288,6 +298,12 @@ void sgpu_edge_index_free(sgpu_edge_index *e);
  * Passes are planned one at a time against the memory every rank has free at that moment (like sgpu_count's bucket-group passes). */
 typedef struct sgpu_dist sgpu_dist;
 int sgpu_dist_begin(sgpu_ctx *ctx, int K, int num_buckets, int mode, int world, int rank, sgpu_dist **out);
+/* the same sequence over this rank's (k+1)-mer set instead of its reads: sgpu_kmers_from_kpomers_ex distributed. mode = 0 or
+ * SGPU_RESULT_ON_HOST; the source may live in HBM or in host memory (its chunks are uploaded for the histogram and every scatter).
+ * Every rank passes the same num_buckets and a set of the same k + 1 >= 2; the sets may be any (k+1)-mer sets, and may overlap:
+ * the ranks end with the k-mers of the union of the sets, each bucket on its owner, without multiplicities. The source must not
+ * change while the count runs; sgpu_kset_free of it is deferred until sgpu_dist_free. */
+int sgpu_dist_begin_kpomers(sgpu_ctx *ctx, const sgpu_kset *kpomers, int num_buckets, int mode, int world, int rank, sgpu_dist **out);
 int64_t sgpu_dist_num_partitions(const sgpu_dist *d);
 int sgpu_dist_local_counts(sgpu_dist *d, uint64_t *out);                 /* num_partitions host entries */
 int sgpu_dist_plan(sgpu_dist *d, const uint64_t *all_counts /* world x num_partitions, rank-major, host */, uint64_t *total_records);

@@ -19,12 +19,14 @@ SYMBOLS = [
     "sgpu_count", "sgpu_kmers_from_kpomers", "sgpu_kmers_from_kpomers_ex",
     "sgpu_kset_size", "sgpu_kset_k", "sgpu_kset_num_buckets", "sgpu_kset_record_bytes", "sgpu_kset_on_host", "sgpu_kset_bucket_sizes",
     "sgpu_kset_checksum", "sgpu_kset_download_keys", "sgpu_kset_download_counts", "sgpu_kset_write_buckets", "sgpu_kset_write_final", "sgpu_kset_free",
+    "sgpu_kset_owned_buckets", "sgpu_kset_write_owned_buckets",
     "sgpu_mphf_build", "sgpu_mphf_serialized_size", "sgpu_mphf_serialize", "sgpu_mphf_lookup", "sgpu_mphf_free",
+    "sgpu_mphf_serialized_size_buckets", "sgpu_mphf_serialize_buckets",
     "sgpu_graph_build", "sgpu_graph_build_ex", "sgpu_graph_build_opts", "sgpu_graph_build_streamed", "sgpu_graph_at_clipper_stats", "sgpu_graph_tip_clipper_stats", "sgpu_graph_masks", "sgpu_graph_coverage", "sgpu_graph_histogram", "sgpu_graph_num_unitigs",
     "sgpu_graph_unitig_bases", "sgpu_graph_unitigs", "sgpu_graph_gfa", "sgpu_graph_write_gfa", "sgpu_graph_free",
     "sgpu_edge_index_build", "sgpu_edge_index_k", "sgpu_edge_index_size", "sgpu_edge_index_serialized_size", "sgpu_edge_index_serialize",
     "sgpu_edge_index_values", "sgpu_edge_index_lookup", "sgpu_edge_index_free",
-    "sgpu_dist_begin", "sgpu_dist_num_partitions", "sgpu_dist_local_counts", "sgpu_dist_plan", "sgpu_dist_free_bytes", "sgpu_dist_next_pass", "sgpu_dist_ipc_handle",
+    "sgpu_dist_begin", "sgpu_dist_begin_kpomers", "sgpu_dist_num_partitions", "sgpu_dist_local_counts", "sgpu_dist_plan", "sgpu_dist_free_bytes", "sgpu_dist_next_pass", "sgpu_dist_ipc_handle",
     "sgpu_dist_open_peers", "sgpu_dist_scatter", "sgpu_dist_exchange", "sgpu_dist_sort", "sgpu_dist_end", "sgpu_dist_free", "sgpu_dist_plan_host",
     "sgpu_dist_cov_begin", "sgpu_dist_cov_ipc_handle", "sgpu_dist_cov_open_peers", "sgpu_dist_cov_bound", "sgpu_dist_cov_fill", "sgpu_dist_cov_filter",
     "sgpu_dist_cov_free", "sgpu_dist_cov_layout_host",
@@ -106,11 +108,15 @@ def load():
     L.sgpu_kset_download_keys.restype = i32; L.sgpu_kset_download_keys.argtypes = [vp, i64, i64, vp]
     L.sgpu_kset_download_counts.restype = i32; L.sgpu_kset_download_counts.argtypes = [vp, i64, i64, vp]
     L.sgpu_kset_write_buckets.restype = i32; L.sgpu_kset_write_buckets.argtypes = [vp, C.c_char_p]
+    L.sgpu_kset_owned_buckets.restype = i32; L.sgpu_kset_owned_buckets.argtypes = [vp, vp]
+    L.sgpu_kset_write_owned_buckets.restype = i32; L.sgpu_kset_write_owned_buckets.argtypes = [vp, C.c_char_p]
     L.sgpu_kset_write_final.restype = i32; L.sgpu_kset_write_final.argtypes = [vp, C.c_char_p]
     L.sgpu_kset_free.restype = None; L.sgpu_kset_free.argtypes = [vp]
     L.sgpu_mphf_build.restype = i32; L.sgpu_mphf_build.argtypes = [vp, vp, pp]
     L.sgpu_mphf_serialized_size.restype = i64; L.sgpu_mphf_serialized_size.argtypes = [vp]
     L.sgpu_mphf_serialize.restype = i32; L.sgpu_mphf_serialize.argtypes = [vp, vp, i64]
+    L.sgpu_mphf_serialized_size_buckets.restype = i64; L.sgpu_mphf_serialized_size_buckets.argtypes = [vp, i32, i32]
+    L.sgpu_mphf_serialize_buckets.restype = i32; L.sgpu_mphf_serialize_buckets.argtypes = [vp, i32, i32, vp, i64]
     L.sgpu_mphf_lookup.restype = i32; L.sgpu_mphf_lookup.argtypes = [vp, vp, i64, vp]
     L.sgpu_mphf_free.restype = None; L.sgpu_mphf_free.argtypes = [vp]
     L.sgpu_graph_build.restype = i32; L.sgpu_graph_build.argtypes = [vp, vp, vp, vp, vp, i32, pp]
@@ -137,6 +143,7 @@ def load():
     L.sgpu_edge_index_lookup.restype = i32; L.sgpu_edge_index_lookup.argtypes = [vp, vp, i64, vp]
     L.sgpu_edge_index_free.restype = None; L.sgpu_edge_index_free.argtypes = [vp]
     L.sgpu_dist_begin.restype = i32; L.sgpu_dist_begin.argtypes = [vp, i32, i32, i32, i32, i32, pp]
+    L.sgpu_dist_begin_kpomers.restype = i32; L.sgpu_dist_begin_kpomers.argtypes = [vp, vp, i32, i32, i32, i32, pp]
     L.sgpu_dist_num_partitions.restype = i64; L.sgpu_dist_num_partitions.argtypes = [vp]
     L.sgpu_dist_local_counts.restype = i32; L.sgpu_dist_local_counts.argtypes = [vp, vp]
     L.sgpu_dist_plan.restype = i32; L.sgpu_dist_plan.argtypes = [vp, vp, C.POINTER(u64)]

@@ -29,7 +29,8 @@ static void child_add(Ctx *c) { c->live_children++; }
 static void child_release(Ctx *c) {
     if (--c->live_children == 0 && c->destroy_pending) ctx_teardown(static_cast<sgpu_ctx *>(c->owner));
 }
-struct sgpu_kset { KSet *s; };
+// readers: distributed counts that read this set (sgpu_dist_begin_kpomers); sgpu_kset_free defers the release to the last of them
+struct sgpu_kset { KSet *s; mutable int readers = 0; mutable bool free_pending = false; };
 struct sgpu_mphf { Mphf *m; };
 struct sgpu_graph { Graph *g; };
 struct sgpu_edge_index { EdgeIndex *e; };
@@ -285,6 +286,26 @@ static void write_range(const KSet *ks, int64_t first, int64_t n, FILE *f) {
     }
 }
 
+// the buckets the set's chunks cover: all of them for a single-GPU count, this rank's share of every pass for a distributed one
+static std::vector<uint8_t> owned_buckets(const KSet *ks) {
+    std::vector<uint8_t> own((size_t)ks->B, 0);
+    for (const Chunk &ch : ks->chunks) std::fill(own.begin() + ch.b_lo, own.begin() + ch.b_hi, (uint8_t)1);
+    return own;
+}
+
+// <prefix>.<b> for every bucket, or for the owned ones only (ranks of a distributed count writing into one directory)
+static void write_bucket_files(const KSet *ks, const char *prefix, bool owned_only) {
+    const std::vector<uint8_t> own = owned_buckets(ks);
+    for (int b = 0; b < ks->B; ++b) {
+        if (owned_only && !own[b]) continue;
+        std::string p = std::string(prefix) + "." + std::to_string(b);
+        FILE *f = fopen(p.c_str(), "wb");
+        SG_CHECK(f, SGPU_EIO, "cannot open bucket file for writing");
+        try { write_range(ks, ks->bstart[b], ks->bsz[b], f); } catch (...) { fclose(f); throw; }
+        fclose(f);
+    }
+}
+
 extern "C" {
 
 int sgpu_kset_checksum(const sgpu_kset *s, uint64_t *out4) {
@@ -306,18 +327,21 @@ int sgpu_kset_download_counts(const sgpu_kset *s, int64_t first, int64_t n, uint
     })
 }
 
+int sgpu_kset_owned_buckets(const sgpu_kset *s, uint8_t *flags) {
+    if (!s || !flags) return SGPU_EINVAL;
+    const std::vector<uint8_t> own = owned_buckets(s->s);
+    memcpy(flags, own.data(), own.size());
+    return SGPU_OK;
+}
 int sgpu_kset_write_buckets(const sgpu_kset *s, const char *prefix) {
     if (!s || !prefix) return SGPU_EINVAL;
     Ctx *c = s->s->ctx;
-    API_TRY(c, {
-        for (int b = 0; b < s->s->B; ++b) {
-            std::string p = std::string(prefix) + "." + std::to_string(b);
-            FILE *f = fopen(p.c_str(), "wb");
-            SG_CHECK(f, SGPU_EIO, "cannot open bucket file for writing");
-            try { write_range(s->s, s->s->bstart[b], s->s->bsz[b], f); } catch (...) { fclose(f); throw; }
-            fclose(f);
-        }
-    })
+    API_TRY(c, write_bucket_files(s->s, prefix, false))
+}
+int sgpu_kset_write_owned_buckets(const sgpu_kset *s, const char *prefix) {
+    if (!s || !prefix) return SGPU_EINVAL;
+    Ctx *c = s->s->ctx;
+    API_TRY(c, write_bucket_files(s->s, prefix, true))
 }
 int sgpu_kset_write_final(const sgpu_kset *s, const char *path) {
     if (!s || !path) return SGPU_EINVAL;
@@ -331,6 +355,7 @@ int sgpu_kset_write_final(const sgpu_kset *s, const char *path) {
 }
 void sgpu_kset_free(sgpu_kset *s) {
     if (!s) return;
+    if (s->readers > 0) { s->free_pending = true; return; }       // released by the last sgpu_dist_free that reads it
     if (s->s) { Ctx *c = s->s->ctx; cudaSetDevice(c->device); delete s->s; child_release(c); }
     delete s;
 }
@@ -353,6 +378,18 @@ int sgpu_mphf_serialize(const sgpu_mphf *m, uint8_t *out, int64_t cap) {
     API_TRY(c, {
         SG_CUDA(cudaSetDevice(c->device));
         mphf_serialize_to(m->m, out, (size_t)cap);
+    })
+}
+int64_t sgpu_mphf_serialized_size_buckets(const sgpu_mphf *m, int b_lo, int b_hi) {
+    if (!m || b_lo < 0 || b_lo > b_hi || b_hi > m->m->B) return -1;
+    return (int64_t)mphf_serialized_size_buckets(m->m, b_lo, b_hi);
+}
+int sgpu_mphf_serialize_buckets(const sgpu_mphf *m, int b_lo, int b_hi, uint8_t *out, int64_t cap) {
+    if (!m || !out || cap < 0) return SGPU_EINVAL;
+    Ctx *c = m->m->ctx;
+    API_TRY(c, {
+        SG_CUDA(cudaSetDevice(c->device));
+        mphf_serialize_buckets_to(m->m, b_lo, b_hi, out, (size_t)cap);
     })
 }
 int sgpu_mphf_lookup(const sgpu_mphf *m, const uint64_t *keys, int64_t n, uint64_t *out_idx) {
@@ -542,7 +579,7 @@ void sgpu_graph_free(sgpu_graph *g) {
 
 }  // extern "C"
 
-struct sgpu_dist { DistState *d; Ctx *c; };
+struct sgpu_dist { DistState *d; Ctx *c; const sgpu_kset *src; };     // src: the (k+1)-mer set read by sgpu_dist_begin_kpomers
 extern "C" {
 int sgpu_dist_begin(sgpu_ctx *ctx, int K, int num_buckets, int mode, int world, int rank, sgpu_dist **out) {
     if (!ctx || !out) return SGPU_EINVAL;
@@ -552,7 +589,21 @@ int sgpu_dist_begin(sgpu_ctx *ctx, int K, int num_buckets, int mode, int world, 
         SG_CUDA(cudaSetDevice(c->device));
         const bool on_host = (mode & SGPU_RESULT_ON_HOST) != 0;
         DistState *d = dist_begin(c, K, num_buckets, mode & ~SGPU_RESULT_ON_HOST, world, rank, on_host);
-        *out = new sgpu_dist{d, c};
+        *out = new sgpu_dist{d, c, nullptr};
+        child_add(c);
+    })
+}
+int sgpu_dist_begin_kpomers(sgpu_ctx *ctx, const sgpu_kset *kpomers, int num_buckets, int mode, int world, int rank, sgpu_dist **out) {
+    if (!ctx || !kpomers || !out) return SGPU_EINVAL;
+    *out = nullptr;
+    Ctx *c = &ctx->c;
+    API_TRY(c, {
+        SG_CHECK(mode == 0 || mode == SGPU_RESULT_ON_HOST, SGPU_EINVAL, "bad mode");
+        SG_CHECK(!kpomers->free_pending, SGPU_EINVAL, "the (k+1)-mer set has been freed");
+        SG_CUDA(cudaSetDevice(c->device));
+        DistState *d = dist_begin_kpomers(c, kpomers->s, num_buckets, world, rank, mode == SGPU_RESULT_ON_HOST);
+        *out = new sgpu_dist{d, c, kpomers};
+        kpomers->readers++;
         child_add(c);
     })
 }
@@ -604,8 +655,10 @@ void sgpu_dist_free(sgpu_dist *d) {
     Ctx *c = d->c;
     cudaSetDevice(c->device);
     dist_free(d->d);
+    const sgpu_kset *src = d->src;
     delete d;
     child_release(c);
+    if (src && --src->readers == 0 && src->free_pending) sgpu_kset_free(const_cast<sgpu_kset *>(src));
 }
 int sgpu_dist_plan_host(int world, int num_buckets, int key_bits_in_partition, const uint64_t *all_counts, uint64_t budget_bytes, int record_bytes,
                         int *pass_bounds, uint64_t *max_recv) {

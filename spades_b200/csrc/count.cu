@@ -2006,26 +2006,34 @@ KSet *count_from_reads(Ctx *ctx, int K, int B, int mode, bool result_on_host) {
     }
 }
 
+// one source per chunk of a (k+1)-mer set, read in place (a host set's chunks go through a ChunkStager)
+static std::vector<KmerSetSrc> kpomer_sources(const KSet *kp) {
+    std::vector<KmerSetSrc> srcs;
+    for (const Chunk &c : kp->chunks) {
+        KmerSetSrc s; s.words = c.keys.p; s.n = c.n; s.nwords = (uint64_t)c.n * kp->nw; s.K = kp->K - 1; s.stride = (uint32_t)kp->nw;
+        srcs.push_back(s);
+    }
+    return srcs;
+}
+static void check_kpomer_source(const KSet *kp) {
+    SG_CHECK(kp->K >= 2, 2, "source k-mers too short");
+    SG_CHECK(kp->nw == nwords_of(kp->K), 2, "unsupported k-mer word combination");
+}
+
 template <int NW>
 static KSet *kmers_from_kpomers_nw(Ctx *ctx, const KSet *kp, int B, bool on_host) {
     const int K = kp->K - 1;
     // a host (k+1)-mer set: every launch that reads a chunk's words reads its staged copy. Allocated before the passes are
     // planned, so the planner sees the two staging buffers.
     std::unique_ptr<ChunkStager> stage(kp->on_host ? new ChunkStager(kp, false) : nullptr);
-    std::vector<KmerSetSrc> srcs;
-    for (const Chunk &c : kp->chunks) {
-        KmerSetSrc s; s.words = c.keys.p; s.n = c.n; s.nwords = (uint64_t)c.n * kp->nw; s.K = K; s.stride = (uint32_t)kp->nw;
-        srcs.push_back(s);
-    }
     KSetBuilder set(ctx, K, NW, B, false, false, on_host);
-    run_count<NW, false>(ctx, srcs, K, (uint64_t)kp->n * 2, set, stage.get());
+    run_count<NW, false>(ctx, kpomer_sources(kp), K, (uint64_t)kp->n * 2, set, stage.get());
     return set.finish();
 }
 
 KSet *kmers_from_kpomers(Ctx *ctx, const KSet *kp, int B, bool result_on_host) {
-    SG_CHECK(kp->K >= 2, 2, "source k-mers too short");
+    check_kpomer_source(kp);
     SG_CHECK(B >= 1 && B <= (1 << 20), 2, "num_buckets must be in [1, 2^20]");
-    SG_CHECK(kp->nw == nwords_of(kp->K), 2, "unsupported k-mer word combination");
     ctx->times = PhaseTimes();
     switch (nwords_of(kp->K - 1)) {
         case 1: return kmers_from_kpomers_nw<1>(ctx, kp, B, result_on_host);
@@ -2156,13 +2164,14 @@ struct PullSrc { const uint64_t *sbuf; const uint64_t *pbase; const uint32_t *bl
 
 struct DistState {
     Ctx *ctx = nullptr;
-    int K = 0, B = 0, mode = 0, nw = 0, G = 0;
+    int K = 0, B = 0, nw = 0, G = 0;
     DistPlan plan;
     std::vector<uint64_t> h_cnt_all;         // world x PA_all
     DArr<uint64_t> sbuf, xbuf;               // staging buffer (peers read it; later the ping-pong partner) and the merged buffer
     DArr<uint64_t> pbase;                    // [G][max partitions of a pass]: piece starts of the current pass (peers read it)
     std::vector<PullSrc> peers;              // world entries (own entry = local pointers)
     std::unique_ptr<KSetBuilder> set;        // this rank's buckets, until sgpu_dist_end hands them over
+    std::unique_ptr<ChunkStager> stage;      // a host (k+1)-mer set: its chunks are uploaded for the histogram and for every scatter
     virtual ~DistState() = default;
     virtual void begin() = 0;
     virtual void local_counts(uint64_t *h_out) = 0;
@@ -2240,15 +2249,15 @@ __global__ void __launch_bounds__(kPullThreads) dist_pull_k(const PullSrc *__res
     }
 }
 
-template <int NW, bool BOTH>
+// Src: the context's reads (ReadsSrc), or the chunks of this rank's (k+1)-mer set (KmerSetSrc), set in job.srcs before begin()
+template <int NW, class Src, bool BOTH>
 struct DistStateNW : DistState {
-    LevelAJob<NW, ReadsSrc, BOTH> job;
+    LevelAJob<NW, Src, BOTH> job;
 
     void begin() override {
         Timer tm(ctx->stream);
         Trace tr(ctx->stream);
-        job.ctx = ctx; job.K = K; job.B = B; job.rA = plan.rA; job.G = G;
-        job.srcs.assign(1, reads_source(ctx, K));
+        job.ctx = ctx; job.K = K; job.B = B; job.rA = plan.rA; job.G = G; job.stage = stage.get();
         job.s_lo = 0; job.s_hi = B; job.PA_all = plan.PA_all;
         levelA_count(job, tm, tr);
     }
@@ -2329,27 +2338,25 @@ struct DistStateNW : DistState {
     }
 };
 
-template <int NW>
-static DistState *dist_state_new(int mode) {
-    if (mode == kAllWindows) return new DistStateNW<NW, true>();
-    return new DistStateNW<NW, false>();
+template <int NW, class Src, bool BOTH>
+static DistState *dist_state_of(std::vector<Src> srcs) {
+    auto *d = new DistStateNW<NW, Src, BOTH>();
+    d->job.srcs = std::move(srcs);
+    return d;
 }
+template <int NW>
+static DistState *dist_state_new(Ctx *ctx, int K, int mode) {
+    std::vector<ReadsSrc> srcs{reads_source(ctx, K)};
+    return mode == kAllWindows ? dist_state_of<NW, ReadsSrc, true>(srcs) : dist_state_of<NW, ReadsSrc, false>(srcs);
+}
+template <int NW>
+static DistState *dist_state_kpomers(const KSet *kp) { return dist_state_of<NW, KmerSetSrc, false>(kpomer_sources(kp)); }
 
-DistState *dist_begin(Ctx *ctx, int K, int B, int mode, int world, int rank, bool result_on_host) {
-    SG_CHECK(K >= 1 && K <= 128, 2, "K must be in [1,128]");
-    SG_CHECK(B >= 1 && B <= kLevelAMaxParts, 2, "distributed count: num_buckets must be in [1, 8192]");
-    SG_CHECK(world >= 1 && world <= 255 && rank >= 0 && rank < world, 2, "bad world/rank");
-    SG_CHECK(mode == kCanonical || mode == kAllWindows, 2, "bad mode");
-    ensure_reads_on_device(ctx);
-    ctx->times = PhaseTimes();
-    DistState *d = nullptr;
-    switch (nwords_of(K)) {
-        case 1: d = dist_state_new<1>(mode); break;
-        case 2: d = dist_state_new<2>(mode); break;
-        case 3: d = dist_state_new<3>(mode); break;
-        default: d = dist_state_new<4>(mode); break;
-    }
-    d->ctx = ctx; d->K = K; d->B = B; d->mode = mode; d->nw = nwords_of(K);
+// geometry, set and level-A histogram of a distributed count whose sources d already holds
+// (`counts`, `double_selfrc`: as KSetBuilder's); d is deleted on failure
+static DistState *dist_start(DistState *d, Ctx *ctx, int K, int B, int world, int rank, bool counts, bool double_selfrc, bool result_on_host,
+                             const KSet *staged) {
+    d->ctx = ctx; d->K = K; d->B = B; d->nw = nwords_of(K);
     d->G = ctx->num_sms * levelA_ctas_per_sm();
     // every rank must use the same geometry, so it depends on B only. As many level-A partitions as the shared-memory tables allow:
     // an owner's segment is the union of all ranks' records of a partition, so finer partitions keep refinement at one round
@@ -2358,10 +2365,51 @@ DistState *dist_begin(Ctx *ctx, int K, int B, int mode, int world, int rank, boo
     d->plan.world = world; d->plan.rank = rank; d->plan.B = B; d->plan.rA = rA; d->plan.PA_all = (uint32_t)B << rA;
     ctx->times.level_a_key_bits = (uint64_t)rA;
     try {
-        d->set.reset(new KSetBuilder(ctx, K, d->nw, B, mode == kCanonical, mode == kCanonical && K % 2 == 0, result_on_host));
+        // a host source's staging buffers are allocated before the histogram, so sgpu_dist_free_bytes sees them from the first pass
+        if (staged) d->stage.reset(new ChunkStager(staged, false));
+        d->set.reset(new KSetBuilder(ctx, K, d->nw, B, counts, double_selfrc, result_on_host));
         d->begin();
     } catch (...) { delete d; throw; }
     return d;
+}
+
+static void check_dist_args(int B, int world, int rank) {
+    SG_CHECK(B >= 1 && B <= kLevelAMaxParts, 2, "distributed count: num_buckets must be in [1, 8192]");
+    SG_CHECK(world >= 1 && world <= 255 && rank >= 0 && rank < world, 2, "bad world/rank");
+}
+
+DistState *dist_begin(Ctx *ctx, int K, int B, int mode, int world, int rank, bool result_on_host) {
+    SG_CHECK(K >= 1 && K <= 128, 2, "K must be in [1,128]");
+    check_dist_args(B, world, rank);
+    SG_CHECK(mode == kCanonical || mode == kAllWindows, 2, "bad mode");
+    ensure_reads_on_device(ctx);
+    ctx->times = PhaseTimes();
+    DistState *d = nullptr;
+    switch (nwords_of(K)) {
+        case 1: d = dist_state_new<1>(ctx, K, mode); break;
+        case 2: d = dist_state_new<2>(ctx, K, mode); break;
+        case 3: d = dist_state_new<3>(ctx, K, mode); break;
+        default: d = dist_state_new<4>(ctx, K, mode); break;
+    }
+    return dist_start(d, ctx, K, B, world, rank, mode == kCanonical, mode == kCanonical && K % 2 == 0, result_on_host, nullptr);
+}
+
+// the k-mers of this rank's (k+1)-mer set, bucket-owned like dist_begin's count; the records are those of kmers_from_kpomers
+// (no multiplicities). The ranks' sets may overlap: every owner's sort removes the duplicates its pieces bring.
+DistState *dist_begin_kpomers(Ctx *ctx, const KSet *kp, int B, int world, int rank, bool result_on_host) {
+    check_kpomer_source(kp);
+    SG_CHECK(kp->ctx == ctx, 2, "the (k+1)-mer set belongs to another context");
+    check_dist_args(B, world, rank);
+    ctx->times = PhaseTimes();
+    const int K = kp->K - 1;
+    DistState *d = nullptr;
+    switch (nwords_of(K)) {
+        case 1: d = dist_state_kpomers<1>(kp); break;
+        case 2: d = dist_state_kpomers<2>(kp); break;
+        case 3: d = dist_state_kpomers<3>(kp); break;
+        default: d = dist_state_kpomers<4>(kp); break;
+    }
+    return dist_start(d, ctx, K, B, world, rank, false, false, result_on_host, kp->on_host ? kp : nullptr);
 }
 uint32_t dist_num_partitions(const DistState *d) { return d->plan.PA_all; }
 void dist_local_counts(DistState *d, uint64_t *h_out) { d->local_counts(h_out); }

@@ -354,10 +354,10 @@ __global__ void ser_patches_k(const SerPatch *__restrict__ patches, uint64_t n, 
     if (p.nbytes == 8) img32[(p.dst_byte >> 2) + 1] = (uint32_t)(p.value >> 32);
 }
 
-size_t mphf_serialized_size(const Mphf *m) {
+size_t mphf_serialized_size_buckets(const Mphf *m, int b_lo, int b_hi) {
     const int B = m->B;
-    size_t total = 8;
-    for (int b = 0; b < B; ++b) {
+    size_t total = 0;
+    for (int b = b_lo; b < b_hi; ++b) {
         total += 28 + 8;
         if (m->bsz[b])
             for (int l = 0; l < kLevels; ++l) {
@@ -365,20 +365,24 @@ size_t mphf_serialized_size(const Mphf *m) {
                 total += 16 + 8 * m->nchar[p] + 8 + 8 * ((m->nchar[p] + 7) / 8);
             }
     }
-    return total + 8 * ((size_t)B + 1);
+    return total;
 }
+size_t mphf_serialized_size(const Mphf *m) { return 8 + mphf_serialized_size_buckets(m, 0, m->B) + 8 * ((size_t)m->B + 1); }
 
-void mphf_serialize_to(const Mphf *m, uint8_t *out, size_t cap) {
+// the image of buckets [b_lo, b_hi), with num_segments before and segment_starts after when `whole` (then [b_lo, b_hi) = [0, B))
+static void serialize_image(const Mphf *m, int b_lo, int b_hi, bool whole, uint8_t *out, size_t cap) {
     Ctx *ctx = m->ctx;
     const int B = m->B;
-    const size_t total = mphf_serialized_size(m);
+    SG_CHECK(b_lo >= 0 && b_lo <= b_hi && b_hi <= B, 2, "bucket range outside the index");
+    const size_t total = whole ? mphf_serialized_size(m) : mphf_serialized_size_buckets(m, b_lo, b_hi);
     SG_CHECK(total <= cap, 2, "output buffer too small for the serialized index");
+    if (total == 0) return;
     std::vector<SerPiece> pieces;
     std::vector<SerPatch> patches;
     size_t pos = 0;
     auto patch = [&](uint64_t v, uint32_t nbytes) { patches.push_back(SerPatch{pos, v, nbytes, 0}); pos += nbytes; };
-    patch((uint64_t)B, 8);
-    for (int b = 0; b < B; ++b) {
+    if (whole) patch((uint64_t)B, 8);
+    for (int b = b_lo; b < b_hi; ++b) {
         const double gamma = 4.0; uint64_t gbits; memcpy(&gbits, &gamma, 8);
         const uint64_t nelem = (uint64_t)m->bsz[b];
         patch(gbits, 8); patch((uint64_t)kLevels, 4);
@@ -396,7 +400,8 @@ void mphf_serialize_to(const Mphf *m, uint8_t *out, size_t cap) {
         }
         patch(0, 8);                                // final-hash map size (must be empty, checked at build time)
     }
-    for (int i = 0; i <= B; ++i) patch(m->starts[i], 8);
+    if (whole)
+        for (int i = 0; i <= B; ++i) patch(m->starts[i], 8);
     SG_CHECK(pos == total, 6, "internal: serialized size mismatch");
     DArr<uint32_t> img(ctx, total / 4 + 2);
     DArr<SerPiece> dp(ctx, pieces.size() + 1);
@@ -413,6 +418,8 @@ void mphf_serialize_to(const Mphf *m, uint8_t *out, size_t cap) {
     SG_CUDA(cudaMemcpyAsync(out, img.p, total, cudaMemcpyDeviceToHost, ctx->stream));
     SG_CUDA(cudaStreamSynchronize(ctx->stream));
 }
+void mphf_serialize_to(const Mphf *m, uint8_t *out, size_t cap) { serialize_image(m, 0, m->B, true, out, cap); }
+void mphf_serialize_buckets_to(const Mphf *m, int b_lo, int b_hi, uint8_t *out, size_t cap) { serialize_image(m, b_lo, b_hi, false, out, cap); }
 
 void mphf_lookup_host_keys(Ctx *ctx, const Mphf *m, const uint64_t *h_keys, int64_t n, uint64_t *h_out) {
     if (n <= 0) return;

@@ -431,6 +431,7 @@ void kset_checksum(const KSet *ks, uint64_t *out4);
 struct DistState;
 struct DistPlan;
 DistState *dist_begin(Ctx *ctx, int K, int B, int mode, int world, int rank, bool result_on_host = false);
+DistState *dist_begin_kpomers(Ctx *ctx, const KSet *kp, int B, int world, int rank, bool result_on_host);
 uint32_t dist_num_partitions(const DistState *d);
 void dist_local_counts(DistState *d, uint64_t *h_out);
 void dist_plan(DistState *d, const uint64_t *cnt_all, uint64_t *total_records);
@@ -450,6 +451,9 @@ int dist_plan_host(int world, int B, int rA, const uint64_t *cnt_all, uint64_t b
 Mphf *mphf_build(Ctx *ctx, const KSet *ks);
 size_t mphf_serialized_size(const Mphf *m);
 void mphf_serialize_to(const Mphf *m, uint8_t *out, size_t cap);
+// the bytes of buckets [b_lo, b_hi) alone: the middle of mphf_serialize_to's image, without num_segments and segment_starts
+size_t mphf_serialized_size_buckets(const Mphf *m, int b_lo, int b_hi);
+void mphf_serialize_buckets_to(const Mphf *m, int b_lo, int b_hi, uint8_t *out, size_t cap);
 void mphf_lookup_host_keys(Ctx *ctx, const Mphf *m, const uint64_t *h_keys, int64_t n, uint64_t *h_out);
 
 static inline int div_up(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }

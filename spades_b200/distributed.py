@@ -13,6 +13,68 @@ from .kmer_index import KMerDiskStorage, SGPU_CANONICAL, SGPU_RESULT_ON_HOST
 SGPU_IPC_BYTES = 96
 
 
+def _backend_device(group):
+    import torch.distributed as dist
+    return "cuda" if dist.get_backend(group) == "nccl" else "cpu"
+
+
+def _distributed_count(ctx, group, begin, budget_bytes):
+    """the pass loop of a distributed count over the ranks of `group`: begin(world, rank, handle pointer) starts it (sgpu_dist_begin
+    or sgpu_dist_begin_kpomers); returns (this rank's KMerDiskStorage, passes)"""
+    import torch
+    import torch.distributed as dist
+    L = ctx.L
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    backend_dev = _backend_device(group)
+    h = C.c_void_p()
+    ctx.check(begin(world, rank, C.byref(h)))
+    try:
+        npart = L.sgpu_dist_num_partitions(h)
+        local = np.zeros(npart, np.uint64)
+        ctx.check(L.sgpu_dist_local_counts(h, local.ctypes.data_as(C.c_void_p)))
+        # all_gather of the per-partition record counts (world x npart x 8 bytes: small)
+        t_local = torch.from_numpy(local.view(np.int64)).to(backend_dev)
+        gathered = [torch.empty_like(t_local) for _ in range(world)]
+        dist.all_gather(gathered, t_local, group=group)
+        all_counts = np.ascontiguousarray(torch.stack(gathered).cpu().numpy().view(np.uint64))
+        total = C.c_uint64()
+        ctx.check(L.sgpu_dist_plan(h, all_counts.ctypes.data_as(C.c_void_p), C.byref(total)))
+        npass = 0
+        while True:
+            # every pass is planned against what ALL ranks can allocate right now (earlier passes' outputs are resident)
+            if budget_bytes is None:
+                fb = C.c_uint64()
+                ctx.check(L.sgpu_dist_free_bytes(h, C.byref(fb)))
+                tb = torch.tensor([fb.value], dtype=torch.int64, device=backend_dev)
+                dist.all_reduce(tb, op=dist.ReduceOp.MIN, group=group)
+                budget = int(int(tb.item()) * 0.90)
+            else:
+                budget = int(budget_bytes)                 # tests: a fixed per-pass budget
+            p = C.c_int()
+            ctx.check(L.sgpu_dist_next_pass(h, budget, C.byref(p)))
+            if p.value < 0:
+                break
+            desc = np.zeros(SGPU_IPC_BYTES, np.uint8)
+            ctx.check(L.sgpu_dist_ipc_handle(h, desc.ctypes.data_as(C.c_void_p)))
+            t_h = torch.from_numpy(desc).to(backend_dev)
+            hs = [torch.empty_like(t_h) for _ in range(world)]
+            dist.all_gather(hs, t_h, group=group)
+            descs = np.ascontiguousarray(torch.stack(hs).cpu().numpy())
+            ctx.check(L.sgpu_dist_open_peers(h, descs.ctypes.data_as(C.c_void_p)))     # peers' arenas are mapped once per process
+            ctx.check(L.sgpu_dist_scatter(h, p.value))    # local partition into the staging buffer
+            dist.barrier(group=group)                     # every rank's staging buffer is complete
+            ctx.check(L.sgpu_dist_exchange(h, p.value))   # one kernel: pull my pieces from all peers over NVLink + merge
+            dist.barrier(group=group)                     # nobody reads my staging buffer any more (it becomes the sort's partner)
+            ctx.check(L.sgpu_dist_sort(h, p.value))
+            npass += 1
+        dist.barrier(group=group)
+        ks = C.c_void_p()
+        ctx.check(L.sgpu_dist_end(h, C.byref(ks)))
+        return KMerDiskStorage(ctx, ks), npass
+    finally:
+        L.sgpu_dist_free(h)
+
+
 class DistributedKMerCounter:
     """KMerDiskCounter over a read set sharded across the ranks of a torch.distributed process group. result_on_host: each rank's
     set goes to its pinned host memory, pass by pass behind the next one."""
@@ -25,60 +87,82 @@ class DistributedKMerCounter:
         pass
 
     def Count(self, num_buckets, budget_bytes=None):
-        import torch
-        import torch.distributed as dist
-        ctx, L = self.ctx, self.ctx.L
-        world, rank = dist.get_world_size(self.group), dist.get_rank(self.group)
-        backend_dev = "cuda" if dist.get_backend(self.group) == "nccl" else "cpu"
-        h = C.c_void_p()
         mode = self.mode | (SGPU_RESULT_ON_HOST if self.result_on_host else 0)
-        ctx.check(L.sgpu_dist_begin(ctx.h, self.K, num_buckets, mode, world, rank, C.byref(h)))
-        try:
-            npart = L.sgpu_dist_num_partitions(h)
-            local = np.zeros(npart, np.uint64)
-            ctx.check(L.sgpu_dist_local_counts(h, local.ctypes.data_as(C.c_void_p)))
-            # all_gather of the per-partition record counts (world x npart x 8 bytes: small)
-            t_local = torch.from_numpy(local.view(np.int64)).to(backend_dev)
-            gathered = [torch.empty_like(t_local) for _ in range(world)]
-            dist.all_gather(gathered, t_local, group=self.group)
-            all_counts = np.ascontiguousarray(torch.stack(gathered).cpu().numpy().view(np.uint64))
-            total = C.c_uint64()
-            ctx.check(L.sgpu_dist_plan(h, all_counts.ctypes.data_as(C.c_void_p), C.byref(total)))
-            npass = 0
-            while True:
-                # every pass is planned against what ALL ranks can allocate right now (earlier passes' outputs are resident)
-                if budget_bytes is None:
-                    fb = C.c_uint64()
-                    ctx.check(L.sgpu_dist_free_bytes(h, C.byref(fb)))
-                    tb = torch.tensor([fb.value], dtype=torch.int64, device=backend_dev)
-                    dist.all_reduce(tb, op=dist.ReduceOp.MIN, group=self.group)
-                    budget = int(int(tb.item()) * 0.90)
-                else:
-                    budget = int(budget_bytes)                 # tests: a fixed per-pass budget
-                p = C.c_int()
-                ctx.check(L.sgpu_dist_next_pass(h, budget, C.byref(p)))
-                if p.value < 0:
-                    break
-                desc = np.zeros(SGPU_IPC_BYTES, np.uint8)
-                ctx.check(L.sgpu_dist_ipc_handle(h, desc.ctypes.data_as(C.c_void_p)))
-                t_h = torch.from_numpy(desc).to(backend_dev)
-                hs = [torch.empty_like(t_h) for _ in range(world)]
-                dist.all_gather(hs, t_h, group=self.group)
-                descs = np.ascontiguousarray(torch.stack(hs).cpu().numpy())
-                ctx.check(L.sgpu_dist_open_peers(h, descs.ctypes.data_as(C.c_void_p)))     # peers' arenas are mapped once per process
-                ctx.check(L.sgpu_dist_scatter(h, p.value))    # local partition into the staging buffer
-                dist.barrier(group=self.group)                # every rank's staging buffer is complete
-                ctx.check(L.sgpu_dist_exchange(h, p.value))   # one kernel: pull my pieces from all peers over NVLink + merge
-                dist.barrier(group=self.group)                # nobody reads my staging buffer any more (it becomes the sort's partner)
-                ctx.check(L.sgpu_dist_sort(h, p.value))
-                npass += 1
-            dist.barrier(group=self.group)
-            ks = C.c_void_p()
-            ctx.check(L.sgpu_dist_end(h, C.byref(ks)))
-            self.npass = npass
-            return KMerDiskStorage(ctx, ks)
-        finally:
-            L.sgpu_dist_free(h)
+        st, self.npass = _distributed_count(self.ctx, self.group, lambda world, rank, out: self.ctx.L.sgpu_dist_begin(
+            self.ctx.h, self.K, num_buckets, mode, world, rank, out), budget_bytes)
+        return st
+
+
+class DistributedKmersFromKpomers:
+    """KMerDiskCounter over a DeBruijnKMerKMerSplitter across the ranks of a torch.distributed process group: every rank brings a
+    (k+1)-mer set (its shard of a DistributedKMerCounter count, or any other; the sets may overlap), and every rank gets the buckets
+    it owns of the k-mers of the union of the sets, as sgpu_kmers_from_kpomers_ex gives them on one GPU. The source may live in HBM
+    or in host memory; result_on_host: this rank's k-mers go to its pinned host memory, pass by pass behind the next one."""
+
+    def __init__(self, ctx, kpomer_storage, group=None, result_on_host=False):
+        self.ctx, self.kpomers, self.group, self.result_on_host = ctx, kpomer_storage, group, result_on_host
+        self.npass = 0
+
+    def close(self):
+        pass
+
+    def Count(self, num_buckets, budget_bytes=None):
+        import torch.distributed as dist
+        if not self.kpomers.h:
+            raise ValueError("the (k+1)-mer set has been freed")
+        # the ranks' level-A geometries and bucket functions only agree for one B and one k
+        shape = (self.kpomers.k(), int(num_buckets))
+        shapes = [None] * dist.get_world_size(self.group)
+        dist.all_gather_object(shapes, shape, group=self.group)
+        if any(tuple(x) != shape for x in shapes):
+            raise ValueError("the ranks' (k+1, num_buckets) differ: %s" % (shapes,))
+        mode = SGPU_RESULT_ON_HOST if self.result_on_host else 0
+        st, self.npass = _distributed_count(self.ctx, self.group, lambda world, rank, out: self.ctx.L.sgpu_dist_begin_kpomers(
+            self.ctx.h, self.kpomers.h, num_buckets, mode, world, rank, out), budget_bytes)
+        return st
+
+
+def assemble_kmer_index(ctx, storage, mphf, group=None):
+    """KMerIndex::serialize of the union of the ranks' bucket-owned k-mer sets, from each rank's set (`storage`, from a distributed
+    count) and its index (`mphf`, KMerIndexBuilder.BuildIndex of it). A bucket's bytes depend on its own keys only, so each owner
+    sends the serialized bytes of the buckets it owns; rank 0 writes num_segments, every bucket's bytes in bucket order and the
+    segment_starts of the union's bucket sizes. Returns the bytes on rank 0, None elsewhere."""
+    import torch
+    import torch.distributed as dist
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    backend_dev = _backend_device(group)
+    B = storage.num_buckets()
+    mine = torch.from_numpy(np.concatenate([storage.bucket_sizes(), storage.owned_buckets().astype(np.int64)])).to(backend_dev)
+    allv = [torch.empty_like(mine) for _ in range(world)]
+    dist.all_gather(allv, mine, group=group)
+    allv = torch.stack(allv).cpu().numpy()
+    bsz_all, owned_all = allv[:, :B], allv[:, B:].astype(bool)
+    if not (owned_all.sum(axis=0) == 1).all():
+        raise ValueError("every bucket must be owned by exactly one rank (sets from one distributed count)")
+    if (bsz_all[~owned_all] != 0).any():
+        raise ValueError("a rank holds records of a bucket it does not own")
+    own = owned_all[rank]
+    runs, b = [], 0
+    while b < B:                     # the serialized bytes of every maximal run of owned buckets
+        if own[b]:
+            e = b
+            while e < B and own[e]:
+                e += 1
+            runs.append((b, mphf.serialize_buckets(b, e)))
+            b = e
+        else:
+            b += 1
+    pieces = [None] * world if rank == 0 else None
+    dist.gather_object(runs, pieces, dst=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
+    if rank != 0:
+        return None
+    # segment_starts as the single-GPU index computes them (mphf.cu): the running sum stops before the last entry
+    bsz = bsz_all.sum(axis=0).astype(np.uint64)
+    starts = np.zeros(B + 1, np.uint64)
+    starts[1:B] = np.cumsum(bsz[:B - 1])
+    starts[B] = bsz[B - 1]
+    body = [blob for _, blob in sorted((r for rr in pieces for r in rr), key=lambda r: r[0])]
+    return np.uint64(B).tobytes() + b"".join(body) + starts.tobytes()
 
 
 def distributed_cov_filter(ctx, k_plus_one, threshold, group=None, apply=True, phase_done=None):
@@ -92,7 +176,7 @@ def distributed_cov_filter(ctx, k_plus_one, threshold, group=None, apply=True, p
     import torch.distributed as dist
     L = ctx.L
     world, rank = dist.get_world_size(group), dist.get_rank(group)
-    backend_dev = "cuda" if dist.get_backend(group) == "nccl" else "cpu"
+    backend_dev = _backend_device(group)
     n, nw = C.c_int64(), C.c_uint64()
     ctx.check(L.sgpu_reads_info(ctx.h, C.byref(n), C.byref(nw)))
     keep = np.zeros(max(n.value, 1), np.uint8)

@@ -127,6 +127,16 @@ class KMerDiskStorage:
     def write_buckets(self, prefix):
         self.ctx.check(self.ctx.L.sgpu_kset_write_buckets(self.h, str(prefix).encode()))
 
+    def owned_buckets(self):
+        """bool [B]: the buckets this set holds (all of them, or this rank's share of a distributed count)"""
+        out = np.zeros(self._B, np.uint8)
+        self.ctx.check(self.ctx.L.sgpu_kset_owned_buckets(self.h, _p(out)))
+        return out.astype(bool)
+
+    def write_owned_buckets(self, prefix):
+        """prefix.<b> for the owned buckets only: the ranks of a distributed count writing into one directory leave every bucket file once"""
+        self.ctx.check(self.ctx.L.sgpu_kset_write_owned_buckets(self.h, str(prefix).encode()))
+
     def merge(self, path):
         """KMerDiskStorage::merge -> final_kmers file."""
         self.ctx.check(self.ctx.L.sgpu_kset_write_final(self.h, str(path).encode()))
@@ -202,6 +212,15 @@ class KMerIndex:
 
     def serialized_size(self) -> int:
         return int(self.ctx.L.sgpu_mphf_serialized_size(self.h))
+
+    def serialize_buckets(self, b_lo, b_hi) -> bytes:
+        """the serialized buckets [b_lo, b_hi) alone, as they appear inside serialize()"""
+        n = self.ctx.L.sgpu_mphf_serialized_size_buckets(self.h, b_lo, b_hi)
+        if n < 0:
+            raise ValueError("bucket range [%d, %d) outside the index" % (b_lo, b_hi))
+        buf = np.zeros(max(n, 1), np.uint8)
+        self.ctx.check(self.ctx.L.sgpu_mphf_serialize_buckets(self.h, b_lo, b_hi, _p(buf), n))
+        return buf[:n].tobytes()
 
     def serialize_into(self, host_ptr, cap):
         """KMerIndex::serialize bytes written to caller memory (e.g. a pinned buffer); returns the size."""
