@@ -11,8 +11,10 @@
 //   3. values : EdgeInfoUpdater::UpdateKMers puts (EdgeId, offset) for every window of every edge -- conjugate edges included -- that
 //               is minimal as it stands (edge_info_updater.hpp:41-47); a K-mer that is put twice ends as a TOMBSTONE (PutInIndex,
 //               edge_position_index.hpp:152-167) -- order independent: one put -> its position, more -> removed (a self-reverse-
-//               complementary K-mer is minimal on both strands, so it is always removed). Edge ids as FastGraphFromSequencesConstructor hands them out: edge i -> 3 + 2i, conjugate +1, a self-conjugate
-//               edge has one id and is visited once (graph_core.hpp:233,514-531).
+//               complementary K-mer is minimal on both strands: on an ordinary edge it is put from the edge and its conjugate and
+//               removed; at the centre of a self-conjugate edge, visited once, it is put once and keeps its position -- with K = k+1
+//               every self-conjugate edge has one). Edge ids as FastGraphFromSequencesConstructor hands them out: edge i -> 3 + 2i,
+//               conjugate +1, a self-conjugate edge has one id and is visited once (graph_core.hpp:233,514-531).
 #include <algorithm>
 #include <thread>
 #include <vector>

@@ -72,6 +72,32 @@ def at_reads(n, L, glen, err, seed):
     return out + ["A" * L] * 5 + ["AT" * (L // 2)] * 3
 
 
+def _random_seq(rng, n):
+    return "".join("ACGT"[i] for i in rng.integers(0, 4, n))
+
+
+def pal_reads(half, n_pal, n_hairpin, seed, base=()):
+    """`base` plus palindromes x + rc(x) (|x| = half) planted in random context, and reads along hairpins y + rc(y) (|y| = 120).
+    A planted palindrome is a self-reverse-complementary window of length 2 * half on an ordinary edge; a hairpin becomes a
+    self-conjugate edge, whose centre (k+1)-mer is its own reverse complement."""
+    rng = np.random.default_rng(seed)
+    reads = list(base)
+    for _ in range(n_pal):
+        x = _random_seq(rng, half)
+        reads.append(_random_seq(rng, 60) + x + revcomp(x) + _random_seq(rng, 60))
+    for _ in range(n_hairpin):
+        y = _random_seq(rng, 120)
+        h = y + revcomp(y)
+        reads += [h[i:i + 150] for i in range(0, len(h) - 150 + 1, 15)]
+    return reads
+
+
+def isolated_reads(n, seed):
+    """n random 70-bp reads: n isolated edges, 4 n vertices counting conjugates"""
+    rng = np.random.default_rng(seed)
+    return [_random_seq(rng, 70) for _ in range(n)]
+
+
 def run_probe(mode, reads, k, B, T=2, early_tc=0, early_at=False, edge_index=None):
     with tempfile.TemporaryDirectory() as d:
         rf = os.path.join(d, "reads.txt")
@@ -205,6 +231,19 @@ if __name__ == "__main__":
     save("syn_k21_B20_K15_eigraph", "eigraph", synthetic_reads(600, 100, 1500, 0.01, seed=5), 21, 20, edge_index=15)
     save("loops_k21_B10_eigraph", "eigraph", loops_reads(), 21, 10, edge_index=0)
     save("ecoli_k55_B20_K33_eigraph", "eigraph", ec[:1200], 55, 20, edge_index=33)
+    # every key width (K = 97: four words, K = 66: three), K = 128 through the (k+1)-mer path, K = 1 and 2 (every slot put many times)
+    save("syn_k99_B20_K97_eigraph", "eigraph", synthetic_reads(250, 150, 1500, 0.01, seed=5), 99, 20, edge_index=97)
+    save("syn_k127_B20_eigraph", "eigraph", synthetic_reads(400, 150, 1200, 0.005, seed=9), 127, 20, edge_index=0)
+    save("syn_k21_B20_K1_eigraph", "eigraph", synthetic_reads(100, 100, 1000, 0.01, seed=10), 21, 20, edge_index=1)
+    save("syn_k21_B20_K2_eigraph", "eigraph", synthetic_reads(100, 100, 1000, 0.01, seed=10), 21, 20, edge_index=2)
+    # self-reverse-complementary K-mers: on ordinary edges (put from both strands: tombstones) and at the centre of self-conjugate
+    # edges (visited once: a position)
+    save("pal_k77_B20_K66_eigraph", "eigraph", pal_reads(33, 20, 10, 12, synthetic_reads(100, 150, 1500, 0.01, seed=11)), 77, 20, edge_index=66)
+    save("pal_k21_B20_eigraph", "eigraph", pal_reads(11, 20, 30, 13), 21, 20, edge_index=0)
+    # the (k+1)-mer path's branch rule: 16 vertices against 20 chunks (one segment, segment_starts_[1] = n), 20 (single index, 0)
+    save("iso4_k21_B20_eigraph", "eigraph", isolated_reads(4, 14), 21, 20, edge_index=0)
+    save("iso5_k21_B20_eigraph", "eigraph", isolated_reads(5, 15), 21, 20, edge_index=0)
+    save("empty_k21_B20_eigraph", "eigraph", ["ACGTACGTAC", "GGGTTTAAACCC"], 21, 20, edge_index=0)
     for nm, (rd, _) in GTEST_CASES.items():
         save("gtest_" + nm + "_k5", "graph", rd, 5, 2)
     # construction_test.cpp:97-105 (SimpleTestEarlyPairedInfo, k=3): its coverage table is the known answer in tests/test_oracle_golden.py

@@ -139,6 +139,27 @@ def check_edge_index(g, ei_bytes, ids, offs, nbuckets):
     return bad
 
 
+def edge_index_single(unitigs, k, chunks):
+    """the (k+1)-mer path's branch: with more than one vertex chunk and at least as many vertices as chunks KMerIndexBuilder takes its
+    single-index branch, which never fills segment_starts_[1] (kmer_index_builder.hpp:481-493); with fewer vertices the graph is one
+    chunk and the segmented branch stores n there. Vertices = the distinct canonical ends of the edges, each with its conjugate."""
+    from spades_b200.packing import revcomp
+    ends = set()
+    for s in unitigs:
+        for v in (s[:k], s[-k:]):
+            ends.add(min(v, revcomp(v)))
+    return chunks > 1 and 2 * len(ends) >= chunks
+
+
+def edge_index_bytes(mphf, unitigs, k, K, chunks):
+    """the oracle MPHF's KMerIndex::serialize as the EdgeIndex refill writes it: K = k+1 over `chunks` vertex chunks leaves
+    segment_starts_[1] = 0 in the single-index branch (edge_index_single); the oracle's one segment stores n there"""
+    ser = mphf.serialize()
+    if K == k + 1 and edge_index_single(unitigs, k, chunks):
+        ser = ser[:-8] + b"\0" * 8
+    return ser
+
+
 def check_count(g, art):
     bad = []
     if not np.array_equal(np.frombuffer(g["final_kmers"].tobytes(), np.uint64), np.asarray(art["final_kmers"], np.uint64).ravel()):

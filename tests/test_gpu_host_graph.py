@@ -178,7 +178,7 @@ def test_empty_host_sets():
     assert art["unitigs"] == [] and len(art["masks"]) == 0
 
 
-@pytest.mark.parametrize("k,B,K", [(33, 6, 25), (21, 6, None)])
+@pytest.mark.parametrize("k,B,K", [(33, 6, 25), (21, 6, None), (99, 6, 97)])
 def test_edge_index_over_a_graph_from_host_sets(k, B, K):
     from spades_b200.graph import EdgeIndex
     reads = synthetic_reads(1000, 150, 1500, 0.01, seed=80 + k)
@@ -197,9 +197,7 @@ def test_edge_index_over_a_graph_from_host_sets(k, B, K):
         art, cnt, _, _, _, (ids, offs, ser, slots) = _host_path(c, reads, k, B, then=refill)
     _check_counters(cnt, k, True, True)
     assert _compare(art, want, B) == []
-    want_ser = m.serialize()
-    if K is None:
-        want_ser = want_ser[:-8] + b"\0" * 8
+    want_ser = G.edge_index_bytes(m, want["unitigs"], k, K or k + 1, B)
     assert np.array_equal(ids, want_ids) and np.array_equal(offs, want_offs)
     assert G.index_equal(want_ser, ser, 1 if K is None else B)
     assert np.array_equal(slots, np.array([m.lookup(key) for key in ks.keys], np.uint64))

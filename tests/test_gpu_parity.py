@@ -102,26 +102,74 @@ def test_edge_index_refill_matches_reference_golden(name):
     ei.free(); gr.free()
 
 
-def test_edge_index_refill_matches_oracle_random():
+def _edge_index_reads(kind, k, K, seed):
+    import os, sys
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
+    from make_golden import isolated_reads, pal_reads
+    if kind == "syn":
+        return synthetic_reads(800, 150, 1500, 0.01, seed=seed)
+    if kind == "pal":              # palindromes of length K (self-RC windows) and hairpins (self-conjugate edges)
+        return pal_reads((K or k + 1) // 2, 20, 10, seed, synthetic_reads(300, 150, 1500, 0.01, seed=seed))
+    if kind == "small":            # a few hundred edges: the oracle's loop puts every window of K = 1 or 2
+        return synthetic_reads(150, 100, 1500, 0.01, seed=seed)
+    if kind == "big":              # > 4096 edges: the unitigs are packed on several host threads
+        return synthetic_reads(3000, 150, 4000, 0.02, seed=seed)
+    if kind.startswith("iso"):
+        return isolated_reads(int(kind[3:]), seed)
+    assert kind == "empty"
+    return ["ACGTACGTAC", "GGGTTTAAACCC"]
+
+
+def _check_edge_index_refill(k, B, K, kind, seed):
+    """sgpu_edge_index_build against the oracle's refill: ids, offsets, the serialized index (with the branch the (k+1)-mer path
+    takes for B vertex chunks) and a lookup of every key"""
     from gpu_util import ctx
     from spades_b200.graph import DeBruijnGraphConstructor, EdgeIndex
-    from spades_b200.packing import pack_reads
     c = ctx()
+    c.set_reads(*pack_reads(_edge_index_reads(kind, k, K, seed)))
+    gr = DeBruijnGraphConstructor(c, k, B).ConstructGraph()
+    u = gr.unitigs()
+    ei = EdgeIndex(gr, K, B)
+    ids, offs = ei.values()
+    ks, m, want_ids, want_offs = O.edge_index(u, k, K, 1 if K is None else B)
+    # each case holds what it is there for
+    if kind == "pal":              # self-conjugate edges; self-RC windows on ordinary edges for K < k+1 (at K = k+1 there are none)
+        Kw = K or k + 1
+        on_ordinary = [s[j:j + Kw] for s in u if s != revcomp(s) for j in range(len(s) - Kw + 1) if s[j:j + Kw] == revcomp(s[j:j + Kw])]
+        assert any(s == revcomp(s) for s in u) and bool(on_ordinary) == (K is not None)
+    if kind == "big":
+        assert len(u) >= 4096
+    if kind.startswith("iso"):
+        assert G.edge_index_single(u, k, B) == (kind == "iso5")
+    if kind == "empty":
+        assert u == [] and ks.n == 0
+    assert ei.size() == ks.n and np.array_equal(ids, want_ids) and np.array_equal(offs, want_offs)
+    assert G.index_equal(G.edge_index_bytes(m, u, k, K or k + 1, B), ei.serialize(), 1 if K is None else B)
+    slots = ei.seq_idx(ks.keys)
+    assert np.array_equal(slots, np.array([m.lookup(key) for key in ks.keys], np.uint64))
+    assert np.array_equal(np.sort(slots), np.arange(ks.n, dtype=np.uint64))
+    # the reads' set is untouched by the refill: counting again gives the same (k+1)-mers
+    assert np.array_equal(DeBruijnGraphConstructor(c, k, B).ConstructGraph().kpomers.kmers(), gr.kpomers.kmers())
+    ei.free(); gr.free()
+
+
+def test_edge_index_refill_matches_oracle_random():
     for k, B, K, seed in ((21, 6, None, 71), (33, 4, 25, 72), (55, 12, None, 73), (77, 3, 41, 74)):
-        reads = synthetic_reads(800, 150, 1500, 0.01, seed=seed)
-        c.set_reads(*pack_reads(reads))
-        gr = DeBruijnGraphConstructor(c, k, B).ConstructGraph()
-        ei = EdgeIndex(gr, K, B)
-        ids, offs = ei.values()
-        ks, m, want_ids, want_offs = O.edge_index(gr.unitigs(), k, K, 1 if K is None else B)
-        ser = m.serialize()
-        if K is None:                      # B vertex chunks (> 1, fewer than the vertices): the single-index branch leaves segment_starts_[1] = 0
-            ser = ser[:-8] + b"\0" * 8
-        assert ei.size() == ks.n and np.array_equal(ids, want_ids) and np.array_equal(offs, want_offs)
-        assert G.index_equal(ser, ei.serialize(), 1 if K is None else B)
-        # the reads' set is untouched by the refill: counting again gives the same (k+1)-mers
-        assert np.array_equal(DeBruijnGraphConstructor(c, k, B).ConstructGraph().kpomers.kmers(), gr.kpomers.kmers())
-        ei.free(); gr.free()
+        _check_edge_index_refill(k, B, K, "syn", seed)
+
+
+@pytest.mark.parametrize("k,B,K,kind,seed", [
+    (33, 4, 31, "syn", 75), (33, 4, 32, "syn", 76), (41, 5, 33, "syn", 77),              # one key word | two
+    (77, 6, 63, "syn", 78), (63, 6, None, "syn", 79), (99, 7, 65, "syn", 80),            # two | three
+    (99, 5, 96, "syn", 81), (99, 6, 97, "syn", 82), (127, 6, None, "syn", 83),           # three | four, K = 128
+    (55, 6, 40, "pal", 84), (21, 6, None, "pal", 85),
+    (21, 6, 1, "small", 86), (21, 6, 2, "small", 87),
+    (21, 20, None, "iso4", 14), (21, 20, None, "iso5", 15), (21, 6, None, "empty", 0), (21, 6, 15, "empty", 0),
+    (21, 16, None, "big", 1), (21, 16, 15, "big", 1)])
+def test_edge_index_refill_matches_oracle_cases(k, B, K, kind, seed):
+    """both sides of every key-word boundary, K = 1 and 2, self-RC windows and self-conjugate edges, both sides of the single-index
+    branch, the empty graph, and a graph whose unitigs are packed on several host threads"""
+    _check_edge_index_refill(k, B, K, kind, seed)
 
 
 @pytest.mark.parametrize("k,B,n,L,glen,err,seed", [(21, 16, 3000, 100, 4000, 0.02, 51), (55, 20, 3000, 150, 4000, 0.02, 52), (77, 3, 1500, 150, 2000, 0.01, 53),

@@ -64,15 +64,7 @@ def test_oracle_edge_index_matches_reference_golden(name):
     K = int(g["ei_k"][0])
     B = 1 if K == g["k"] + 1 else g["B"]
     ks, m, ids, offs = O.edge_index(r["unitigs"].seqs, g["k"], K, B)
-    ser = m.serialize()
-    # (k+1)-mer path: with more than one vertex chunk KMerIndexBuilder takes its single-index branch, which never fills segment_starts_[1]
-    # (kmer_index_builder.hpp:481-493); vertices = both ends of every edge, each with its conjugate
-    ends = set()
-    for s in r["unitigs"].seqs:
-        for v in (s[:g["k"]], s[-g["k"]:]):
-            ends.add(min(v, revcomp(v)))
-    if K == g["k"] + 1 and (2 * len(ends)) // int(g["ei_chunks"][0]) > 0:
-        ser = ser[:-8] + b"\0" * 8
+    ser = G.edge_index_bytes(m, r["unitigs"].seqs, g["k"], K, int(g["ei_chunks"][0]))
     assert G.check_edge_index(g, ser, ids, offs, B) == []
 
 
