@@ -59,6 +59,16 @@ __device__ __forceinline__ bool window_self_rc(const uint64_t *seq, int j, int K
         if (base_at(seq, j + i) != 3 - base_at(seq, j + K - 1 - i)) return false;
     return true;
 }
+// f(j, h) for every window j of a read of L >= K bases, h its hash
+template <class F>
+__device__ __forceinline__ void for_each_window(const uint64_t *seq, int L, int K, F &&f) {
+    CycHash h = cyc_init(seq, K);
+    for (int j = 0;; ++j) {
+        f(j, h);
+        if (j + K >= L) break;
+        cyc_roll(h, base_at(seq, j), base_at(seq, j + K), K);
+    }
+}
 
 // ---- pass 1: HyperLogLog registers (hll.hpp:34-41) --------------------------------------------------------------------------
 __global__ void cov_hll_k(const uint64_t *__restrict__ words, const uint64_t *__restrict__ offs, const uint32_t *__restrict__ lens, int64_t n, int K,
@@ -67,42 +77,49 @@ __global__ void cov_hll_k(const uint64_t *__restrict__ words, const uint64_t *__
     if (r >= n) return;
     const int L = (int)lens[r];
     if (L < K) return;
-    const uint64_t *seq = words + offs[r];
-    CycHash h = cyc_init(seq, K);
-    for (int j = 0;; ++j) {
+    for_each_window(words + offs[r], L, K, [&](int, const CycHash &h) {
         const uint64_t d = h.value();
         const uint32_t id = (uint32_t)(d >> 40);
         const uint64_t low = d & ((1ull << 40) - 1);
-        const uint32_t rho = (uint32_t)((low == 0 ? 64 : __clzll((long long)low)) - 24 + 1);
+        const uint32_t rho = (uint32_t)(__clzll((long long)low) - 24 + 1);     // __clzll(0) = 64
         if (reg[id] < rho) atomicMax(&reg[id], rho);
-        if (j + K >= L) break;
-        cyc_roll(h, base_at(seq, j), base_at(seq, j + K), K);
-    }
+    });
 }
 
 // ---- the (key -> count) table --------------------------------------------------------------------------------------------------
 // entry = (key + 1) << 16 | count; 0 = empty. key < 2^47.
+template <bool SYSTEM>
+__device__ __forceinline__ unsigned long long cov_cas(unsigned long long *a, unsigned long long cmp, unsigned long long val) {
+    if constexpr (SYSTEM) return atomicCAS_system(a, cmp, val);
+    else return atomicCAS(a, cmp, val);
+}
 struct CovTable {
     unsigned long long *e;
     uint64_t cap;
     uint64_t key_mask;
     unsigned *overflow;         // set when a probe sequence visited every slot (cannot happen while the HLL bound holds; checked on the host)
     __device__ __forceinline__ uint64_t slot_of(uint64_t key) const { return __umul64hi(key * 0x9E3779B97F4A7C15ULL, cap); }
-    // CQFProcessor::ProcessKmer: nothing once the count has reached the threshold
+    // CQFProcessor::ProcessKmer: nothing once the count has reached the threshold. SYSTEM: ranks on other GPUs insert into the same
+    // table at the same time.
+    template <bool SYSTEM>
     __device__ __forceinline__ void add(uint64_t key, unsigned thr) const {
         const unsigned long long tag = (key + 1) << 16;
         uint64_t s = slot_of(key);
         for (uint64_t probes = 0;; ++probes) {
-            if (probes > cap) { *overflow = 1u; return; }
+            if (probes > cap) {
+                if constexpr (SYSTEM) atomicExch_system(overflow, 1u);
+                else *overflow = 1u;
+                return;
+            }
             unsigned long long cur = e[s];
             if (cur == 0) {
-                const unsigned long long old = atomicCAS(&e[s], 0ull, tag | 1ull);
+                const unsigned long long old = cov_cas<SYSTEM>(&e[s], 0ull, tag | 1ull);
                 if (old == 0) return;
                 cur = old;
             }
             if ((cur & ~0xffffull) == tag) {
                 while ((cur & 0xffffull) < thr) {
-                    const unsigned long long old = atomicCAS(&e[s], cur, cur + 1);
+                    const unsigned long long old = cov_cas<SYSTEM>(&e[s], cur, cur + 1);
                     if (old == cur) return;
                     cur = old;
                 }
@@ -124,43 +141,105 @@ struct CovTable {
     }
 };
 
+// ---- which table a key's count lives in ----------------------------------------------------------------------------------------
+// The owner of a key among `world` tables is the high word of a second multiplicative hash of the masked key scaled by `world`, so it
+// does not depend on the slot function inside a table (which takes the high word of key * 0x9E37...).
+__host__ __device__ __forceinline__ uint32_t cov_owner(uint64_t key, uint32_t world) {
+    const uint64_t h = key * 0xC2B2AE3D27D4EB4FULL;
+#ifdef __CUDA_ARCH__
+    return (uint32_t)__umul64hi(h, world);
+#else
+    return (uint32_t)(((unsigned __int128)h * world) >> 64);
+#endif
+}
+
+// A route gives the key of a window, whether this launch owns the key, the table its count lives in, the scope of the table's atomics
+// and whether a read's verdict is split over several launches (`split`: the windows below the threshold are carried in below[r]).
+
+// one table for every key
+struct WholeTable {
+    CovTable t;
+    static constexpr bool system = false, split = false;
+    __device__ __forceinline__ uint64_t key(const CycHash &h) const { return h.value() & t.key_mask; }
+    __device__ __forceinline__ bool owns(uint64_t) const { return true; }
+    __device__ __forceinline__ const CovTable &table(uint64_t) const { return t; }
+};
+
+// Key-range passes: a table too large for the device is built and read in P passes over the resident reads. Pass p holds the keys with
+// cov_owner(key, P) == p in a table of cov_slice_capacity(bound, P) entries. Every key lands in exactly one pass with all of its
+// windows, so its count, each read's number of windows below the threshold and the distinct keys summed over the passes are those of
+// the single table. The pass hash composes with the rank owner: floor(h*W*P / 2^64) / P == floor(h*W / 2^64), so
+// cov_owner(key, W*P) / P == cov_owner(key, W) and a distributed filter with passes can take id = cov_owner(key, W*P), owner = id / P,
+// pass = id % P without changing which rank owns a key.
+struct KeyRange {
+    CovTable t;
+    uint32_t passes, pass;
+    static constexpr bool system = false, split = true;
+    __device__ __forceinline__ uint64_t key(const CycHash &h) const { return h.value() & t.key_mask; }
+    __device__ __forceinline__ bool owns(uint64_t key) const { return cov_owner(key, passes) == pass; }
+    __device__ __forceinline__ const CovTable &table(uint64_t) const { return t; }
+    __device__ __forceinline__ bool last() const { return pass + 1 == passes; }
+};
+
+// The distributed filter: the table is split into one slice per rank, a key lives in its owner's slice. Ranks on other GPUs insert
+// into the same slices at the same time (system scope).
+struct OwnerSlices {
+    const CovTable *slices;
+    uint32_t world;
+    uint64_t key_mask;
+    static constexpr bool system = true, split = false;
+    __device__ __forceinline__ uint64_t key(const CycHash &h) const { return h.value() & key_mask; }
+    __device__ __forceinline__ bool owns(uint64_t) const { return true; }
+    // by value: the compiler cannot tell that `slices` is not written by the CAS of an insert, so a reference would be read again
+    // after every CAS (__restrict__ on a member does not change that)
+    __device__ __forceinline__ CovTable table(uint64_t key) const { return slices[cov_owner(key, world)]; }
+};
+
 // ---- pass 2: counts up to the threshold ------------------------------------------------------------------------------------------
+template <class Route>
 __global__ void cov_fill_k(const uint64_t *__restrict__ words, const uint64_t *__restrict__ offs, const uint32_t *__restrict__ lens, int64_t n, int K,
-                           CovTable t, unsigned thr) {
+                           const Route route, unsigned thr) {
     const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n) return;
     const int L = (int)lens[r];
     if (L < K) return;
     const uint64_t *seq = words + offs[r];
-    CycHash h = cyc_init(seq, K);
-    for (int j = 0;; ++j) {
-        const uint64_t key = h.value() & t.key_mask;
-        t.add(key, thr);
-        if ((K & 1) == 0 && h.fwd == h.rvs && window_self_rc(seq, j, K)) t.add(key, thr);
-        if (j + K >= L) break;
-        cyc_roll(h, base_at(seq, j), base_at(seq, j + K), K);
-    }
+    for_each_window(seq, L, K, [&](int j, const CycHash &h) {
+        const uint64_t key = route.key(h);
+        if (!route.owns(key)) return;
+        const CovTable &t = route.table(key);
+        t.add<Route::system>(key, thr);
+        if ((K & 1) == 0 && h.fwd == h.rvs && window_self_rc(seq, j, K)) t.add<Route::system>(key, thr);
+    });
 }
 
 // ---- pass 3: the verdict per read (coverage_filtering_read_wrapper.hpp:37-72) --------------------------------------------------------
+// A split route adds the read's windows of this launch below the threshold to below[r] (one thread per read, no atomics); its last
+// pass gives the verdict from the sum. Other routes do not touch below.
+template <class Route>
 __global__ void cov_filter_k(const uint64_t *__restrict__ words, const uint64_t *__restrict__ offs, const uint32_t *__restrict__ lens, int64_t n, int K,
-                             CovTable t, unsigned thr, uint8_t *__restrict__ keep, uint32_t *__restrict__ keep_words) {
+                             const Route route, unsigned thr, uint32_t *__restrict__ below, uint8_t *__restrict__ keep,
+                             uint32_t *__restrict__ keep_words) {
     const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n) return;
     const int L = (int)lens[r];
-    bool k = false;
+    bool k;
     if (L < K) {
         k = thr == 0;                                          // CountMedianMlt returns 0 for a read shorter than K
     } else {
-        const uint64_t *seq = words + offs[r];
-        CycHash h = cyc_init(seq, K);
-        uint32_t below = 0;
-        for (int j = 0;; ++j) {
-            below += t.count(h.value() & t.key_mask) < thr;
-            if (j + K >= L) break;
-            cyc_roll(h, base_at(seq, j), base_at(seq, j + K), K);
+        uint32_t b = 0;
+        for_each_window(words + offs[r], L, K, [&](int, const CycHash &h) {
+            const uint64_t key = route.key(h);
+            if (route.owns(key)) b += route.table(key).count(key) < thr;
+        });
+        if constexpr (Route::split) {
+            if (route.pass) b += below[r];
+            if (!route.last()) { below[r] = b; return; }
         }
-        k = below <= (uint32_t)(L - K + 1) / 2;                // element size/2 of the sorted multiplicities >= threshold
+        k = b <= (uint32_t)(L - K + 1) / 2;                    // element size/2 of the sorted multiplicities >= threshold
+    }
+    if constexpr (Route::split) {
+        if (!route.last()) return;
     }
     keep[r] = k ? 1 : 0;
     keep_words[r] = k ? (uint32_t)((L + 31) >> 5) : 0u;
@@ -191,18 +270,6 @@ __global__ void cov_distinct_k(const unsigned long long *__restrict__ e, uint64_
     if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, (unsigned long long)c);
 }
 
-// ---- the distributed filter: the table is split into one slice per rank, a key lives in its owner's slice ----------------------------
-// The owner is the high word of a second multiplicative hash of the masked key scaled by the world size, so it does not depend on
-// the slot function inside a slice (which takes the high word of key * 0x9E37...).
-__host__ __device__ __forceinline__ uint32_t cov_owner(uint64_t key, uint32_t world) {
-    const uint64_t h = key * 0xC2B2AE3D27D4EB4FULL;
-#ifdef __CUDA_ARCH__
-    return (uint32_t)__umul64hi(h, world);
-#else
-    return (uint32_t)(((unsigned __int128)h * world) >> 64);
-#endif
-}
-
 // HLL registers of the union = element-wise max of the ranks' registers (read through the peers' mapped arenas)
 __global__ void cov_hll_merge_k(const uint4 *const *__restrict__ regs, int world, uint4 *__restrict__ out, uint32_t n4) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -213,130 +280,6 @@ __global__ void cov_hll_merge_k(const uint4 *const *__restrict__ regs, int world
         m.x = max(m.x, r.x); m.y = max(m.y, r.y); m.z = max(m.z, r.z); m.w = max(m.w, r.w);
     }
     out[i] = m;
-}
-
-// CovTable::add with system-scope CAS: ranks on other GPUs insert into the same slice at the same time
-__device__ __forceinline__ void cov_add_system(const CovTable &t, uint64_t key, unsigned thr) {
-    const unsigned long long tag = (key + 1) << 16;
-    uint64_t s = t.slot_of(key);
-    for (uint64_t probes = 0;; ++probes) {
-        if (probes > t.cap) { atomicExch_system(t.overflow, 1u); return; }
-        unsigned long long cur = t.e[s];
-        if (cur == 0) {
-            const unsigned long long old = atomicCAS_system(&t.e[s], 0ull, tag | 1ull);
-            if (old == 0) return;
-            cur = old;
-        }
-        if ((cur & ~0xffffull) == tag) {
-            while ((cur & 0xffffull) < thr) {
-                const unsigned long long old = atomicCAS_system(&t.e[s], cur, cur + 1);
-                if (old == cur) return;
-                cur = old;
-            }
-            return;
-        }
-        if (++s == t.cap) s = 0;
-    }
-}
-
-// pass 2 over this rank's reads: every window's key goes to its owner's slice
-__global__ void cov_fill_dist_k(const uint64_t *__restrict__ words, const uint64_t *__restrict__ offs, const uint32_t *__restrict__ lens, int64_t n,
-                                int K, const CovTable *__restrict__ slices, uint32_t world, uint64_t key_mask, unsigned thr) {
-    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= n) return;
-    const int L = (int)lens[r];
-    if (L < K) return;
-    const uint64_t *seq = words + offs[r];
-    CycHash h = cyc_init(seq, K);
-    for (int j = 0;; ++j) {
-        const uint64_t key = h.value() & key_mask;
-        const CovTable &t = slices[cov_owner(key, world)];
-        cov_add_system(t, key, thr);
-        if ((K & 1) == 0 && h.fwd == h.rvs && window_self_rc(seq, j, K)) cov_add_system(t, key, thr);
-        if (j + K >= L) break;
-        cyc_roll(h, base_at(seq, j), base_at(seq, j + K), K);
-    }
-}
-
-// pass 3 over this rank's reads: the same verdict as cov_filter_k, each window's count read from its owner's slice
-__global__ void cov_filter_dist_k(const uint64_t *__restrict__ words, const uint64_t *__restrict__ offs, const uint32_t *__restrict__ lens, int64_t n,
-                                  int K, const CovTable *__restrict__ slices, uint32_t world, uint64_t key_mask, unsigned thr,
-                                  uint8_t *__restrict__ keep, uint32_t *__restrict__ keep_words) {
-    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= n) return;
-    const int L = (int)lens[r];
-    bool k = false;
-    if (L < K) {
-        k = thr == 0;
-    } else {
-        const uint64_t *seq = words + offs[r];
-        CycHash h = cyc_init(seq, K);
-        uint32_t below = 0;
-        for (int j = 0;; ++j) {
-            const uint64_t key = h.value() & key_mask;
-            below += slices[cov_owner(key, world)].count(key) < thr;
-            if (j + K >= L) break;
-            cyc_roll(h, base_at(seq, j), base_at(seq, j + K), K);
-        }
-        k = below <= (uint32_t)(L - K + 1) / 2;
-    }
-    keep[r] = k ? 1 : 0;
-    keep_words[r] = k ? (uint32_t)((L + 31) >> 5) : 0u;
-}
-
-// ---- key-range passes: a table too large for the device is built and read in P passes over the resident reads ----------------------
-// Pass p holds the keys with cov_owner(key, P) == p in a table of cov_slice_capacity(bound, P) entries. Every key lands in exactly one
-// pass with all of its windows, so its count, each read's number of windows below the threshold and the distinct keys summed over the
-// passes are those of the single table. The pass hash composes with the rank owner: floor(h*W*P / 2^64) / P == floor(h*W / 2^64), so
-// cov_owner(key, W*P) / P == cov_owner(key, W) and a distributed filter with passes can take id = cov_owner(key, W*P), owner = id / P,
-// pass = id % P without changing which rank owns a key.
-
-// cov_fill_k restricted to the keys of pass `pass`
-__global__ void cov_fill_pass_k(const uint64_t *__restrict__ words, const uint64_t *__restrict__ offs, const uint32_t *__restrict__ lens, int64_t n,
-                                int K, CovTable t, unsigned thr, uint32_t passes, uint32_t pass) {
-    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= n) return;
-    const int L = (int)lens[r];
-    if (L < K) return;
-    const uint64_t *seq = words + offs[r];
-    CycHash h = cyc_init(seq, K);
-    for (int j = 0;; ++j) {
-        const uint64_t key = h.value() & t.key_mask;
-        if (cov_owner(key, passes) == pass) {
-            t.add(key, thr);
-            if ((K & 1) == 0 && h.fwd == h.rvs && window_self_rc(seq, j, K)) t.add(key, thr);
-        }
-        if (j + K >= L) break;
-        cyc_roll(h, base_at(seq, j), base_at(seq, j + K), K);
-    }
-}
-
-// cov_filter_k over pass `pass`: the read's windows of this pass below the threshold are added to below[r] (one thread per read, no
-// atomics); the last pass gives the verdict from the sum
-__global__ void cov_filter_pass_k(const uint64_t *__restrict__ words, const uint64_t *__restrict__ offs, const uint32_t *__restrict__ lens, int64_t n,
-                                  int K, CovTable t, unsigned thr, uint32_t passes, uint32_t pass, uint32_t *__restrict__ below,
-                                  uint8_t *__restrict__ keep, uint32_t *__restrict__ keep_words) {
-    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= n) return;
-    const bool last = pass + 1 == passes;
-    const int L = (int)lens[r];
-    bool k = thr == 0;                                         // CountMedianMlt returns 0 for a read shorter than K
-    if (L >= K) {
-        const uint64_t *seq = words + offs[r];
-        CycHash h = cyc_init(seq, K);
-        uint32_t b = pass ? below[r] : 0u;
-        for (int j = 0;; ++j) {
-            const uint64_t key = h.value() & t.key_mask;
-            if (cov_owner(key, passes) == pass) b += t.count(key) < thr;
-            if (j + K >= L) break;
-            cyc_roll(h, base_at(seq, j), base_at(seq, j + K), K);
-        }
-        if (!last) { below[r] = b; return; }
-        k = b <= (uint32_t)(L - K + 1) / 2;
-    }
-    if (!last) return;
-    keep[r] = k ? 1 : 0;
-    keep_words[r] = k ? (uint32_t)((L + 31) >> 5) : 0u;
 }
 
 }  // namespace
@@ -363,18 +306,53 @@ static unsigned cov_key_bits(size_t maxn) {
     return key_bits;
 }
 
-// What follows the verdict kernel, in both entry points: where each survivor and its words go (order kept), the number kept,
-// the flags for the caller and, with apply, the survivors as the context's read set (what CovFilteringWrap does to the streams).
+// pass 1 over the context's reads into 2^24 device registers (enqueued on the context's stream)
+static void cov_hll(Ctx *ctx, int K, uint32_t *reg) {
+    cudaStream_t st = ctx->stream;
+    const int64_t n = ctx->n_reads;
+    SG_CUDA(cudaMemsetAsync(reg, 0, (size_t)4 << 24, st));
+    if (n) { cov_hll_k<<<div_up(n, 128), 128, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, reg); ctx->launches++; }
+}
+
+struct CovBound {
+    size_t maxn = 0;            // cardinality upper bound
+    unsigned key_bits = 0;
+};
+// the bound of 2^24 device registers, once the work enqueued before them is done (synchronises)
+static CovBound cov_bound(Ctx *ctx, const uint32_t *reg) {
+    std::vector<uint32_t> h_reg((size_t)1 << 24);
+    SG_CUDA(cudaMemcpyAsync(h_reg.data(), reg, h_reg.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    SG_CUDA(cudaGetLastError());
+    SG_CUDA(cudaStreamSynchronize(ctx->stream));
+    CovBound b;
+    b.maxn = (size_t)hll_upper_bound(h_reg);
+    b.key_bits = cov_key_bits(b.maxn);
+    return b;
+}
+
+// What the verdict kernel feeds, and what follows it, in both entry points: the distinct-key counter, where each survivor and its
+// words go (order kept), the number kept, the flags for the caller, the statistics and, with apply, the survivors as the context's
+// read set (what CovFilteringWrap does to the streams).
 struct CovVerdicts {
     Ctx *ctx;
     int64_t n;
     DArr<uint8_t> keep;
     DArr<uint32_t> keep_words, flag;
+    DArr<unsigned long long> d_distinct;
     DArr<uint64_t> new_off, new_idx;
     uint64_t kept = 0, kept_words = 0;
-    explicit CovVerdicts(Ctx *c) : ctx(c), n(c->n_reads), keep(c, (size_t)c->n_reads + 1), keep_words(c, (size_t)c->n_reads + 1), flag(c, (size_t)c->n_reads + 1) {}
-    // after the verdict kernel: enqueues the scans and the copies of the totals and of keep_out (the caller synchronises)
-    void scan(uint8_t *keep_out) {
+    unsigned long long distinct = 0;
+    explicit CovVerdicts(Ctx *c) : ctx(c), n(c->n_reads), keep(c, (size_t)c->n_reads + 1), keep_words(c, (size_t)c->n_reads + 1), flag(c, (size_t)c->n_reads + 1),
+                                   d_distinct(c, 1) {
+        SG_CUDA(cudaMemsetAsync(d_distinct.p, 0, 8, c->stream));
+    }
+    // adds a table's occupied slots (one pass's, or this rank's slice) to the distinct keys
+    void count_distinct(const unsigned long long *e, uint64_t cap) {
+        cov_distinct_k<<<ctx->num_sms * 4, 256, 0, ctx->stream>>>(e, cap, d_distinct.p);
+        ctx->launches++;
+    }
+    // after the verdict kernel and the distinct counts; a set *overflow (when given) fails the call before any result is written
+    void finish(uint8_t *keep_out, const unsigned *overflow, const CovBound &b, uint64_t *stats, int apply) {
         cudaStream_t st = ctx->stream;
         if (n) { cov_keep_count_k<<<div_up(n, 256), 256, 0, st>>>(keep.p, n, flag.p); ctx->launches++; }
         SG_CUDA(cudaMemsetAsync(keep_words.p + n, 0, 4, st));
@@ -385,6 +363,14 @@ struct CovVerdicts {
         SG_CUDA(cudaMemcpyAsync(&kept, new_idx.p + n, 8, cudaMemcpyDeviceToHost, st));
         SG_CUDA(cudaMemcpyAsync(&kept_words, new_off.p + n, 8, cudaMemcpyDeviceToHost, st));
         if (keep_out && n) SG_CUDA(cudaMemcpyAsync(keep_out, keep.p, (size_t)n, cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaMemcpyAsync(&distinct, d_distinct.p, 8, cudaMemcpyDeviceToHost, st));
+        unsigned ovf = 0;
+        if (overflow) SG_CUDA(cudaMemcpyAsync(&ovf, overflow, 4, cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaGetLastError());
+        SG_CUDA(cudaStreamSynchronize(st));
+        SG_CHECK(!ovf, 6, "coverage filter: more distinct keys than the cardinality bound allows (table full)");
+        if (stats) { stats[0] = b.maxn; stats[1] = b.key_bits; stats[2] = distinct; stats[3] = kept; }
+        if (apply) this->apply();
     }
     void apply() {
         cudaStream_t st = ctx->stream;
@@ -410,63 +396,51 @@ void cov_filter(Ctx *ctx, int K, unsigned thr, int apply, int passes, uint8_t *k
     const int64_t n = ctx->n_reads;
     const int T = 128;
     // 1. cardinality upper bound
-    std::vector<uint32_t> h_reg((size_t)1 << 24);
+    CovBound b;
     {
         DArr<uint32_t> reg(ctx, (size_t)1 << 24);
-        SG_CUDA(cudaMemsetAsync(reg.p, 0, reg.bytes(), st));
-        if (n) { cov_hll_k<<<div_up(n, T), T, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, reg.p); ctx->launches++; }
-        SG_CUDA(cudaMemcpyAsync(h_reg.data(), reg.p, reg.bytes(), cudaMemcpyDeviceToHost, st));
-        SG_CUDA(cudaStreamSynchronize(st));
+        cov_hll(ctx, K, reg.p);
+        b = cov_bound(ctx, reg.p);
     }
-    const size_t maxn = (size_t)hll_upper_bound(h_reg);
     // 2. the table: one, or one per key range when one table does not fit next to the per-read arrays (cov_plan.h)
-    const unsigned key_bits = cov_key_bits(maxn);
     const uint64_t budget = ctx->budget_left();
-    const CovPassPlan plan = cov_pass_plan(maxn, n, budget);
+    const CovPassPlan plan = cov_pass_plan(b.maxn, n, budget);
     if (!passes) {
         if (!plan.passes) {
             char m[256];
             snprintf(m, sizeof m, "coverage filter: %llu device bytes needed with %d key-range passes (cardinality bound %zu), %llu left",
-                     (unsigned long long)plan.need, kCovMaxPasses, maxn, (unsigned long long)budget);
+                     (unsigned long long)plan.need, kCovMaxPasses, b.maxn, (unsigned long long)budget);
             throw Error(4, m);
         }
         passes = plan.passes;
     }
     CovVerdicts v(ctx);
-    DArr<unsigned long long> d_cnt(ctx, 1);
     DArr<unsigned> d_ovf(ctx, 1);
     DArr<uint32_t> below;
     if (passes > 1) below.alloc(ctx, (size_t)n + 1);
     CovTable t;
-    t.cap = cov_pass_capacity(maxn, passes);
-    t.key_mask = (1ull << key_bits) - 1;
+    t.cap = cov_pass_capacity(b.maxn, passes);
+    t.key_mask = (1ull << b.key_bits) - 1;
     DArr<unsigned long long> table(ctx, t.cap);
     t.e = table.p;
     ctx->times.cov_filter_passes = (uint64_t)passes;
     ctx->times.cov_filter_table_bytes = table.bytes();
-    SG_CUDA(cudaMemsetAsync(d_cnt.p, 0, 8, st));
     SG_CUDA(cudaMemsetAsync(d_ovf.p, 0, 4, st));
     t.overflow = d_ovf.p;
-    if (passes == 1) {
+    // 3. per pass: clear the table, insert the windows' keys, look them up per read
+    const auto roll = [&](const auto route) {
+        cov_fill_k<<<div_up(n, T), T, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, route, thr);
+        cov_filter_k<<<div_up(n, T), T, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, route, thr, below.p, v.keep.p, v.keep_words.p);
+        ctx->launches += 2;
+    };
+    for (int p = 0; p < passes; ++p) {
         SG_CUDA(cudaMemsetAsync(table.p, 0, table.bytes(), st));
         if (n) {
-            cov_fill_k<<<div_up(n, T), T, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, t, thr);
-            cov_filter_k<<<div_up(n, T), T, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, t, thr, v.keep.p, v.keep_words.p);
-            ctx->launches += 2;
+            if (passes == 1) roll(WholeTable{t});
+            else roll(KeyRange{t, (uint32_t)passes, (uint32_t)p});
         }
-        cov_distinct_k<<<ctx->num_sms * 4, 256, 0, st>>>(table.p, t.cap, d_cnt.p);
-        ctx->launches++;
-    } else {
-        for (int p = 0; p < passes; ++p) {
-            SG_CUDA(cudaMemsetAsync(table.p, 0, table.bytes(), st));
-            if (n) {
-                cov_fill_pass_k<<<div_up(n, T), T, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, t, thr, (uint32_t)passes, (uint32_t)p);
-                cov_filter_pass_k<<<div_up(n, T), T, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, t, thr, (uint32_t)passes, (uint32_t)p,
-                                                             below.p, v.keep.p, v.keep_words.p);
-                ctx->launches += 2;
-            }
-            cov_distinct_k<<<ctx->num_sms * 4, 256, 0, st>>>(table.p, t.cap, d_cnt.p);       // adds to the count of the passes before
-            ctx->launches++;
+        v.count_distinct(table.p, t.cap);
+        if (p + 1 < passes) {                          // the overflow flag is sticky: a full table stops the call before the next pass
             unsigned overflow = 0;
             SG_CUDA(cudaMemcpyAsync(&overflow, d_ovf.p, 4, cudaMemcpyDeviceToHost, st));
             SG_CUDA(cudaGetLastError());
@@ -476,16 +450,7 @@ void cov_filter(Ctx *ctx, int K, unsigned thr, int apply, int passes, uint8_t *k
     }
     table.release();                                   // the scans and the compaction below take its place (same stream)
     below.release();
-    v.scan(keep_out);
-    unsigned long long distinct = 0;
-    SG_CUDA(cudaMemcpyAsync(&distinct, d_cnt.p, 8, cudaMemcpyDeviceToHost, st));
-    unsigned overflow = 0;
-    SG_CUDA(cudaMemcpyAsync(&overflow, d_ovf.p, 4, cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaGetLastError());
-    SG_CUDA(cudaStreamSynchronize(st));
-    SG_CHECK(!overflow, 6, "coverage filter: more distinct keys than the cardinality bound allows (table full)");
-    if (stats) { stats[0] = maxn; stats[1] = key_bits; stats[2] = distinct; stats[3] = v.kept; }
-    if (apply) v.apply();
+    v.finish(keep_out, d_ovf.p, b, stats, apply);
 }
 
 // ---- distributed filter (sgpu_dist_cov_*): every rank holds a shard of the reads; the result equals cov_filter over the union --------
@@ -498,8 +463,8 @@ struct CovDist {
     unsigned thr = 0;
     DArr<uint32_t> reg;                      // this rank's HLL registers (peers read them in bound)
     DArr<unsigned long long> slice;          // this rank's slice: cap entries, then the overflow flag (peers write both in fill)
-    uint64_t maxn = 0, cap = 0;
-    unsigned key_bits = 0;
+    CovBound bound;
+    uint64_t cap = 0;
     std::vector<const uint32_t *> peer_reg;  // rank-indexed, as this process sees them
     std::vector<CovTable> peer_slice;
     bool filled = false;
@@ -519,13 +484,10 @@ CovDist *dist_cov_begin(Ctx *ctx, int K, unsigned thr, int world, int rank) {
     ensure_reads_on_device(ctx);
     std::unique_ptr<CovDist> d(new CovDist);
     d->ctx = ctx; d->K = K; d->thr = thr; d->world = world; d->rank = rank;
-    cudaStream_t st = ctx->stream;
-    const int64_t n = ctx->n_reads;
     d->reg.alloc(ctx, (size_t)1 << 24);
-    SG_CUDA(cudaMemsetAsync(d->reg.p, 0, d->reg.bytes(), st));
-    if (n) { cov_hll_k<<<div_up(n, 128), 128, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, K, d->reg.p); ctx->launches++; }
+    cov_hll(ctx, K, d->reg.p);
     SG_CUDA(cudaGetLastError());
-    SG_CUDA(cudaStreamSynchronize(st));                 // the registers are complete before they are published
+    SG_CUDA(cudaStreamSynchronize(ctx->stream));        // the registers are complete before they are published
     return d.release();
 }
 
@@ -557,7 +519,7 @@ void dist_cov_open_peers(CovDist *d, const uint8_t *descs) {
             CovTable &t = d->peer_slice[g];
             t.e = (unsigned long long *)(base + ds.off_slice);
             t.cap = ds.slice_cap;
-            t.key_mask = (1ull << d->key_bits) - 1;
+            t.key_mask = (1ull << d->bound.key_bits) - 1;
             t.overflow = (unsigned *)(t.e + t.cap);
         }
     }
@@ -568,7 +530,6 @@ void dist_cov_bound(CovDist *d) {
     SG_CHECK(d->reg.p && (int)d->peer_reg.size() == d->world && !d->slice.p, 2,
              "sgpu_dist_cov_bound runs once, after sgpu_dist_cov_open_peers with the descriptors of sgpu_dist_cov_begin");
     cudaStream_t st = ctx->stream;
-    std::vector<uint32_t> h_reg((size_t)1 << 24);
     {
         DArr<uint32_t> merged(ctx, (size_t)1 << 24);
         DArr<uint64_t> regs(ctx, (size_t)d->world);
@@ -576,13 +537,9 @@ void dist_cov_bound(CovDist *d) {
         const uint32_t n4 = (1u << 24) / 4;
         cov_hll_merge_k<<<div_up(n4, 256), 256, 0, st>>>((const uint4 *const *)regs.p, d->world, (uint4 *)merged.p, n4);
         ctx->launches++;
-        SG_CUDA(cudaMemcpyAsync(h_reg.data(), merged.p, merged.bytes(), cudaMemcpyDeviceToHost, st));
-        SG_CUDA(cudaGetLastError());
-        SG_CUDA(cudaStreamSynchronize(st));
+        d->bound = cov_bound(ctx, merged.p);
     }
-    d->maxn = (uint64_t)(size_t)hll_upper_bound(h_reg);
-    d->key_bits = cov_key_bits((size_t)d->maxn);
-    d->cap = cov_slice_capacity(d->maxn, d->world);
+    d->cap = cov_slice_capacity(d->bound.maxn, d->world);
     d->slice.alloc(ctx, d->cap + 1);
     SG_CUDA(cudaMemsetAsync(d->slice.p, 0, d->slice.bytes(), st));
     SG_CUDA(cudaStreamSynchronize(st));                 // the slice is empty before it is published
@@ -599,8 +556,8 @@ void dist_cov_fill(CovDist *d) {
     DArr<CovTable> slices(ctx, (size_t)d->world);
     SG_CUDA(cudaMemcpyAsync(slices.p, d->peer_slice.data(), (size_t)d->world * sizeof(CovTable), cudaMemcpyHostToDevice, st));
     if (n) {
-        cov_fill_dist_k<<<div_up(n, 128), 128, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, d->K, slices.p, (uint32_t)d->world,
-                                                        (1ull << d->key_bits) - 1, d->thr);
+        const OwnerSlices route{slices.p, (uint32_t)d->world, (1ull << d->bound.key_bits) - 1};
+        cov_fill_k<<<div_up(n, 128), 128, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, d->K, route, d->thr);
         ctx->launches++;
     }
     SG_CUDA(cudaGetLastError());
@@ -622,22 +579,14 @@ void dist_cov_filter(CovDist *d, int apply, uint8_t *keep_out, uint64_t *stats) 
     DArr<CovTable> slices(ctx, (size_t)d->world);
     SG_CUDA(cudaMemcpyAsync(slices.p, d->peer_slice.data(), (size_t)d->world * sizeof(CovTable), cudaMemcpyHostToDevice, st));
     CovVerdicts v(ctx);
-    DArr<unsigned long long> d_cnt(ctx, 1);
-    SG_CUDA(cudaMemsetAsync(d_cnt.p, 0, 8, st));
     if (n) {
-        cov_filter_dist_k<<<div_up(n, 128), 128, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, d->K, slices.p, (uint32_t)d->world,
-                                                          (1ull << d->key_bits) - 1, d->thr, v.keep.p, v.keep_words.p);
+        const OwnerSlices route{slices.p, (uint32_t)d->world, (1ull << d->bound.key_bits) - 1};
+        cov_filter_k<<<div_up(n, 128), 128, 0, st>>>(ctx->d_words, ctx->d_offs, ctx->d_lens, n, d->K, route, d->thr, nullptr, v.keep.p,
+                                                     v.keep_words.p);
         ctx->launches++;
     }
-    cov_distinct_k<<<ctx->num_sms * 4, 256, 0, st>>>(d->slice.p, d->cap, d_cnt.p);
-    ctx->launches++;
-    v.scan(keep_out);
-    unsigned long long distinct = 0;
-    SG_CUDA(cudaMemcpyAsync(&distinct, d_cnt.p, 8, cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaGetLastError());
-    SG_CUDA(cudaStreamSynchronize(st));                 // this rank reads no slice any more
-    if (stats) { stats[0] = d->maxn; stats[1] = d->key_bits; stats[2] = distinct; stats[3] = v.kept; }
-    if (apply) v.apply();
+    v.count_distinct(d->slice.p, d->cap);
+    v.finish(keep_out, nullptr, d->bound, stats, apply);      // synchronises: this rank reads no slice any more
 }
 
 void dist_cov_free(CovDist *d) { delete d; }
