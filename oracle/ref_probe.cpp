@@ -13,7 +13,7 @@
 // test/debruijn/test_utils.cpp:128-138).
 //
 // usage: ref_probe <mode: count|graph|bench> <reads.txt> <k> <num_buckets> <nthreads> <outdir>   (env PROBE_EARLY_TC=<bound>: graph mode
-//        also runs EarlyTipClipperProcessor before the unitig extraction)
+//        also runs EarlyTipClipperProcessor before the unitig extraction; PROBE_EARLY_AT, PROBE_NO_LOOPS: see below)
 //   reads.txt: one ACGT read per line (N-trimming is the ingest layer's job)
 #include "io/reads/vector_reader.hpp"
 #include "io/reads/rc_reader_wrapper.hpp"
@@ -254,9 +254,17 @@ int main(int argc, char **argv) {
     }
 
     // PROBE_EARLY_AT=1: the RNA pipeline's early low-complexity clipper (stages/construction.cpp:317-340: at_ratio 0.8, min 10, max 200)
-    // between the mask fill and everything downstream; masks_at.bin = the array after it, at_removed.txt = the two return values
-    if (getenv("PROBE_EARLY_AT")) {
-        EarlyLowComplexityClipperProcessor at(ext, 0.8, 10, 200);
+    // between the mask fill and everything downstream; masks_at.bin = the array after it, at_removed.txt = the two return values.
+    // PROBE_EARLY_AT=<ratio>,<min_length>,<max_length> runs it with those parameters instead.
+    if (const char *atp = getenv("PROBE_EARLY_AT")) {
+        double ratio = 0.8;
+        size_t min_len = 10, max_len = 200;
+        if (strchr(atp, ',')) {
+            unsigned long long mn = 0, mx = 0;
+            if (sscanf(atp, "%lf,%llu,%llu", &ratio, &mn, &mx) != 3) { fprintf(stderr, "PROBE_EARLY_AT: want ratio,min,max\n"); return 2; }
+            min_len = (size_t)mn; max_len = (size_t)mx;
+        }
+        EarlyLowComplexityClipperProcessor at(ext, ratio, min_len, max_len);
         size_t e = at.RemoveATEdges();
         size_t t = at.RemoveATTips();
         std::ofstream ms(outdir / "masks_at.bin", std::ios::binary);
@@ -276,8 +284,13 @@ int main(int argc, char **argv) {
         rs << removed << "\n";
     }
 
+    // PROBE_NO_LOOPS=1: keep_perfect_loops = false, DeBruijnGraphExtentionConstructor::ConstructGraph(false)
+    // (debruijn_graph_constructor.hpp:590-596): the unbranching paths only, no perfect loops
     unsigned nchunks = 16 * omp_get_max_threads();
-    std::vector<Sequence> edges = UnbranchingPathExtractor(ext, k).ExtractUnbranchingPathsAndLoops(nchunks);
+    const char *no_loops = getenv("PROBE_NO_LOOPS");
+    std::vector<Sequence> edges = (no_loops && atoi(no_loops))
+                                  ? UnbranchingPathExtractor(ext, k).ExtractUnbranchingPaths(nchunks)
+                                  : UnbranchingPathExtractor(ext, k).ExtractUnbranchingPathsAndLoops(nchunks);
     {
         std::ofstream os(outdir / "unitigs.txt");
         for (const auto &e : edges) os << e.str() << "\n";

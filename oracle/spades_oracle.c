@@ -605,7 +605,9 @@ int64_t orc_early_tip_clip(const kset_t *km, const mphf_t *mk, uint8_t *masks, i
     if (snapshot) { view = (uint8_t *)malloc((size_t)(km->n ? km->n : 1)); memcpy(view, masks, (size_t)km->n); }
     gctx_t g; g.m = mk; g.K = K; g.masks = view;
     uint64_t *tips[4];
-    for (int c = 0; c < 4; ++c) tips[c] = (uint64_t *)malloc((size_t)(length_bound + 2) * 8);
+    /* a walk visits each oriented k-mer at most once, so a bound beyond 2 n never binds: the buffers need no more than that */
+    const int64_t cap = length_bound < 2 * km->n ? length_bound : 2 * km->n;
+    for (int c = 0; c < 4; ++c) tips[c] = (uint64_t *)malloc((size_t)(cap + 2) * 8);
     uint64_t *tj = NULL; int64_t ntj = 0, ctj = 0;          /* tipped junctions: k-mer words */
     int64_t removed = 0;
     for (int64_t i = 0; i < km->n; ++i) {
@@ -726,7 +728,7 @@ void orc_early_at_clip(const kset_t *km, const mphf_t *mk, uint8_t *masks, doubl
     uint8_t *view = masks;
     if (snapshot) { view = (uint8_t *)malloc((size_t)(km->n ? km->n : 1)); memcpy(view, masks, (size_t)km->n); }
     g.masks = view;
-    uint64_t *tip = (uint64_t *)malloc((size_t)(max_len + 1) * 8);
+    uint64_t *tip = (uint64_t *)malloc((size_t)((max_len < 2 * km->n ? max_len : 2 * km->n) + 1) * 8);   /* a walk visits each oriented k-mer once */
     uint64_t *roots = NULL; int64_t nr = 0, cr = 0;
     int64_t removed_kmers = 0;
     for (int64_t i = 0; i < km->n; ++i) {

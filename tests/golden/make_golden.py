@@ -33,15 +33,16 @@ def ecoli_reads():
     return reads
 
 
-def loops_reads():
+def loops_reads(loop_len=120, hairpin_len=150):
+    """windows of a 500-bp circle (a perfect loop) and of a 400-bp hairpin circle x + rc(x); windows longer than k + 1 for every k"""
     rng = np.random.default_rng(5)
     g = "".join("ACGT"[i] for i in rng.integers(0, 4, 500))
     gg = g + g
-    reads = [gg[i:i + 120] for i in range(0, 500, 7)]
+    reads = [gg[i:i + loop_len] for i in range(0, 500, 7)]
     x = "".join("ACGT"[i] for i in rng.integers(0, 4, 200))
     h = x + revcomp(x)
     hh = h + h
-    reads += [hh[i:i + 150] for i in range(0, 400, 5)]
+    reads += [hh[i:i + hairpin_len] for i in range(0, 400, 5)]
     return reads
 
 
@@ -72,6 +73,25 @@ def at_reads(n, L, glen, err, seed):
     return out + ["A" * L] * 5 + ["AT" * (L // 2)] * 3
 
 
+def at_arm_reads(arm_len, L, seed):
+    """error-free windows of a stem that forks into an A-rich arm and a random arm, and one read that leaves the random arm for a
+    4-base poly-A tip. The A-rich arm (88% A between C and G, no run longer than 12: it shares no k-mer with at_reads' A/T tails) is a
+    low-complexity dead-end chain of arm_len vertices, so RemoveATTips clips it only when max_length >= arm_len. The poly-A tip
+    is low-complexity on its own, but not once the root's last nucleotides are counted up to min_length."""
+    rng = np.random.default_rng(seed)
+    stem = _random_seq(rng, 150)
+    rich, run = "A", 1
+    while len(rich) < arm_len:
+        c = "A" if run < 12 and rng.random() < 0.88 else "CG"[int(rng.integers(0, 2))]
+        rich += c
+        run = run + 1 if c == "A" else 0
+    arms = [rich, "C" + _random_seq(rng, 199)]                          # the fork: A | C
+    reads = [s[i:i + L] for s in (stem + a for a in arms) for i in range(0, len(s) - L + 1, 10)]
+    s = stem + arms[1]
+    j = max(j for j in range(len(s) - L + 4) if s[j + L - 4] != "A")
+    return reads + [s[j:j + L - 4] + "AAAA"]
+
+
 def _random_seq(rng, n):
     return "".join("ACGT"[i] for i in rng.integers(0, 4, n))
 
@@ -98,7 +118,7 @@ def isolated_reads(n, seed):
     return [_random_seq(rng, 70) for _ in range(n)]
 
 
-def run_probe(mode, reads, k, B, T=2, early_tc=0, early_at=False, edge_index=None):
+def run_probe(mode, reads, k, B, T=2, early_tc=0, early_at=False, edge_index=None, no_loops=False):
     with tempfile.TemporaryDirectory() as d:
         rf = os.path.join(d, "reads.txt")
         open(rf, "w").write("\n".join(reads) + "\n")
@@ -110,6 +130,8 @@ def run_probe(mode, reads, k, B, T=2, early_tc=0, early_at=False, edge_index=Non
             env["PROBE_EARLY_AT"] = "1"                # EarlyLowComplexityClipperProcessor (RNA pipeline), before the tip clipper
         if early_tc:
             env["PROBE_EARLY_TC"] = str(early_tc)      # EarlyTipClipperProcessor between mask fill and unitig extraction
+        if no_loops:
+            env["PROBE_NO_LOOPS"] = "1"                # keep_perfect_loops = false: unbranching paths only
         subprocess.check_call([PROBE, mode, rf, str(k), str(B), str(T), out], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL, env=env)
         res = {}
         for f in os.listdir(out):
@@ -120,12 +142,15 @@ def run_probe(mode, reads, k, B, T=2, early_tc=0, early_at=False, edge_index=Non
 
 
 def save(name, mode, reads, k, B, early_tc=0, edge_index=None):
+    if ONLY and name not in ONLY:
+        return
     """mode "tcgraph" = graph mode with the pipeline's early tip clipper (length bound early_tc); masks_bin is the array
     before the clipper, masks_tc_bin after it, everything downstream (unitigs, GFA) comes from the clipped index.
     mode "atgraph" = graph mode with the RNA pipeline's early A/T clipper (masks_at_bin, at_removed_txt), followed by the tip clipper
-    when early_tc is given (then masks_tc_bin is the array after both)."""
-    res = run_probe("graph" if mode in ("tcgraph", "atgraph", "eigraph") else mode, reads, k, B, early_tc=early_tc, early_at=(mode == "atgraph"),
-                    edge_index=edge_index)
+    when early_tc is given (then masks_tc_bin is the array after both).
+    mode "nlgraph" = graph mode with keep_perfect_loops = false."""
+    res = run_probe("graph" if mode in ("tcgraph", "atgraph", "eigraph", "nlgraph") else mode, reads, k, B, early_tc=early_tc,
+                    early_at=(mode == "atgraph"), edge_index=edge_index, no_loops=(mode == "nlgraph"))
     if edge_index is not None:
         res["ei_k"] = np.array([edge_index if edge_index else k + 1])
         res["ei_chunks"] = np.array([10 * 2])          # run_probe's T = 2: the (k+1)-mer path walks the edges in 10 x T vertex chunks
@@ -138,6 +163,8 @@ def save(name, mode, reads, k, B, early_tc=0, edge_index=None):
 
 
 def save_covfilter(name, reads, k, thr):
+    if ONLY and name not in ONLY:
+        return
     """SURVEY 8f-3: ref_probe covfilter = the pipeline's CoverageFilter phase (EstimateCardinalityUpperBound -> qf::cqf ->
     FillCoverageHistogram -> CoverageFilter on every read) over (k+1)-mers; keeps the cardinality bound, the filter's key bits, the
     verdict per read and the SymmetricCyclicHash of every window of the first 64 reads."""
@@ -189,6 +216,8 @@ def ingest_case_files():
 
 
 def save_ingest():
+    if ONLY and "ingest_cases" not in ONLY:
+        return
     res = {}
     with tempfile.TemporaryDirectory() as d:
         for name, data in ingest_case_files().items():
@@ -202,7 +231,11 @@ def save_ingest():
     print("ingest_cases", {a: len(b) for a, b in res.items()})
 
 
+ONLY = set()          # fixture names to (re)write (the command line); empty = all of them
+
+
 if __name__ == "__main__":
+    ONLY.update(sys.argv[1:])
     save_ingest()
     ec = ecoli_reads()
     save("ecoli_k21_B40_graph", "graph", ec, 21, 40)          # BASELINE.json configs[0]
@@ -213,6 +246,9 @@ if __name__ == "__main__":
     save("syn_k21_B10_graph", "graph", synthetic_reads(400, 100, 1500, 0.01, seed=1), 21, 10)
     save("syn_k33_B5_count", "count", synthetic_reads(300, 100, 1500, 0.01, seed=2), 33, 5)
     save("loops_k21_B10_graph", "graph", loops_reads(), 21, 10)
+    # keep_perfect_loops = false: the circles' edges are left out; synthetic reads add ordinary unitigs
+    save("loops_k21_B10_nlgraph", "nlgraph", loops_reads() + synthetic_reads(300, 120, 700, 0.02, seed=3), 21, 10)
+    save("loops_k127_B7_nlgraph", "nlgraph", loops_reads(250, 250) + synthetic_reads(200, 250, 1000, 0.0005, seed=17), 127, 7)
     save("dense_k5_B4_graph", "graph", synthetic_reads(200, 60, 200, 0.02, seed=3), 5, 4)
     save("dense_k3_B1_graph", "graph", synthetic_reads(100, 40, 100, 0.02, seed=4), 3, 1)
     # Construction stage with early_tc (stages/construction.cpp:289-302): length bound = read length - k
@@ -221,11 +257,16 @@ if __name__ == "__main__":
     save("syn_k21_B10_tcgraph", "tcgraph", synthetic_reads(2000, 100, 3000, 0.02, seed=6), 21, 10, early_tc=79)
     save("loops_k21_B10_tcgraph", "tcgraph", loops_reads() + synthetic_reads(300, 120, 700, 0.02, seed=3), 21, 10, early_tc=99)
     save("dense_k7_B4_tcgraph", "tcgraph", synthetic_reads(800, 60, 400, 0.03, seed=14), 7, 4, early_tc=10)
+    # four-word k-mers: the multi-k pipeline's k = 99 and 127 on 250-bp reads
+    save("syn_k99_B9_tcgraph", "tcgraph", synthetic_reads(150, 250, 1000, 0.001, seed=15), 99, 9, early_tc=250 - 99)
+    save("syn_k127_B5_tcgraph", "tcgraph", synthetic_reads(150, 250, 1000, 0.001, seed=16), 127, 5, early_tc=250 - 127)
     # RNA pipeline: EarlyATClipper (stages/construction.cpp:317-340), alone and followed by the tip clipper (:447-450)
     save("rna_k21_B8_atgraph", "atgraph", at_reads(3000, 100, 3000, 0.01, 1), 21, 8)
     save("rna_k33_B5_atgraph", "atgraph", at_reads(1000, 150, 1500, 0.02, 2), 33, 5, early_tc=150 - 33)       # fixtures stay below 1 MB
     save("rna_k55_B16_atgraph", "atgraph", at_reads(1000, 150, 2000, 0.01, 3), 55, 16, early_tc=150 - 55)
     save("rna_k11_B3_atgraph", "atgraph", at_reads(1500, 60, 800, 0.05, 4), 11, 3)
+    # four-word k-mers (k = 97): 250-bp reads and an A-rich dead-end arm of 350 vertices, past RemoveATTips' max_length of 200
+    save("rna_k97_B6_atgraph", "atgraph", at_reads(120, 250, 800, 0.002, 5) + at_arm_reads(350, 250, 6), 97, 6, early_tc=250 - 97)
     # EdgeIndex refill (SURVEY 8f-1): the (k+1)-mer index of the pipeline and the counting path with a smaller K; B = 10 x 2 threads
     save("syn_k21_B20_eigraph", "eigraph", synthetic_reads(600, 100, 1500, 0.01, seed=5), 21, 20, edge_index=0)
     save("syn_k21_B20_K15_eigraph", "eigraph", synthetic_reads(600, 100, 1500, 0.01, seed=5), 21, 20, edge_index=15)

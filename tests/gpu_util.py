@@ -24,11 +24,13 @@ def release():
         _CTX = None
 
 
-def gpu_graph_artifacts(reads, k, B, keep_loops=True, early_tc=0, early_at=False):
+def gpu_graph_artifacts(reads, k, B, keep_loops=True, early_tc=0, early_at=False, at_params=(0.8, 10, 200)):
+    """at_params: (ratio, min_length, max_length) of the A/T clipper"""
     c = ctx()
     c.set_reads(*pack_reads(reads))
+    ratio, min_len, max_len = at_params
     g = DeBruijnGraphConstructor(c, k, B).ConstructGraph(keep_perfect_loops=keep_loops, with_coverage=True, early_tip_clipper_length=early_tc,
-                                                       early_at_clipper=early_at)
+                                                       early_at_clipper=early_at, at_ratio=ratio, at_min_length=min_len, at_max_length=max_len)
     art = dict(kpomers=g.kpomers.kmers(), kp_bsz=g.kpomers.bucket_sizes(), kmers=g.kmers.kmers(),
                kmer_index=g.kmer_index.serialize(), kpomer_index=g.kpomer_index.serialize(), masks=g.masks(),
                cov=g.coverage(), hist=g.histogram().astype(np.int64), unitigs=g.unitigs(), gfa=g.gfa())

@@ -204,10 +204,12 @@ def gfa(u: Unitigs, mk: Mphf, mkp: Mphf = None, cov=None, version="SPAdes-4.3.0-
     return s
 
 
-def full_graph(reads, k, B, early_tc=0, early_at=False):
+def full_graph(reads, k, B, early_tc=0, early_at=False, keep_loops=True, at_params=(0.8, 10, 200)):
     """Whole path on a list of ACGT strings; returns dict of artefacts named like ref_probe's files.
     early_tc > 0: run the early tip clipper with that length bound between the mask fill and the unitig extraction
-    (stages/construction.cpp:289-302); `masks` then holds the clipped array and `masks_raw` the one before."""
+    (stages/construction.cpp:289-302); `masks` then holds the clipped array and `masks_raw` the one before.
+    early_at: the A/T clipper with at_params = (ratio, min_length, max_length) before it. keep_loops = False: the unbranching
+    paths only, without the perfect loops (ConstructGraph(false), debruijn_graph_constructor.hpp:590-596)."""
     from spades_b200.packing import pack_reads
     if k % 2 == 0:
         raise ValueError("k must be odd (projects/spades_tools/gbuilder.cpp:125): with even k a k-mer can be its own reverse complement")
@@ -221,12 +223,12 @@ def full_graph(reads, k, B, early_tc=0, early_at=False):
     tc = None
     at = None
     if early_at:                  # the RNA pipeline's EarlyATClipper runs before the tip clipper (stages/construction.cpp:447-450)
-        mk_arr, at = early_at_clip(km, mk, mk_arr)
+        mk_arr, at = early_at_clip(km, mk, mk_arr, *at_params)
     if early_tc:
         mk_arr, removed, tipped, clipped = early_tip_clip(km, mk, mk_arr, early_tc)
         tc = dict(removed=removed, tipped=tipped, clipped=clipped)
     cov = coverage(kp, mkp)
-    u = Unitigs(km, mk, mk_arr, True)
+    u = Unitigs(km, mk, mk_arr, keep_loops)
     return dict(kp=kp, km=km, mk=mk, mkp=mkp, masks=mk_arr, masks_raw=raw, tc=tc, at=at, cov=cov, hist=histogram(cov), unitigs=u,
                 gfa=gfa(u, mk, mkp, cov))
 

@@ -160,7 +160,7 @@ def test_graph_path_on_pass_split_sets(k, B, budget, kind):
     _check_lookups(lookups, want)
 
 
-@pytest.mark.parametrize("k,B", [(21, 24), (55, 16)])
+@pytest.mark.parametrize("k,B", [(21, 24), (55, 16), (127, 40)])
 def test_early_tip_clipper_on_pass_split_sets(k, B):
     L = 150
     reads = synthetic_reads(3000, L, 3000, 0.02, seed=50 + k) + _loop_reads()

@@ -68,7 +68,8 @@ def test_early_at_clipper_matches_reference_golden(name):
     assert G.check_graph(g, art) == []
 
 
-@pytest.mark.parametrize("k,B,n,L,glen,seed", [(21, 8, 2500, 100, 2500, 61), (55, 12, 2500, 150, 4000, 62), (77, 3, 1500, 150, 2500, 63), (13, 2, 1500, 60, 700, 64)])
+@pytest.mark.parametrize("k,B,n,L,glen,seed", [(21, 8, 2500, 100, 2500, 61), (55, 12, 2500, 150, 4000, 62), (77, 3, 1500, 150, 2500, 63), (13, 2, 1500, 60, 700, 64),
+                                               (63, 7, 1500, 150, 2500, 65), (97, 5, 600, 250, 2500, 66), (127, 4, 600, 250, 2500, 67)])
 def test_early_at_clipper_matches_oracle_random(k, B, n, L, glen, seed):
     import sys, os
     sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
@@ -173,7 +174,9 @@ def test_edge_index_refill_matches_oracle_cases(k, B, K, kind, seed):
 
 
 @pytest.mark.parametrize("k,B,n,L,glen,err,seed", [(21, 16, 3000, 100, 4000, 0.02, 51), (55, 20, 3000, 150, 4000, 0.02, 52), (77, 3, 1500, 150, 2000, 0.01, 53),
-                                                   (9, 3, 1000, 60, 600, 0.1, 54), (33, 2, 2000, 120, 900, 0.03, 55)])
+                                                   (9, 3, 1000, 60, 600, 0.1, 54), (33, 2, 2000, 120, 900, 0.03, 55),
+                                                   (31, 6, 2000, 100, 2500, 0.02, 56), (63, 9, 2000, 150, 3000, 0.01, 57),       # last word full (62 bits)
+                                                   (99, 7, 800, 250, 3000, 0.005, 58), (127, 5, 800, 250, 3000, 0.005, 59)])     # four words
 def test_early_tip_clipper_matches_oracle_random(k, B, n, L, glen, err, seed):
     from gpu_util import gpu_graph_artifacts
     reads = synthetic_reads(n, L, glen, err, seed=seed)

@@ -12,8 +12,8 @@ import oracle as O
 from spades_b200.packing import pack_reads, revcomp, unpack_kmers
 
 
-def oracle_artifacts(reads, k, B, early_tc=0, early_at=False):
-    r = O.full_graph(reads, k, B, early_tc=early_tc, early_at=early_at)
+def oracle_artifacts(reads, k, B, early_tc=0, early_at=False, keep_loops=True, at_params=(0.8, 10, 200)):
+    r = O.full_graph(reads, k, B, early_tc=early_tc, early_at=early_at, keep_loops=keep_loops, at_params=at_params)
     art = dict(kpomers=r["kp"].keys, kp_bsz=r["kp"].bsz, kmers=r["km"].keys, kmer_index=r["mk"].serialize(),
                kpomer_index=r["mkp"].serialize(), masks=r["masks"], cov=r["cov"], hist=r["hist"],
                unitigs=r["unitigs"].seqs, gfa=r["gfa"])
@@ -38,6 +38,25 @@ def test_oracle_early_at_clipper_matches_reference_golden(name):
     snap_m, snap_s = O.early_at_clip(r["km"], r["mk"], r["masks_raw"], snapshot=True)
     seq_m, seq_s = O.early_at_clip(r["km"], r["mk"], r["masks_raw"], snapshot=False)
     assert np.array_equal(snap_m, seq_m) and snap_s == seq_s == r["at"]
+
+
+def test_oracle_early_at_clipper_golden_reaches_max_length():
+    """rna_k97: an A-rich dead-end arm of 350 vertices. RemoveATTips gives up on it at max_length 200 (early_simplification.hpp:
+    292-302) and clips it without that bound, so the fixture takes the "too long" branch"""
+    g = G.load("rna_k97_B6_atgraph")
+    at200 = O.full_graph(g["reads"], g["k"], g["B"], early_at=True)["at"]
+    at_inf = O.full_graph(g["reads"], g["k"], g["B"], early_at=True, at_params=(0.8, 10, 10 ** 6))["at"]
+    assert at_inf[2] - at200[2] >= 350 and at_inf[3] > at200[3]
+
+
+@pytest.mark.parametrize("name", G.names("nlgraph"))
+def test_oracle_no_loops_matches_reference_golden(name):
+    """keep_perfect_loops = false (ConstructGraph(false) -> ExtractUnbranchingPaths, debruijn_graph_constructor.hpp:590-596): unitigs
+    and GFA without the perfect loops against the unmodified reference; the same reads with loops kept give more unitigs"""
+    g = G.load(name)
+    art, r = oracle_artifacts(g["reads"], g["k"], g["B"], keep_loops=False)
+    assert G.check_graph(g, art) == []
+    assert len(O.full_graph(g["reads"], g["k"], g["B"])["unitigs"].seqs) > len(r["unitigs"].seqs)
 
 
 @pytest.mark.parametrize("name", G.names("tcgraph"))

@@ -19,10 +19,12 @@ import pytest
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 sys.path.insert(0, os.path.dirname(HERE))
+sys.path.insert(0, os.path.join(HERE, "golden"))
 
 import golden_util as G  # noqa: E402
 import oracle as O  # noqa: E402
 from spades_b200.packing import synthetic_reads  # noqa: E402
+from make_golden import at_reads, loops_reads  # noqa: E402
 from test_oracle_golden import oracle_artifacts  # noqa: E402
 
 PROBE = os.path.join(os.path.dirname(HERE), "oracle", "_ref", "ref_probe")
@@ -31,7 +33,12 @@ RECORD = os.path.join(G.GOLDEN_DIR, "oracle_vs_reference.json")
 GRAPH_CASES = [(21, 16, 11), (31, 5, 12), (55, 30, 13), (63, 9, 14), (77, 4, 15), (127, 6, 16)]
 COUNT_CASES = [(21, 16, 21), (55, 16, 22), (100, 3, 23)]
 TC_CASES = [(21, 16, 3000, 100, 4000, 0.01, 41, 1), (21, 8, 3000, 100, 2000, 0.03, 42, 8), (55, 30, 3000, 150, 5000, 0.01, 43, 3),
-            (77, 4, 1500, 150, 2000, 0.01, 44, 8), (9, 3, 1000, 60, 600, 0.1, 45, 8)]
+            (77, 4, 1500, 150, 2000, 0.01, 44, 8), (9, 3, 1000, 60, 600, 0.1, 45, 8),
+            (99, 7, 600, 250, 3000, 0.005, 46, 1), (127, 5, 600, 250, 3000, 0.005, 47, 8)]      # four-word k-mers, 250-bp reads
+# keep_perfect_loops = false: (k, B, seed, T) over the loop and hairpin circles plus synthetic reads
+NL_CASES = [(21, 9, 61, 3), (127, 4, 62, 8)]
+# the A/T clipper at non-default (ratio, min_length, max_length), then the tip clipper: (k, B, n, L, glen, err, seed, T, at_params)
+AT_CASES = [(33, 6, 1200, 150, 1500, 0.01, 71, 8, (0.7, 20, 60))]
 COV_CASES = [(21, 2, 51, 1), (20, 3, 52, 8), (55, 2, 53, 3), (63, 4, 54, 8), (69, 2, 55, 2), (127, 3, 56, 8), (11, 6, 57, 8)]
 
 
@@ -39,7 +46,7 @@ def _sha(b):
     return hashlib.sha256(bytes(b)).hexdigest()
 
 
-def run_probe(mode, reads, k, B, T=3, early_tc=0):
+def run_probe(mode, reads, k, B, T=3, early_tc=0, at_params=None, no_loops=False):
     with tempfile.TemporaryDirectory() as d:
         rf = os.path.join(d, "reads.txt")
         open(rf, "w").write("\n".join(reads) + "\n")
@@ -47,6 +54,10 @@ def run_probe(mode, reads, k, B, T=3, early_tc=0):
         env = dict(os.environ)
         if early_tc:
             env["PROBE_EARLY_TC"] = str(early_tc)
+        if at_params is not None:
+            env["PROBE_EARLY_AT"] = "%r,%d,%d" % tuple(at_params)
+        if no_loops:
+            env["PROBE_NO_LOOPS"] = "1"
         subprocess.check_call([PROBE, mode, rf, str(k), str(B), str(T), out], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL, env=env, timeout=600)
         g = {f.replace(".", "_"): np.frombuffer(open(os.path.join(out, f), "rb").read(), np.uint8)
              for f in os.listdir(out) if os.path.isfile(os.path.join(out, f))}
@@ -57,12 +68,13 @@ def run_probe(mode, reads, k, B, T=3, early_tc=0):
 def graph_digests_of_reference(g, keys):
     """SHA-256 of each artefact of a ref_probe graph run, in the form golden_util.check_graph compares (only `keys`)"""
     k, B = g["k"], g["B"]
-    masks = g["masks_tc_bin"] if "masks_tc_bin" in g else g["masks_bin"]
+    masks = g["masks_tc_bin"] if "masks_tc_bin" in g else (g["masks_at_bin"] if "masks_at_bin" in g else g["masks_bin"])
     canon = {"kpomers": lambda: g["kpomers"].tobytes(), "kp_bsz": lambda: G._txt_ints(g["kpomer_bucket_sizes_txt"]).tobytes(),
              "kmers": lambda: g["kmers"].tobytes(), "kmer_index": lambda: G.index_canonical(G.strip_uleb_k(g["kmer_index_bin"].tobytes(), k), B),
              "kpomer_index": lambda: G.index_canonical(G.strip_uleb_k(g["kpomer_index_bin"].tobytes(), k + 1), B),
              "masks": lambda: masks.tobytes(), "masks_raw": lambda: g["masks_bin"].tobytes(),
              "tc_removed": lambda: str(int(g["tc_removed_txt"].tobytes().decode().split()[0])).encode(),
+             "at_removed": lambda: " ".join(g["at_removed_txt"].tobytes().decode().split()).encode(),
              "cov": lambda: g["coverage_bin"].tobytes(), "hist": lambda: G._txt_ints(g["histogram_txt"]).tobytes(),
              "unitigs": lambda: "\n".join(g["unitigs_txt"].tobytes().decode().split()).encode(), "gfa": lambda: g["graph_gfa"].tobytes()}
     return {key: _sha(canon[key]()) for key in keys}
@@ -73,6 +85,7 @@ def graph_digests_of(art, B):
              "kmers": lambda v: np.asarray(v, np.uint64).ravel().tobytes(), "kmer_index": lambda v: G.index_canonical(v, B),
              "kpomer_index": lambda v: G.index_canonical(v, B), "masks": lambda v: np.asarray(v, np.uint8).tobytes(),
              "masks_raw": lambda v: np.asarray(v, np.uint8).tobytes(), "tc_removed": lambda v: str(int(v)).encode(),
+             "at_removed": lambda v: " ".join(str(int(x)) for x in v).encode(),
              "cov": lambda v: np.asarray(v, np.uint32).tobytes(), "hist": lambda v: np.asarray(v, np.int64).tobytes(),
              "unitigs": lambda v: "\n".join(v).encode(), "gfa": lambda v: v.encode()}
     return {key: _sha(canon[key](v)) for key, v in art.items()}
@@ -92,6 +105,18 @@ def _tc_id(k, B, n, L, glen, err, seed, T):
 
 def _tc_reads(n, L, glen, err, seed):
     return synthetic_reads(n, L, glen, err, seed=seed)
+
+
+def _nl_id(k, B, seed, T):
+    return "nl_k%d_B%d_s%d_T%d" % (k, B, seed, T)
+
+
+def _nl_reads(seed):
+    return loops_reads(250, 250) + synthetic_reads(400, 250, 1500, 0.002, seed=seed)
+
+
+def _at_id(k, B, n, L, glen, err, seed, T, at_params):
+    return "at_k%d_B%d_n%d_L%d_g%d_e%g_s%d_T%d_r%g_min%d_max%d" % ((k, B, n, L, glen, err, seed, T) + tuple(at_params))
 
 
 def _cov_reads(seed):
@@ -137,6 +162,31 @@ def test_oracle_vs_live_reference_early_tip_clipper(k, B, n, L, glen, err, seed,
     assert r["tc"]["removed"] > 0
 
 
+@pytest.mark.parametrize("k,B,seed,T", NL_CASES)
+def test_oracle_vs_live_reference_no_loops(k, B, seed, T):
+    """keep_perfect_loops = false: the unbranching paths of the reference's ExtractUnbranchingPaths, without the loops"""
+    reads = _nl_reads(seed)
+    art, r = oracle_artifacts(reads, k, B, keep_loops=False)
+    want = _recorded(_nl_id(k, B, seed, T))
+    got = graph_digests_of(art, B)
+    assert sorted(want) == sorted(got)
+    assert [key for key in want if want[key] != got[key]] == []
+    assert len(O.full_graph(reads, k, B)["unitigs"].seqs) > len(r["unitigs"].seqs)
+
+
+@pytest.mark.parametrize("k,B,n,L,glen,err,seed,T,at_params", AT_CASES)
+def test_oracle_vs_live_reference_early_at_clipper_parameters(k, B, n, L, glen, err, seed, T, at_params):
+    """EarlyLowComplexityClipperProcessor constructed with non-default ratio, min_length and max_length, then the tip clipper; the
+    parameters change the result against the pipeline's (0.8, 10, 200)"""
+    reads = at_reads(n, L, glen, err, seed)
+    art, r = oracle_artifacts(reads, k, B, early_tc=L - k, early_at=True, at_params=at_params)
+    want = _recorded(_at_id(k, B, n, L, glen, err, seed, T, at_params))
+    got = graph_digests_of(art, B)
+    assert sorted(want) == sorted(got)
+    assert [key for key in want if want[key] != got[key]] == []
+    assert r["at"][2] > 0 and r["at"] != O.full_graph(reads, k, B, early_tc=L - k, early_at=True)["at"]
+
+
 @pytest.mark.parametrize("k,thr,seed,T", COV_CASES)
 def test_oracle_vs_live_reference_coverage_prefilter(k, thr, seed, T):
     """SURVEY 8f-3: the CoverageFilter phase of the unmodified reference (HLL bound -> qf::cqf -> median filter, filled by T racing
@@ -168,6 +218,13 @@ def record():
         k, B, n, L, glen, err, seed, T = c
         g = run_probe("graph", _tc_reads(n, L, glen, err, seed), k, B, T=T, early_tc=L - k)
         out[_tc_id(*c)] = graph_digests_of_reference(g, graph_keys + ["tc_removed", "masks_raw"])
+    for k, B, seed, T in NL_CASES:
+        g = run_probe("graph", _nl_reads(seed), k, B, T=T, no_loops=True)
+        out[_nl_id(k, B, seed, T)] = graph_digests_of_reference(g, graph_keys)
+    for c in AT_CASES:
+        k, B, n, L, glen, err, seed, T, at_params = c
+        g = run_probe("graph", at_reads(n, L, glen, err, seed), k, B, T=T, early_tc=L - k, at_params=at_params)
+        out[_at_id(*c)] = graph_digests_of_reference(g, graph_keys + ["tc_removed", "at_removed"])
     for k, thr, seed, T in COV_CASES:
         with tempfile.TemporaryDirectory() as d:
             rf = os.path.join(d, "reads.txt")
