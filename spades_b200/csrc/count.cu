@@ -16,8 +16,6 @@
 //   C  local sort        : one CTA per segment: LSD radix sort in shared memory over the remaining key bits
 //      (optimistic 32-bit window + verification, full range on failure), run-length unique/count, written
 //      back in place; then a compaction copy into the dense bucket-major result.
-#include <time.h>
-
 #include <algorithm>
 #include <chrono>
 #include <memory>
@@ -1475,8 +1473,8 @@ struct Timer {
     float stop() { cudaEventRecord(b, s); cudaEventSynchronize(b); float ms = 0; cudaEventElapsedTime(&ms, a, b); return ms; }
 };
 
-// Environment, read ONCE per process and clamped to what the kernels support. User options: SGPU_ARENA_GB (sgpu_internal.h) and
-// SGPU_TRACE (per-phase wall clock on stderr). Tuning knobs kept for A/B runs on the GPU box:
+// Environment, read ONCE per process and clamped to what the kernels support. User options: SGPU_ARENA_GB and SGPU_TRACE
+// (sgpu_internal.h). Tuning knobs kept for A/B runs on the GPU box:
 //   SGPU_PA_MAX   level-A partitions for the whole job (default 4096; every (CTA, partition) pair is an open write stream)
 //   SGPU_RMAX     key bits per refinement round (default 11 = 2048 bins per CTA)
 //   SGPU_A_SUB    partition sub-ranges per level-A scatter pass (default 0 = automatic)
@@ -1484,7 +1482,6 @@ struct Tuning {
     uint32_t pa_max = 4096;
     uint32_t rmax = 11;
     int a_sub = 0;
-    bool trace = false;
 };
 static const Tuning &tuning() {
     static const Tuning t = [] {
@@ -1492,24 +1489,10 @@ static const Tuning &tuning() {
         if (const char *e = getenv("SGPU_PA_MAX")) x.pa_max = (uint32_t)std::min(8192, std::max(1, atoi(e)));
         if (const char *e = getenv("SGPU_RMAX")) x.rmax = (uint32_t)std::min(11, std::max(1, atoi(e)));
         if (const char *e = getenv("SGPU_A_SUB")) x.a_sub = std::min(64, std::max(0, atoi(e)));
-        x.trace = getenv("SGPU_TRACE") != nullptr;
         return x;
     }();
     return t;
 }
-
-struct Trace {
-    bool on; cudaStream_t st; double t0;
-    static double now() { struct timespec ts; clock_gettime(CLOCK_MONOTONIC, &ts); return ts.tv_sec * 1e3 + ts.tv_nsec * 1e-6; }
-    Trace(cudaStream_t s) : on(tuning().trace), st(s), t0(now()) {}
-    void mark(const char *what) {
-        if (!on) return;
-        cudaStreamSynchronize(st);
-        double t = now();
-        fprintf(stderr, "[sgpu-trace] %-28s %9.3f ms\n", what, t - t0);
-        t0 = t;
-    }
-};
 
 static int ilog2_floor(uint64_t v) { int r = 0; while (v >>= 1) ++r; return r; }
 
@@ -1728,16 +1711,20 @@ struct LevelAJob {
     std::vector<DArr<uint64_t>> tile_off; // per source: first id of every tile
     std::vector<DArr<uint16_t>> ids;      // per source: 2-byte partition id per record slot
     std::vector<uint64_t> h_part;         // host copy of part_total_all
-    ChunkStager *stage = nullptr;         // sources are the chunks of a host set: each launch reads the chunk's staged copy
-    // runs launch(src) for every non-empty source, in order; a staged source is uploaded behind the launches of the one before
+    ChunkStager *stage = nullptr;         // the set whose chunks are the sources (null for the reads): each launch reads what it hands over
+    // runs launch(si, src) for every non-empty source, in order; a host set's chunk is uploaded behind the launches of the one before
     template <class F>
     void for_each_src(F &&launch) const {
-        for (size_t si = 0; si < srcs.size(); ++si) {
-            Src src = srcs[si];
-            if (stage) stage->acquire(si, &src.words, nullptr);
-            if (src.n) launch(si, src);
-            if (stage) stage->release(si);
-        }
+        if (stage)
+            stage->sweep([&](const Chunk &ch, const uint64_t *keys, const uint32_t *) {
+                const size_t si = (size_t)(&ch - stage->ks->chunks.data());
+                Src src = srcs[si];
+                src.words = keys;
+                launch(si, src);
+            });
+        else
+            for (size_t si = 0; si < srcs.size(); ++si)
+                if (srcs[si].n) launch(si, srcs[si]);
     }
     uint64_t bucket_records(int b) const {
         uint64_t s = 0;
@@ -1904,7 +1891,7 @@ static void run_count(Ctx *ctx, const std::vector<Src> &srcs, int K, uint64_t es
     const size_t W = 8 * NW;
     cudaStream_t st = ctx->stream;
     Timer tm(st);
-    Trace tr(st);
+    Trace tr("sgpu count", st);
 
     // ---- level-A geometry for the whole job. Partition id = (bucket, top rA key bits). ONE histogram pass over the
     // source serves every bucket-group pass (the groups are contiguous partition ranges), so a multi-pass job hashes
@@ -2006,7 +1993,7 @@ KSet *count_from_reads(Ctx *ctx, int K, int B, int mode, bool result_on_host) {
     }
 }
 
-// one source per chunk of a (k+1)-mer set, read in place (a host set's chunks go through a ChunkStager)
+// one source per chunk of a (k+1)-mer set; the launches read the words a ChunkStager over the set hands over
 static std::vector<KmerSetSrc> kpomer_sources(const KSet *kp) {
     std::vector<KmerSetSrc> srcs;
     for (const Chunk &c : kp->chunks) {
@@ -2023,11 +2010,10 @@ static void check_kpomer_source(const KSet *kp) {
 template <int NW>
 static KSet *kmers_from_kpomers_nw(Ctx *ctx, const KSet *kp, int B, bool on_host) {
     const int K = kp->K - 1;
-    // a host (k+1)-mer set: every launch that reads a chunk's words reads its staged copy. Allocated before the passes are
-    // planned, so the planner sees the two staging buffers.
-    std::unique_ptr<ChunkStager> stage(kp->on_host ? new ChunkStager(kp, false) : nullptr);
+    // allocated before the passes are planned, so the planner sees a host set's two staging buffers
+    ChunkStager stage(kp, false);
     KSetBuilder set(ctx, K, NW, B, false, false, on_host);
-    run_count<NW, false>(ctx, kpomer_sources(kp), K, (uint64_t)kp->n * 2, set, stage.get());
+    run_count<NW, false>(ctx, kpomer_sources(kp), K, (uint64_t)kp->n * 2, set, &stage);
     return set.finish();
 }
 
@@ -2067,19 +2053,11 @@ void kset_checksum(const KSet *ks, uint64_t *out4) {
     Ctx *ctx = ks->ctx;
     DArr<unsigned long long> d(ctx, 4);
     SG_CUDA(cudaMemsetAsync(d.p, 0, 32, ctx->stream));
-    std::unique_ptr<ChunkStager> stage(ks->on_host ? new ChunkStager(ks, true) : nullptr);     // a host set streams through the device
-    for (size_t i = 0; i < ks->chunks.size(); ++i) {
-        const Chunk &c = ks->chunks[i];
-        const uint64_t *keys = c.keys.p;
-        const uint32_t *counts = ks->has_counts ? c.counts.p : nullptr;
-        if (stage) stage->acquire(i, &keys, &counts);
-        if (c.n) {
-            kset_checksum_k<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(keys, counts, (uint64_t)c.n, ks->nw, d.p);
-            ctx->launches++;
-        }
-        if (stage) stage->release(i);
-    }
-    SG_CUDA(cudaGetLastError());
+    ChunkStager stage(ks, true);                 // a host set streams through the device
+    stage.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *counts) {
+        kset_checksum_k<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(keys, counts, (uint64_t)c.n, ks->nw, d.p);
+        ctx->launches++;
+    });
     unsigned long long h[4];
     SG_CUDA(cudaMemcpyAsync(h, d.p, 32, cudaMemcpyDeviceToHost, ctx->stream));
     SG_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -2171,7 +2149,7 @@ struct DistState {
     DArr<uint64_t> pbase;                    // [G][max partitions of a pass]: piece starts of the current pass (peers read it)
     std::vector<PullSrc> peers;              // world entries (own entry = local pointers)
     std::unique_ptr<KSetBuilder> set;        // this rank's buckets, until sgpu_dist_end hands them over
-    std::unique_ptr<ChunkStager> stage;      // a host (k+1)-mer set: its chunks are uploaded for the histogram and for every scatter
+    std::unique_ptr<ChunkStager> stage;      // a (k+1)-mer source: the histogram and every scatter read its chunks through it
     virtual ~DistState() = default;
     virtual void begin() = 0;
     virtual void local_counts(uint64_t *h_out) = 0;
@@ -2256,7 +2234,7 @@ struct DistStateNW : DistState {
 
     void begin() override {
         Timer tm(ctx->stream);
-        Trace tr(ctx->stream);
+        Trace tr("sgpu count", ctx->stream);
         job.ctx = ctx; job.K = K; job.B = B; job.rA = plan.rA; job.G = G; job.stage = stage.get();
         job.s_lo = 0; job.s_hi = B; job.PA_all = plan.PA_all;
         levelA_count(job, tm, tr);
@@ -2267,7 +2245,7 @@ struct DistStateNW : DistState {
     void scatter(int p) override {
         // local partition of this rank's shard for the pass's buckets into the staging buffer (CTA-major pieces)
         Timer tm(ctx->stream);
-        Trace tr(ctx->stream);
+        Trace tr("sgpu count", ctx->stream);
         const int b_lo = plan.pass_lo(p), b_hi = plan.pass_lo(p + 1);
         uint64_t I = 0, total = 0;
         for (uint32_t q = 0; q < plan.PA_all; ++q) {
@@ -2329,7 +2307,7 @@ struct DistStateNW : DistState {
             SG_CUDA(cudaMemcpyAsync(d_tot.p, tot.data(), (size_t)(PA + 1) * 8, cudaMemcpyHostToDevice, st));
             SG_CUDA(cudaMemcpyAsync(d_start.p, start.data(), (size_t)(PA + 1) * 8, cudaMemcpyHostToDevice, st));
             Timer tm(st);
-            Trace tr(st);
+            Trace tr("sgpu count", st);
             sort_pass<NW>(ctx, K, xbuf, sbuf, d_start.p, d_tot.p, PA, plan.rA, (uint32_t)my_lo, my_hi, *set, tm, tr);
         } else {
             set->open(my_lo, my_hi, 0);          // nothing arrived: the pass still has its (empty) chunk
@@ -2352,10 +2330,10 @@ static DistState *dist_state_new(Ctx *ctx, int K, int mode) {
 template <int NW>
 static DistState *dist_state_kpomers(const KSet *kp) { return dist_state_of<NW, KmerSetSrc, false>(kpomer_sources(kp)); }
 
-// geometry, set and level-A histogram of a distributed count whose sources d already holds
-// (`counts`, `double_selfrc`: as KSetBuilder's); d is deleted on failure
+// geometry, set and level-A histogram of a distributed count whose sources d already holds (`counts`, `double_selfrc`: as
+// KSetBuilder's; `src_set`: the (k+1)-mer set whose chunks are the sources, null for the reads); d is deleted on failure
 static DistState *dist_start(DistState *d, Ctx *ctx, int K, int B, int world, int rank, bool counts, bool double_selfrc, bool result_on_host,
-                             const KSet *staged) {
+                             const KSet *src_set) {
     d->ctx = ctx; d->K = K; d->B = B; d->nw = nwords_of(K);
     d->G = ctx->num_sms * levelA_ctas_per_sm();
     // every rank must use the same geometry, so it depends on B only. As many level-A partitions as the shared-memory tables allow:
@@ -2366,7 +2344,7 @@ static DistState *dist_start(DistState *d, Ctx *ctx, int K, int B, int world, in
     ctx->times.level_a_key_bits = (uint64_t)rA;
     try {
         // a host source's staging buffers are allocated before the histogram, so sgpu_dist_free_bytes sees them from the first pass
-        if (staged) d->stage.reset(new ChunkStager(staged, false));
+        if (src_set) d->stage.reset(new ChunkStager(src_set, false));
         d->set.reset(new KSetBuilder(ctx, K, d->nw, B, counts, double_selfrc, result_on_host));
         d->begin();
     } catch (...) { delete d; throw; }
@@ -2409,7 +2387,7 @@ DistState *dist_begin_kpomers(Ctx *ctx, const KSet *kp, int B, int world, int ra
         case 3: d = dist_state_kpomers<3>(kp); break;
         default: d = dist_state_kpomers<4>(kp); break;
     }
-    return dist_start(d, ctx, K, B, world, rank, false, false, result_on_host, kp->on_host ? kp : nullptr);
+    return dist_start(d, ctx, K, B, world, rank, false, false, result_on_host, kp);
 }
 uint32_t dist_num_partitions(const DistState *d) { return d->plan.PA_all; }
 void dist_local_counts(DistState *d, uint64_t *h_out) { d->local_counts(h_out); }

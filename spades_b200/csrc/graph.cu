@@ -5,9 +5,8 @@
 //   UnbranchingPathExtractor (src/common/assembly_graph/construction/debruijn_graph_constructor.hpp:184-410)
 //   FastGraphFromSequencesConstructor::CollectLinkRecords (…:473-487) and GraphCoverageFiller (graph_support/coverage_filling.hpp:52-70)
 #include <algorithm>
-
-#include <chrono>
-#include <memory>
+#include <array>
+#include <optional>
 
 #include "graph.h"
 #include "mphf_dev.cuh"
@@ -683,27 +682,6 @@ __global__ void loop_write_k(const LoopInfo *__restrict__ info, int64_t nl, int 
 }
 
 // ---- host orchestration ----------------------------------------------------------------------------------------------
-// The chunks of a k-mer set, in order: a device set's own arrays, or a host set's chunks staged through two device buffers (each
-// sweep uploads the set once). Only the sweeps read the sets, so the graph needs the MPHFs, masks and coverage resident, not the sets.
-struct ChunkSource {
-    const KSet *ks;
-    std::unique_ptr<ChunkStager> stage;
-    ChunkSource(const KSet *s, bool counts) : ks(s), stage(s->on_host ? new ChunkStager(s, counts) : nullptr) {}
-    // f(chunk, keys, counts) for every non-empty chunk
-    template <class F>
-    void sweep(F &&f) {
-        for (size_t c = 0; c < ks->chunks.size(); ++c) {
-            const Chunk &ch = ks->chunks[c];
-            const uint64_t *keys = ch.keys.p;
-            const uint32_t *counts = ch.counts.p;
-            if (stage) stage->acquire(c, &keys, &counts);
-            if (ch.n) f(ch, keys, counts);
-            if (stage) stage->release(c);
-        }
-        SG_CUDA(cudaGetLastError());
-    }
-};
-
 // the keys of a sweep's flagged records, in final_kmers order, as one compacted list per chunk that has any (so they are never
 // held twice, as a join would)
 struct KeyParts {
@@ -711,9 +689,9 @@ struct KeyParts {
     std::vector<uint64_t> sizes;
     uint64_t total = 0;
 };
-// per chunk: flags -> scan -> compacted keys. flags(ch, keys, flag) fills flag[0, ch.n).
+// per chunk: flags -> scan -> compacted keys. flags(ch, keys, flag) launches one kernel that fills flag[0, ch.n).
 template <int NW, class Flags>
-static KeyParts collect_keys(Ctx *ctx, ChunkSource &src, Flags &&flags) {
+static KeyParts collect_keys(Ctx *ctx, ChunkStager &src, Flags &&flags) {
     cudaStream_t st = ctx->stream;
     int64_t mx = 1;
     for (const Chunk &c : src.ks->chunks) mx = std::max(mx, c.n);
@@ -723,6 +701,7 @@ static KeyParts collect_keys(Ctx *ctx, ChunkSource &src, Flags &&flags) {
     src.sweep([&](const Chunk &ch, const uint64_t *keys, const uint32_t *) {
         SG_CUDA(cudaMemsetAsync(flag.p + ch.n, 0, 4, st));
         flags(ch, keys, flag.p);
+        ctx->launches++;
         exclusive_scan_u32_to_u64(ctx, flag.p, pos.p, (size_t)ch.n + 1);
         uint64_t m = 0;
         SG_CUDA(cudaMemcpyAsync(&m, pos.p + ch.n, 8, cudaMemcpyDeviceToHost, st));
@@ -738,37 +717,66 @@ static KeyParts collect_keys(Ctx *ctx, ChunkSource &src, Flags &&flags) {
     return kp;
 }
 
-template <int NW, int NWS>
-static void graph_build_nw(Ctx *ctx, Graph *g, const GraphOptions &opt) {
-    const bool keep_loops = opt.keep_perfect_loops;
-    cudaStream_t st = ctx->stream;
-    const KSet *kp = g->kp, *km = g->km;
-    const int K = km->K;
-    const uint64_t nk = (uint64_t)km->n;
-    MphfDev mk = mphf_dev(g->mk);
-    // SGPU_TRACE: wall-clock milliseconds of the construction phases on stderr (synchronises the stream at every mark)
-    const bool trace = getenv("SGPU_TRACE") != nullptr;
-    auto t_prev = std::chrono::steady_clock::now();
-    auto trace_mark = [&](const char *what) {
-        if (!trace) return;
-        cudaStreamSynchronize(st);
-        const auto now = std::chrono::steady_clock::now();
-        fprintf(stderr, "[sgpu graph] %-28s %9.1f ms\n", what, std::chrono::duration<double, std::milli>(now - t_prev).count());
-        t_prev = now;
-    };
-    const bool have_cov = g->mkp && kp->has_counts;
-    MphfDev mkp = have_cov ? mphf_dev(g->mkp) : MphfDev();
-    // the resident state first, then the staging buffers of the two sets
-    g->masks.alloc(ctx, nk + 8, true);
-    SG_CUDA(cudaMemsetAsync(g->masks.p, 0, g->masks.bytes(), st));
-    if (have_cov) {
-        g->cov.alloc(ctx, (size_t)kp->n + 1, true);
-        SG_CUDA(cudaMemsetAsync(g->cov.p, 0, g->cov.bytes(), st));
+// the text, link records and raw coverage of a batch of edges, as the kernels write them (EdgeOut)
+struct EdgeBatch {
+    uint64_t n, bases;
+    DArr<char> seq;
+    DArr<uint64_t> link_start, link_end;
+    DArr<uint32_t> raw_cov;
+    EdgeBatch(Ctx *ctx, uint64_t n_, uint64_t bases_)
+        : n(n_), bases(bases_), seq(ctx, bases_ + 1), link_start(ctx, n_ + 1), link_end(ctx, n_ + 1), raw_cov(ctx, n_ + 1) {}
+    EdgeOut out(uint8_t *visited) const { return EdgeOut{seq.p, link_start.p, link_end.p, raw_cov.p, visited}; }
+    // appends the batch to g's edges. Its (offset, length) table has n entries, offsets into the batch's text, in device or host
+    // memory (cudaMemcpyDefault); the offsets are rebased onto g->seq.
+    void append(Graph *g, cudaStream_t st, const uint64_t *off, const uint32_t *len) const {
+        const size_t e0 = g->edge_len.size(), b0 = g->seq.size();
+        g->edge_off.resize(e0 + n); g->edge_len.resize(e0 + n);
+        g->link_start.resize(e0 + n); g->link_end.resize(e0 + n); g->raw_cov.resize(e0 + n);
+        g->seq.resize(b0 + bases);
+        if (n) {
+            SG_CUDA(cudaMemcpyAsync(g->edge_off.data() + e0, off, n * 8, cudaMemcpyDefault, st));
+            SG_CUDA(cudaMemcpyAsync(g->edge_len.data() + e0, len, n * 4, cudaMemcpyDefault, st));
+            SG_CUDA(cudaMemcpyAsync(g->link_start.data() + e0, link_start.p, n * 8, cudaMemcpyDeviceToHost, st));
+            SG_CUDA(cudaMemcpyAsync(g->link_end.data() + e0, link_end.p, n * 8, cudaMemcpyDeviceToHost, st));
+            SG_CUDA(cudaMemcpyAsync(g->raw_cov.data() + e0, raw_cov.p, n * 4, cudaMemcpyDeviceToHost, st));
+        }
+        if (bases) SG_CUDA(cudaMemcpyAsync(&g->seq[b0], seq.p, bases, cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaStreamSynchronize(st));
+        for (size_t e = e0; e < e0 + n; ++e) g->edge_off[e] += b0;
     }
-    // masks, and coverage in MPHF order: one sweep over the (k+1)-mers
-    {
-        ChunkSource kps(kp, have_cov);
-        kps.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *counts) {
+};
+
+// One graph construction: what its phases share (an aggregate: {ctx, g, opt} sets the rest). Only the sweeps read the two sets
+// (through a ChunkStager each), so the graph needs the MPHFs, masks and coverage resident, not the sets.
+template <int NW, int NWS>
+struct GraphBuild {
+    Ctx *ctx;
+    Graph *g;
+    const GraphOptions &opt;
+    cudaStream_t st = ctx->stream;
+    int K = g->km->K;
+    uint64_t nk = (uint64_t)g->km->n;
+    bool have_cov = g->mkp && g->kp->has_counts;      // without coverage, g->cov stays unallocated and the kernels get a null pointer
+    MphfDev mk = mphf_dev(g->mk), mkp = have_cov ? mphf_dev(g->mkp) : MphfDev();
+    std::optional<ChunkStager> kmers;                 // the k-mer set, for every sweep after the masks
+    DArr<uint8_t> visited;                            // per k-mer slot: on an edge already (from the unitigs through the loops)
+    Trace tr{"sgpu graph", st};
+    // kernel launches over every non-empty chunk of the k-mer set: launch(chunk, keys) launches one
+    template <class F>
+    void kmer_sweep(F &&launch) {
+        kmers->sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *) { launch(c, keys); ctx->launches++; });
+    }
+
+    // the masks, and the coverage in MPHF order: one sweep over the (k+1)-mers. The resident state first, then the staging
+    // buffers of the two sets, one after the other (the (k+1)-mers' stager is gone before the k-mers' is made).
+    void masks_coverage() {
+        g->masks.alloc(ctx, nk + 8, true);
+        SG_CUDA(cudaMemsetAsync(g->masks.p, 0, g->masks.bytes(), st));
+        if (have_cov) {
+            g->cov.alloc(ctx, (size_t)g->kp->n + 1, true);
+            SG_CUDA(cudaMemsetAsync(g->cov.p, 0, g->cov.bytes(), st));
+        }
+        ChunkStager(g->kp, have_cov).sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *counts) {
             masks_k<NW, NWS><<<div_up(c.n, 256), 256, 0, st>>>(keys, c.n, K, mk, reinterpret_cast<unsigned *>(g->masks.p));
             ctx->launches++;
             if (have_cov) {
@@ -776,14 +784,28 @@ static void graph_build_nw(Ctx *ctx, Graph *g, const GraphOptions &opt) {
                 ctx->launches++;
             }
         });
+        SG_CUDA(cudaStreamSynchronize(st));
+        tr.mark("masks + coverage");
+        kmers.emplace(g->km, false);
     }
-    SG_CUDA(cudaStreamSynchronize(st));
-    trace_mark("masks + coverage");
-    ChunkSource kms(km, false);
-    g->tc_stats[0] = g->tc_stats[1] = g->tc_stats[2] = 0;
-    for (int i = 0; i < 4; ++i) g->at_stats[i] = 0;
-    // the clippers probe every k-mer on a snapshot of the masks (one whole sweep) before any change is applied
-    if (opt.early_at && nk) {
+
+    // The clippers probe every k-mer on a snapshot of the masks (one whole sweep) before any change is applied. Their common
+    // tail: IsolateVertex for the marked k-mers, then one tc_links_k sweep (RemoveInconsistentForwardLinks) over the flagged
+    // (k-mer, orientation) pairs, which counts the clipped links in stats[links]. Returns the clipper's four counters.
+    std::array<unsigned long long, 4> isolate_and_unlink(const uint8_t *mark, const uint8_t *flags, int flags_by_slot, unsigned long long *stats, int links) {
+        tc_apply_k<<<div_up((int64_t)nk, 256), 256, 0, st>>>(g->masks.p, mark, nk);
+        ctx->launches++;
+        kmer_sweep([&](const Chunk &c, const uint64_t *keys) {
+            tc_links_k<NW><<<div_up(2 * c.n, 128), 128, 0, st>>>(keys, c.first, c.n, K, mk, g->masks.p, flags, stats + links, flags_by_slot);
+        });
+        std::array<unsigned long long, 4> hs;
+        SG_CUDA(cudaMemcpyAsync(hs.data(), stats, 32, cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaStreamSynchronize(st));
+        return hs;
+    }
+
+    void at_clipper() {
+        if (!opt.early_at || !nk) return;
         SG_CHECK(opt.at_min_len <= (uint64_t)K, 2, "early A/T clipper: min_length must not exceed k (the reference indexes kh[k - 1 - i])");
         AtParams ap; ap.ratio = opt.at_ratio; ap.min_len = (uint32_t)std::min<uint64_t>(opt.at_min_len, 0x7fffffffu); ap.max_len = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(opt.at_max_len, 1), 0x7fffffffu);
         DArr<uint8_t> eflag(ctx, 2 * nk + 8), mark(ctx, nk + 8);
@@ -792,206 +814,182 @@ static void graph_build_nw(Ctx *ctx, Graph *g, const GraphOptions &opt) {
         SG_CUDA(cudaMemsetAsync(mark.p, 0, mark.bytes(), st));
         SG_CUDA(cudaMemsetAsync(rooted.p, 0, rooted.bytes(), st));
         SG_CUDA(cudaMemsetAsync(stats.p, 0, 32, st));
-        kms.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *) {
+        kmer_sweep([&](const Chunk &c, const uint64_t *keys) {
             at_edges_probe_k<NW><<<div_up(2 * c.n, 128), 128, 0, st>>>(keys, c.n, K, mk, g->masks.p, ap, eflag.p, stats.p);
-            ctx->launches++;
         });
-        kms.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *) {
+        kmer_sweep([&](const Chunk &c, const uint64_t *keys) {
             at_edges_apply_k<NW><<<div_up(2 * c.n, 128), 128, 0, st>>>(keys, c.n, K, mk, g->masks.p, eflag.p, stats.p);
-            ctx->launches++;
         });
-        kms.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *) {
+        kmer_sweep([&](const Chunk &c, const uint64_t *keys) {
             at_tips_probe_k<NW><<<div_up(2 * c.n, 128), 128, 0, st>>>(keys, c.n, K, mk, g->masks.p, ap, mark.p, rooted.p, stats.p);
-            ctx->launches++;
         });
-        tc_apply_k<<<div_up((int64_t)nk, 256), 256, 0, st>>>(g->masks.p, mark.p, nk);
-        ctx->launches++;
-        kms.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *) {
-            tc_links_k<NW><<<div_up(2 * c.n, 128), 128, 0, st>>>(keys, c.first, c.n, K, mk, g->masks.p, rooted.p, stats.p + 3, 1);
-            ctx->launches++;
-        });
-        unsigned long long hs[4];
-        SG_CUDA(cudaMemcpyAsync(hs, stats.p, 32, cudaMemcpyDeviceToHost, st));
-        SG_CUDA(cudaStreamSynchronize(st));
+        const auto hs = isolate_and_unlink(mark.p, rooted.p, 1, stats.p, 3);
         for (int i = 0; i < 4; ++i) g->at_stats[i] = hs[i];
     }
-    const uint64_t early_tc_bound = opt.early_tip_length_bound;
-    if (early_tc_bound && nk) {
+
+    void tip_clipper() {
+        if (!opt.early_tip_length_bound || !nk) return;
         DArr<uint8_t> mark(ctx, nk + 8);
         DArr<uint8_t> tipped(ctx, 2 * nk + 8);
         DArr<unsigned long long> stats(ctx, 4);
         SG_CUDA(cudaMemsetAsync(mark.p, 0, mark.bytes(), st));
         SG_CUDA(cudaMemsetAsync(stats.p, 0, 32, st));
-        const uint32_t bound = (uint32_t)std::min<uint64_t>(early_tc_bound, 0x7fffffffu);
-        kms.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *) {
+        const uint32_t bound = (uint32_t)std::min<uint64_t>(opt.early_tip_length_bound, 0x7fffffffu);
+        kmer_sweep([&](const Chunk &c, const uint64_t *keys) {
             tc_probe_k<NW><<<div_up(2 * c.n, 128), 128, 0, st>>>(keys, c.first, c.n, K, mk, g->masks.p, bound, mark.p, tipped.p, stats.p);
-            ctx->launches++;
         });
-        tc_apply_k<<<div_up((int64_t)nk, 256), 256, 0, st>>>(g->masks.p, mark.p, nk);
-        ctx->launches++;
-        kms.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *) {
-            tc_links_k<NW><<<div_up(2 * c.n, 128), 128, 0, st>>>(keys, c.first, c.n, K, mk, g->masks.p, tipped.p, stats.p + 2, 0);
-            ctx->launches++;
-        });
-        unsigned long long hs[4];
-        SG_CUDA(cudaMemcpyAsync(hs, stats.p, 32, cudaMemcpyDeviceToHost, st));
-        SG_CUDA(cudaStreamSynchronize(st));
-        g->tc_stats[0] = hs[0]; g->tc_stats[1] = hs[1]; g->tc_stats[2] = hs[2];
+        const auto hs = isolate_and_unlink(mark.p, tipped.p, 0, stats.p, 2);
+        for (int i = 0; i < 3; ++i) g->tc_stats[i] = hs[i];
     }
-    g->masks_final.alloc(ctx, nk + 8, true);     // what the reference's ext index holds before unitig extraction mutates it
-    SG_CUDA(cudaMemcpyAsync(g->masks_final.p, g->masks.p, nk, cudaMemcpyDeviceToDevice, st));
-    if (nk == 0) { SG_CUDA(cudaStreamSynchronize(st)); return; }
 
-    trace_mark("early clippers");
-    // junction list: the junctions' keys in final_kmers order, so the unitig kernels never reach into the set
-    KeyParts jk = collect_keys<NW>(ctx, kms, [&](const Chunk &c, const uint64_t *keys, uint32_t *flag) {
-        junction_flags_k<NW><<<div_up(c.n, 256), 256, 0, st>>>(keys, c.n, K, mk, g->masks.p, flag);
-        ctx->launches++;
-    });
-    trace_mark("junction list");
+    // what the reference's extension index holds before the unitig extraction changes it
+    void final_masks() {
+        g->masks_final.alloc(ctx, nk + 8, true);
+        SG_CUDA(cudaMemcpyAsync(g->masks_final.p, g->masks.p, nk, cudaMemcpyDeviceToDevice, st));
+        tr.mark("early clippers");
+    }
+
+    // the junctions' keys in final_kmers order, so the unitig kernels never reach into the set
+    KeyParts junctions() {
+        KeyParts jk = collect_keys<NW>(ctx, *kmers, [&](const Chunk &c, const uint64_t *keys, uint32_t *flag) {
+            junction_flags_k<NW><<<div_up(c.n, 256), 256, 0, st>>>(keys, c.n, K, mk, g->masks.p, flag);
+        });
+        tr.mark("junction list");
+        return jk;
+    }
+
     // unbranching paths, in batches of junctions (never across two chunks' lists) sized from the room left: the 8 slots of a
     // junction cost len + keepf + selfc + eidx + eoff + the compacted (offset, length) = 37 bytes each. The unitig text and link
     // records of a batch depend on its paths' lengths, not on its junctions: they are reckoned at as much again, a heuristic, and a
     // batch whose text needs more still runs (blocks beyond the arena come from the driver). Edge numbers and text offsets carry
     // over from batch to batch.
-    DArr<uint8_t> visited(ctx, nk + 8);
-    SG_CUDA(cudaMemsetAsync(visited.p, 0, visited.bytes(), st));
-    const uint64_t per_junc = 2 * 8 * 37;
-    const uint64_t jbatch = std::max<uint64_t>(4096, ctx->budget_left() / 2 / per_junc);
-    g->edge_len.clear(); g->edge_off.clear(); g->seq.clear();
-    g->link_start.clear(); g->link_end.clear(); g->raw_cov.clear();
-    uint64_t batches = 0;
-    for (size_t part = 0; part < jk.parts.size(); ++part)
-    for (uint64_t q0 = 0, njunc = jk.sizes[part]; q0 < njunc; q0 += jbatch) {
-        const uint64_t nj = std::min(jbatch, njunc - q0);
-        const uint64_t nslots = nj * 8;
-        ++batches;
-        DArr<uint32_t> len(ctx, nslots + 1), keepf(ctx, nslots + 1);
-        DArr<uint8_t> selfc(ctx, nslots + 1);
-        DArr<uint64_t> eidx(ctx, nslots + 1), eoff(ctx, nslots + 1);
-        SG_CUDA(cudaMemsetAsync(len.p, 0, len.bytes(), st));
-        const uint64_t *bkeys = jk.parts[part].p + q0 * NW;
-        unitig_probe_k<NW><<<div_up((int64_t)nslots, 128), 128, 0, st>>>(bkeys, (int64_t)nj, K, mk, g->masks.p, nk, len.p, selfc.p);
-        ctx->launches++;
-        SG_CUDA(cudaGetLastError());
-        exclusive_scan_u32_to_u64(ctx, len.p, eoff.p, nslots + 1);
-        // edge index = rank among kept slots
-        launch_nonzero_flags(ctx, len.p, keepf.p, nslots + 1);
-        exclusive_scan_u32_to_u64(ctx, keepf.p, eidx.p, nslots + 1);
-        uint64_t npaths = 0, nbases = 0;
-        SG_CUDA(cudaMemcpyAsync(&npaths, eidx.p + nslots, 8, cudaMemcpyDeviceToHost, st));
-        SG_CUDA(cudaMemcpyAsync(&nbases, eoff.p + nslots, 8, cudaMemcpyDeviceToHost, st));
-        SG_CUDA(cudaStreamSynchronize(st));
-        trace_mark("unitig probe + offsets");
-        DArr<char> seq(ctx, nbases + 1);
-        DArr<uint64_t> ls(ctx, npaths + 1), le(ctx, npaths + 1);
-        DArr<uint32_t> rc(ctx, npaths + 1);
-        EdgeOut eo; eo.seq = seq.p; eo.link_start = ls.p; eo.link_end = le.p; eo.raw_cov = rc.p; eo.visited = visited.p;
-        unitig_write_k<NW, NWS><<<div_up((int64_t)nslots, 128), 128, 0, st>>>(bkeys, (int64_t)nj, K, mk, g->masks.p, nk, len.p, selfc.p, eidx.p,
-                                                                             eoff.p, mkp, have_cov ? g->cov.p : nullptr, eo);
-        ctx->launches++;
-        SG_CUDA(cudaGetLastError());
-        trace_mark("unitig write");
-        // download path edges: the (offset, length) table is compacted on the device (8 slots per junction, most of them empty)
-        DArr<uint64_t> c_off(ctx, npaths + 1);
-        DArr<uint32_t> c_len(ctx, npaths + 1);
-        edge_table_k<<<div_up((int64_t)nslots, 256), 256, 0, st>>>(len.p, eidx.p, eoff.p, (int64_t)nslots, c_off.p, c_len.p);
-        ctx->launches++;
-        const size_t e0 = g->edge_len.size(), b0 = g->seq.size();
-        g->edge_len.resize(e0 + npaths); g->edge_off.resize(e0 + npaths);
-        g->seq.resize(b0 + nbases);
-        g->link_start.resize(e0 + npaths); g->link_end.resize(e0 + npaths); g->raw_cov.resize(e0 + npaths);
-        if (npaths) {
-            SG_CUDA(cudaMemcpyAsync(g->edge_off.data() + e0, c_off.p, npaths * 8, cudaMemcpyDeviceToHost, st));
-            SG_CUDA(cudaMemcpyAsync(g->edge_len.data() + e0, c_len.p, npaths * 4, cudaMemcpyDeviceToHost, st));
-            SG_CUDA(cudaMemcpyAsync(g->link_start.data() + e0, ls.p, npaths * 8, cudaMemcpyDeviceToHost, st));
-            SG_CUDA(cudaMemcpyAsync(g->link_end.data() + e0, le.p, npaths * 8, cudaMemcpyDeviceToHost, st));
-            SG_CUDA(cudaMemcpyAsync(g->raw_cov.data() + e0, rc.p, npaths * 4, cudaMemcpyDeviceToHost, st));
+    void unitigs(KeyParts jk) {
+        visited.alloc(ctx, nk + 8);
+        SG_CUDA(cudaMemsetAsync(visited.p, 0, visited.bytes(), st));
+        const uint64_t per_junc = 2 * 8 * 37;
+        const uint64_t jbatch = std::max<uint64_t>(4096, ctx->budget_left() / 2 / per_junc);
+        uint64_t batches = 0;
+        for (size_t part = 0; part < jk.parts.size(); ++part)
+        for (uint64_t q0 = 0, njunc = jk.sizes[part]; q0 < njunc; q0 += jbatch) {
+            const uint64_t nj = std::min(jbatch, njunc - q0);
+            const uint64_t nslots = nj * 8;
+            ++batches;
+            DArr<uint32_t> len(ctx, nslots + 1), keepf(ctx, nslots + 1);
+            DArr<uint8_t> selfc(ctx, nslots + 1);
+            DArr<uint64_t> eidx(ctx, nslots + 1), eoff(ctx, nslots + 1);
+            SG_CUDA(cudaMemsetAsync(len.p, 0, len.bytes(), st));
+            const uint64_t *bkeys = jk.parts[part].p + q0 * NW;
+            unitig_probe_k<NW><<<div_up((int64_t)nslots, 128), 128, 0, st>>>(bkeys, (int64_t)nj, K, mk, g->masks.p, nk, len.p, selfc.p);
+            ctx->launches++;
+            SG_CUDA(cudaGetLastError());
+            exclusive_scan_u32_to_u64(ctx, len.p, eoff.p, nslots + 1);
+            // edge index = rank among kept slots
+            launch_nonzero_flags(ctx, len.p, keepf.p, nslots + 1);
+            exclusive_scan_u32_to_u64(ctx, keepf.p, eidx.p, nslots + 1);
+            uint64_t npaths = 0, nbases = 0;
+            SG_CUDA(cudaMemcpyAsync(&npaths, eidx.p + nslots, 8, cudaMemcpyDeviceToHost, st));
+            SG_CUDA(cudaMemcpyAsync(&nbases, eoff.p + nslots, 8, cudaMemcpyDeviceToHost, st));
+            SG_CUDA(cudaStreamSynchronize(st));
+            tr.mark("unitig probe + offsets");
+            EdgeBatch eb(ctx, npaths, nbases);
+            unitig_write_k<NW, NWS><<<div_up((int64_t)nslots, 128), 128, 0, st>>>(bkeys, (int64_t)nj, K, mk, g->masks.p, nk, len.p, selfc.p, eidx.p,
+                                                                                 eoff.p, mkp, g->cov.p, eb.out(visited.p));
+            ctx->launches++;
+            SG_CUDA(cudaGetLastError());
+            tr.mark("unitig write");
+            // the (offset, length) table is compacted on the device (8 slots per junction, most of them empty)
+            DArr<uint64_t> c_off(ctx, npaths + 1);
+            DArr<uint32_t> c_len(ctx, npaths + 1);
+            edge_table_k<<<div_up((int64_t)nslots, 256), 256, 0, st>>>(len.p, eidx.p, eoff.p, (int64_t)nslots, c_off.p, c_len.p);
+            ctx->launches++;
+            eb.append(g, st, c_off.p, c_len.p);
+            if (q0 + nj == njunc) jk.parts[part].release();
+            tr.mark("download + edge table");
         }
-        if (nbases) SG_CUDA(cudaMemcpyAsync(&g->seq[b0], seq.p, nbases, cudaMemcpyDeviceToHost, st));
-        SG_CUDA(cudaStreamSynchronize(st));
-        for (size_t e = e0; e < e0 + npaths; ++e) g->edge_off[e] += b0;
-        if (q0 + nj == njunc) jk.parts[part].release();
-        trace_mark("download + edge table");
+        ctx->times.graph_junction_batches = batches;
     }
-    ctx->times.graph_junction_batches = batches;
-    if (!keep_loops) return;
-    // ---- loops
-    DArr<unsigned long long> d_rem(ctx, 1);
-    SG_CUDA(cudaMemsetAsync(d_rem.p, 0, 8, st));
-    const uint64_t nwords = (nk + 31) / 32;
-    DArr<uint32_t> rem_bits(ctx, nwords + 1);
-    masks_clear_visited_k<<<div_up((int64_t)nk, 256), 256, 0, st>>>(g->masks.p, visited.p, nk, d_rem.p, rem_bits.p);
-    ctx->launches++;
-    unsigned long long rem = 0;
-    SG_CUDA(cudaMemcpyAsync(&rem, d_rem.p, 8, cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaStreamSynchronize(st));
-    if (!rem) return;
-    // final_kmers positions of the remaining slots only (RemSlots): the loop kernels never need 8 B per k-mer
-    DArr<uint64_t> rem_base(ctx, nwords + 1), rem_pos(ctx, rem);
-    {
-        DArr<uint32_t> cnt(ctx, nwords + 1);
-        SG_CUDA(cudaMemsetAsync(cnt.p + nwords, 0, 4, st));
-        popc_words_k<<<div_up((int64_t)nwords, 256), 256, 0, st>>>(rem_bits.p, nwords, cnt.p);
+
+    // perfect loops: the k-mers that are left with one edge in and one out once the paths are removed
+    void loops() {
+        DArr<unsigned long long> d_rem(ctx, 1);
+        SG_CUDA(cudaMemsetAsync(d_rem.p, 0, 8, st));
+        const uint64_t nwords = (nk + 31) / 32;
+        DArr<uint32_t> rem_bits(ctx, nwords + 1);
+        masks_clear_visited_k<<<div_up((int64_t)nk, 256), 256, 0, st>>>(g->masks.p, visited.p, nk, d_rem.p, rem_bits.p);
         ctx->launches++;
-        exclusive_scan_u32_to_u64(ctx, cnt.p, rem_base.p, nwords + 1);
+        unsigned long long rem = 0;
+        SG_CUDA(cudaMemcpyAsync(&rem, d_rem.p, 8, cudaMemcpyDeviceToHost, st));
         SG_CUDA(cudaStreamSynchronize(st));
+        if (!rem) return;
+        // final_kmers positions of the remaining slots only (RemSlots): the loop kernels never need 8 B per k-mer
+        DArr<uint64_t> rem_base(ctx, nwords + 1), rem_pos(ctx, rem);
+        {
+            DArr<uint32_t> cnt(ctx, nwords + 1);
+            SG_CUDA(cudaMemsetAsync(cnt.p + nwords, 0, 4, st));
+            popc_words_k<<<div_up((int64_t)nwords, 256), 256, 0, st>>>(rem_bits.p, nwords, cnt.p);
+            ctx->launches++;
+            exclusive_scan_u32_to_u64(ctx, cnt.p, rem_base.p, nwords + 1);
+            SG_CUDA(cudaStreamSynchronize(st));
+        }
+        RemSlots rs; rs.bits = rem_bits.p; rs.base = rem_base.p;
+        kmer_sweep([&](const Chunk &c, const uint64_t *keys) {
+            loop_pos_k<NW><<<div_up(c.n, 256), 256, 0, st>>>(keys, c.first, c.n, mk, rs, rem_pos.p);
+        });
+        KeyParts lk = collect_keys<NW>(ctx, *kmers, [&](const Chunk &c, const uint64_t *keys, uint32_t *flag) {
+            loop_leader_k<NW><<<div_up(c.n, 128), 128, 0, st>>>(keys, c.first, c.n, nk, K, mk, g->masks.p, rs, rem_pos.p, flag);
+        });
+        rem_pos.release(); rem_base.release(); rem_bits.release();
+        const uint64_t nl = lk.total;
+        if (!nl) return;
+        // the leaders as one list (loops are rare, a few keys)
+        DArr<uint64_t> leaders(ctx, (size_t)nl * NW);
+        for (size_t i = 0, at = 0; i < lk.parts.size(); at += lk.sizes[i], ++i)
+            SG_CUDA(cudaMemcpyAsync(leaders.p + at * NW, lk.parts[i].p, lk.sizes[i] * NW * 8, cudaMemcpyDeviceToDevice, st));
+        DArr<LoopInfo> info(ctx, nl);
+        DArr<uint32_t> llen(ctx, 2 * nl + 1), lkeep(ctx, 2 * nl + 1), sfull(ctx, nl + 1);
+        DArr<uint64_t> leidx(ctx, 2 * nl + 1), leoff(ctx, 2 * nl + 1), soff(ctx, nl + 1);
+        SG_CUDA(cudaMemsetAsync(llen.p, 0, llen.bytes(), st));
+        loop_probe_k<NW, NWS><<<div_up((int64_t)nl, 64), 64, 0, st>>>(leaders.p, (int64_t)nl, K, mk, g->masks.p, info.p, llen.p);
+        ctx->launches++;
+        launch_nonzero_flags(ctx, llen.p, lkeep.p, 2 * nl + 1);
+        exclusive_scan_u32_to_u64(ctx, llen.p, leoff.p, 2 * nl + 1);
+        exclusive_scan_u32_to_u64(ctx, lkeep.p, leidx.p, 2 * nl + 1);
+        std::vector<uint32_t> h_llen(2 * nl + 1);
+        std::vector<LoopInfo> h_info(nl);
+        uint64_t nledges = 0, nlbases = 0;
+        SG_CUDA(cudaMemcpyAsync(h_llen.data(), llen.p, (2 * nl + 1) * 4, cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaMemcpyAsync(h_info.data(), info.p, nl * sizeof(LoopInfo), cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaMemcpyAsync(&nledges, leidx.p + 2 * nl, 8, cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaMemcpyAsync(&nlbases, leoff.p + 2 * nl, 8, cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaStreamSynchronize(st));
+        std::vector<uint64_t> h_soff(nl + 1, 0);
+        for (uint64_t q = 0; q < nl; ++q) h_soff[q + 1] = h_soff[q] + (uint64_t)K + h_info[q].nverts;
+        SG_CUDA(cudaMemcpyAsync(soff.p, h_soff.data(), (nl + 1) * 8, cudaMemcpyHostToDevice, st));
+        DArr<char> scratch(ctx, h_soff[nl] + 1);
+        EdgeBatch eb(ctx, nledges, nlbases);
+        loop_write_k<NW, NWS><<<div_up((int64_t)nl, 64), 64, 0, st>>>(info.p, (int64_t)nl, K, mk, g->masks.p, llen.p, leidx.p, leoff.p, mkp,
+                                                                     g->cov.p, eb.out(visited.p), scratch.p, soff.p);
+        ctx->launches++;
+        SG_CUDA(cudaGetLastError());
+        // the (offset, length) table from the probe's lengths: a loop is one edge, or two where it splits
+        std::vector<uint64_t> off;
+        std::vector<uint32_t> len;
+        for (uint64_t i = 0, at = 0; i < 2 * nl; at += h_llen[i++])
+            if (h_llen[i]) { off.push_back(at); len.push_back(h_llen[i]); }
+        eb.append(g, st, off.data(), len.data());
     }
-    RemSlots rs; rs.bits = rem_bits.p; rs.base = rem_base.p;
-    kms.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *) {
-        loop_pos_k<NW><<<div_up(c.n, 256), 256, 0, st>>>(keys, c.first, c.n, mk, rs, rem_pos.p);
-        ctx->launches++;
-    });
-    KeyParts lk = collect_keys<NW>(ctx, kms, [&](const Chunk &c, const uint64_t *keys, uint32_t *flag) {
-        loop_leader_k<NW><<<div_up(c.n, 128), 128, 0, st>>>(keys, c.first, c.n, nk, K, mk, g->masks.p, rs, rem_pos.p, flag);
-        ctx->launches++;
-    });
-    rem_pos.release(); rem_base.release(); rem_bits.release();
-    const uint64_t nl = lk.total;
-    if (!nl) return;
-    // the leaders as one list (loops are rare, a few keys)
-    DArr<uint64_t> leaders(ctx, (size_t)nl * NW);
-    for (size_t i = 0, at = 0; i < lk.parts.size(); at += lk.sizes[i], ++i)
-        SG_CUDA(cudaMemcpyAsync(leaders.p + at * NW, lk.parts[i].p, lk.sizes[i] * NW * 8, cudaMemcpyDeviceToDevice, st));
-    DArr<LoopInfo> info(ctx, nl);
-    DArr<uint32_t> llen(ctx, 2 * nl + 1), lkeep(ctx, 2 * nl + 1), sfull(ctx, nl + 1);
-    DArr<uint64_t> leidx(ctx, 2 * nl + 1), leoff(ctx, 2 * nl + 1), soff(ctx, nl + 1);
-    SG_CUDA(cudaMemsetAsync(llen.p, 0, llen.bytes(), st));
-    loop_probe_k<NW, NWS><<<div_up((int64_t)nl, 64), 64, 0, st>>>(leaders.p, (int64_t)nl, K, mk, g->masks.p, info.p, llen.p);
-    ctx->launches++;
-    launch_nonzero_flags(ctx, llen.p, lkeep.p, 2 * nl + 1);
-    exclusive_scan_u32_to_u64(ctx, llen.p, leoff.p, 2 * nl + 1);
-    exclusive_scan_u32_to_u64(ctx, lkeep.p, leidx.p, 2 * nl + 1);
-    std::vector<uint32_t> h_llen(2 * nl + 1);
-    std::vector<LoopInfo> h_info(nl);
-    uint64_t nledges = 0, nlbases = 0;
-    SG_CUDA(cudaMemcpyAsync(h_llen.data(), llen.p, (2 * nl + 1) * 4, cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaMemcpyAsync(h_info.data(), info.p, nl * sizeof(LoopInfo), cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaMemcpyAsync(&nledges, leidx.p + 2 * nl, 8, cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaMemcpyAsync(&nlbases, leoff.p + 2 * nl, 8, cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaStreamSynchronize(st));
-    std::vector<uint64_t> h_soff(nl + 1, 0);
-    for (uint64_t q = 0; q < nl; ++q) h_soff[q + 1] = h_soff[q] + (uint64_t)K + h_info[q].nverts;
-    SG_CUDA(cudaMemcpyAsync(soff.p, h_soff.data(), (nl + 1) * 8, cudaMemcpyHostToDevice, st));
-    DArr<char> scratch(ctx, h_soff[nl] + 1), lseq(ctx, nlbases + 1);
-    DArr<uint64_t> lls(ctx, nledges + 1), lle(ctx, nledges + 1);
-    DArr<uint32_t> lrc(ctx, nledges + 1);
-    EdgeOut lo; lo.seq = lseq.p; lo.link_start = lls.p; lo.link_end = lle.p; lo.raw_cov = lrc.p; lo.visited = visited.p;
-    loop_write_k<NW, NWS><<<div_up((int64_t)nl, 64), 64, 0, st>>>(info.p, (int64_t)nl, K, mk, g->masks.p, llen.p, leidx.p, leoff.p, mkp,
-                                                                 have_cov ? g->cov.p : nullptr, lo, scratch.p, soff.p);
-    ctx->launches++;
-    SG_CUDA(cudaGetLastError());
-    const size_t base_edges = g->edge_len.size(), base_bases = g->seq.size();
-    g->seq.resize(base_bases + nlbases);
-    g->link_start.resize(base_edges + nledges); g->link_end.resize(base_edges + nledges); g->raw_cov.resize(base_edges + nledges);
-    SG_CUDA(cudaMemcpyAsync(&g->seq[base_bases], lseq.p, nlbases, cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaMemcpyAsync(g->link_start.data() + base_edges, lls.p, nledges * 8, cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaMemcpyAsync(g->link_end.data() + base_edges, lle.p, nledges * 8, cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaMemcpyAsync(g->raw_cov.data() + base_edges, lrc.p, nledges * 4, cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaStreamSynchronize(st));
-    uint64_t off = base_bases;
-    for (uint64_t i = 0; i < 2 * nl; ++i)
-        if (h_llen[i]) { g->edge_off.push_back(off); g->edge_len.push_back(h_llen[i]); off += h_llen[i]; }
+};
+
+template <int NW, int NWS>
+static void graph_build_nw(Ctx *ctx, Graph *g, const GraphOptions &opt) {
+    GraphBuild<NW, NWS> b{ctx, g, opt};
+    b.masks_coverage();
+    b.at_clipper();
+    b.tip_clipper();
+    b.final_masks();
+    if (!b.nk) return;
+    b.unitigs(b.junctions());
+    if (opt.keep_perfect_loops) b.loops();
 }
 
 __global__ void nonzero_flags_k(const uint32_t *__restrict__ in, uint32_t *__restrict__ out, uint64_t n) {

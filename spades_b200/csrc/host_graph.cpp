@@ -9,7 +9,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <chrono>
 #include <string>
 #include <thread>
 #include <vector>
@@ -39,14 +38,7 @@ inline void put_u(std::string &s, uint64_t v) {
 std::vector<std::string> graph_gfa_chunks(const Graph *g, const char *version) {
     const size_t E = g->edge_len.size();
     const int K = g->k;
-    const bool trace = getenv("SGPU_TRACE") != nullptr;
-    auto t_prev = std::chrono::steady_clock::now();
-    auto trace_mark = [&](const char *what) {
-        if (!trace) return;
-        const auto now = std::chrono::steady_clock::now();
-        fprintf(stderr, "[sgpu gfa]   %-28s %9.1f ms\n", what, std::chrono::duration<double, std::milli>(now - t_prev).count());
-        t_prev = now;
-    };
+    Trace tr("sgpu gfa");
     raw_vector<Rec> recs(2 * E);
     std::vector<uint8_t> selfc(E ? E : 1, 0);
     par_chunks(E, host_threads_for(E), [&](int, size_t lo, size_t hi) {
@@ -62,7 +54,7 @@ std::vector<std::string> graph_gfa_chunks(const Graph *g, const char *version) {
         if (ha != hb) return ha < hb;
         return a.edge_and_mask() < b.edge_and_mask();
     });
-    trace_mark("link records sorted");
+    tr.mark("link records sorted");
     // a vertex = a run of records with one k-mer index; the placeholder records of self-conjugate edges form no vertex
     auto group_start = [&](size_t i) {
         if (i != 0 && (recs[i].hm >> 2) == (recs[i - 1].hm >> 2)) return false;
@@ -133,7 +125,7 @@ std::vector<std::string> graph_gfa_chunks(const Graph *g, const char *version) {
             std::sort(lst.begin() + lst_off[2 * vn + 1], lst.begin() + lst_off[2 * vn + 2]);
         }
     });
-    trace_mark("vertices + edge lists");
+    tr.mark("vertices + edge lists");
     const int TE = host_threads_for(E);
     std::vector<std::string> chunks(1 + (size_t)TE + (size_t)TV);
     chunks[0] = std::string("H\tsp:Z:") + version + "\n";
@@ -176,7 +168,7 @@ std::vector<std::string> graph_gfa_chunks(const Graph *g, const char *version) {
             }
         }
     });
-    trace_mark("S and L lines");
+    tr.mark("S and L lines");
     return chunks;
 }
 

@@ -278,17 +278,11 @@ static void build_nw(Ctx *ctx, const KSet *ks, Mphf *m) {
     } else {
         // a host set is placed chunk by chunk (a chunk is a contiguous bucket range), each chunk uploaded while the one before is placed
         ChunkStager stage(ks, false);
-        for (size_t c = 0; c < ks->chunks.size(); ++c) {
-            const Chunk &ch = ks->chunks[c];
-            const uint64_t *keys = nullptr;
-            stage.acquire(c, &keys, nullptr);
-            if (ch.n) {
-                KeyTable t;
-                t.nchunks = 1; t.first[0] = 0; t.first[1] = ch.n; t.keys[0] = keys;
-                place(t, (uint64_t)ch.n, ch.b_lo, ch.b_hi);
-            }
-            stage.release(c);
-        }
+        stage.sweep([&](const Chunk &ch, const uint64_t *keys, const uint32_t *) {
+            KeyTable t;
+            t.nchunks = 1; t.first[0] = 0; t.first[1] = ch.n; t.keys[0] = keys;
+            place(t, (uint64_t)ch.n, ch.b_lo, ch.b_hi);
+        });
     }
     // ---- ranks
     DArr<uint32_t> pop(ctx, nblocks + 1);

@@ -7,6 +7,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <chrono>
 #include <iterator>
 #include <map>
 #include <stdexcept>
@@ -327,11 +328,11 @@ struct KSet {
     std::vector<int64_t> bstart;       // B+1 exclusive prefix (final_kmers order)
 };
 
-// Brings a host set's chunks to the device one at a time, double-buffered: chunk c + 1 is copied on the stager's own stream
-// while chunk c is used on the context's stream. acquire(c) makes chunk c readable by work enqueued next on ctx->stream; release(c)
-// marks the end of that work (the chunk's buffer may then take chunk c + 2). Chunks are acquired in order, 0 to the last, and a
-// sweep may start again at chunk 0. The uploads have a stream of their own so that they do not queue behind the result copies of
-// a count that writes to host memory (ResultSink, on ctx->copy).
+// A set's chunks on the device, in order. A device set's chunks are read in place, at no cost (no stream, event or buffer). A host
+// set's are brought over one at a time, double-buffered: chunk c + 1 is copied on the stager's own stream while chunk c is used on
+// the context's stream. acquire(c) makes chunk c readable by work enqueued next on ctx->stream; release(c) marks the end of that
+// work (the chunk's buffer may then take chunk c + 2). Chunks are acquired in order, 0 to the last, and a sweep may start again at
+// chunk 0. The uploads have a stream of their own so that they do not queue behind a host-memory count's result copies (ctx->copy).
 struct ChunkStager {
     Ctx *ctx;
     const KSet *ks;
@@ -341,6 +342,7 @@ struct ChunkStager {
     cudaStream_t up = nullptr;
     cudaEvent_t loaded[2] = {nullptr, nullptr}, used[2] = {nullptr, nullptr};
     ChunkStager(const KSet *s, bool counts_too) : ctx(s->ctx), ks(s), with_counts(counts_too && s->has_counts) {
+        if (!ks->on_host) return;
         size_t mx = 1;
         for (const Chunk &c : ks->chunks) mx = std::max(mx, (size_t)c.n);
         SG_CUDA(cudaStreamCreateWithFlags(&up, cudaStreamNonBlocking));
@@ -370,6 +372,11 @@ struct ChunkStager {
         SG_CUDA(cudaEventRecord(loaded[s], up));
     }
     void acquire(size_t c, const uint64_t **k, const uint32_t **cnt) {
+        if (!ks->on_host) {
+            *k = ks->chunks[c].keys.p;
+            if (cnt) *cnt = with_counts ? ks->chunks[c].counts.p : nullptr;
+            return;
+        }
         if (c == 0) prefetch(0);
         const int s = (int)(c & 1);
         SG_CUDA(cudaStreamWaitEvent(ctx->stream, loaded[s], 0));
@@ -377,7 +384,36 @@ struct ChunkStager {
         *k = keys[s].p;
         if (cnt) *cnt = with_counts ? counts[s].p : nullptr;
     }
-    void release(size_t c) { SG_CUDA(cudaEventRecord(used[c & 1], ctx->stream)); }
+    void release(size_t c) { if (ks->on_host) SG_CUDA(cudaEventRecord(used[c & 1], ctx->stream)); }
+    // f(chunk, keys, counts) for every non-empty chunk, in order; counts is null without them
+    template <class F>
+    void sweep(F &&f) {
+        for (size_t c = 0; c < ks->chunks.size(); ++c) {
+            const uint64_t *k = nullptr;
+            const uint32_t *cnt = nullptr;
+            acquire(c, &k, &cnt);
+            if (ks->chunks[c].n) f(ks->chunks[c], k, cnt);
+            release(c);
+        }
+        SG_CUDA(cudaGetLastError());
+    }
+};
+
+// SGPU_TRACE (user option, read once per process): wall-clock milliseconds between marks on stderr, one line per mark. A trace
+// given a stream (a context's is never null) waits for the work enqueued on it at every mark, so that a mark also times that work.
+struct Trace {
+    const char *label;
+    cudaStream_t st;
+    std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
+    explicit Trace(const char *l, cudaStream_t s = nullptr) : label(l), st(s) {}
+    void mark(const char *what) {
+        static const bool on = getenv("SGPU_TRACE") != nullptr;
+        if (!on) return;
+        if (st) cudaStreamSynchronize(st);
+        const auto t = std::chrono::steady_clock::now();
+        fprintf(stderr, "[%s] %-28s %9.3f ms\n", label, what, std::chrono::duration<double, std::milli>(t - t0).count());
+        t0 = t;
+    }
 };
 
 // boomphf-compatible index resident in HBM (one mphf per bucket, BooPHF.h / kmer_index.hpp)
