@@ -351,6 +351,43 @@ void sgpu_dist_cov_free(sgpu_dist_cov *d);
  * for a cardinality bound */
 int sgpu_dist_cov_layout_host(int world, uint64_t cardinality_bound, const uint64_t *keys, int64_t n, uint32_t *owners, uint64_t *slice_capacity);
 
+/* ---- multi-GPU extension masks and coverage (one process per GPU). Every rank brings its bucket-owned (k+1)-mer set (with
+ * multiplicities, from a distributed canonical count) and its index, and its bucket-owned k-mer set (from sgpu_dist_begin_kpomers)
+ * and its index; owners[b] is the rank whose k-mer set holds bucket b (every rank passes the same table). Each rank ends with its
+ * slices of what sgpu_graph_masks / _coverage / _histogram give on one GPU over the union (early clippers off): the masks of its
+ * k-mers and the coverage of its (k+1)-mers, both in the slot order of its own indexes (a key's slot in the union's index is the
+ * same rank inside its bucket, after the union's earlier buckets), and the histogram of its coverage slice (the union's histogram
+ * is the element-wise sum over the ranks). A (k+1)-mer's two mask bits usually belong to k-mers other ranks own: per pass, a range
+ * of destination buckets, every rank writes its contributions into a staging buffer grouped by owner, and every owner streams its
+ * pieces out of the peers' staging buffers (cudaIpc mappings of their arenas, as sgpu_dist_*) into its slice. The coverage needs
+ * no exchange and is filled by begin. kpomer_index = NULL: masks only; the (k+1)-mer sets may then overlap (the coverage needs
+ * every (k+1)-mer bucket on exactly one rank). The sets and indexes must stay alive until sgpu_dist_ext_free.
+ *   begin -> local_counts -> [all_gather counts] -> plan ->
+ *   repeat: free_bytes -> [all_reduce MIN] -> next_pass (-1 = done) -> ipc_handle -> [all_gather descriptors] -> open_peers ->
+ *           scatter [barrier] apply [barrier]
+ *   -> masks / coverage / histogram -> free */
+typedef struct sgpu_dist_ext sgpu_dist_ext;
+int sgpu_dist_ext_begin(sgpu_ctx *ctx, const sgpu_kset *kpomers, const sgpu_mphf *kpomer_index /* NULL: masks only */, const sgpu_kset *kmers,
+                        const sgpu_mphf *kmer_index, const int32_t *owners /* num_buckets */, int world, int rank, sgpu_dist_ext **out);
+int sgpu_dist_ext_local_counts(const sgpu_dist_ext *d, uint64_t *out);     /* num_buckets: this rank's contributions per destination bucket */
+int sgpu_dist_ext_plan(sgpu_dist_ext *d, const uint64_t *all_counts /* world x num_buckets, rank-major */, uint64_t *total_records);
+int sgpu_dist_ext_free_bytes(sgpu_dist_ext *d, uint64_t *out);
+int sgpu_dist_ext_next_pass(sgpu_dist_ext *d, uint64_t budget_bytes, int *pass);     /* budget: the MINIMUM of free_bytes over the ranks */
+int sgpu_dist_ext_ipc_handle(sgpu_dist_ext *d, uint8_t *out /* SGPU_IPC_BYTES */);
+int sgpu_dist_ext_open_peers(sgpu_dist_ext *d, const uint8_t *descriptors /* world x SGPU_IPC_BYTES, rank-major */);
+int sgpu_dist_ext_scatter(sgpu_dist_ext *d, int pass);
+int sgpu_dist_ext_apply(sgpu_dist_ext *d, int pass);
+int sgpu_dist_ext_masks(const sgpu_dist_ext *d, uint8_t *out, int64_t n);          /* n = this rank's k-mers */
+int sgpu_dist_ext_coverage(const sgpu_dist_ext *d, uint32_t *out, int64_t n);      /* n = this rank's (k+1)-mers */
+int64_t sgpu_dist_ext_histogram(const sgpu_dist_ext *d, uint64_t *out, int64_t cap);/* returns this rank's histogram length */
+/* milliseconds spent so far in: the contribution histogram, the scatters, the applies, the coverage fill, the coverage histogram */
+int sgpu_dist_ext_times(const sgpu_dist_ext *d, float *out5);
+void sgpu_dist_ext_free(sgpu_dist_ext *d);
+/* the pass plan alone (pure host arithmetic, no GPU), for a fixed budget and records of record_bytes: returns npass and fills
+ * pass_bounds[0..npass] and the most records any rank sends or any owner receives in one pass */
+int sgpu_dist_ext_plan_host(int world, int num_buckets, const int32_t *owners, const uint64_t *all_counts, uint64_t budget_bytes, int record_bytes,
+                            int *pass_bounds, uint64_t *max_records);
+
 /* self tests of the shared host/device arithmetic (tests only): op 0 = xxh3_64, 1 = xxh3_128 lo, 2 = xxh3_128 hi, 3 = bucket(arg),
  * 4 = is_minimal, 5.. = rc word j. keys: n records of ceil(K/32) words. on_device != 0 runs the same code in a kernel. */
 int sgpu_selftest(sgpu_ctx *ctx, int on_device, int op, int K, uint64_t arg, const uint64_t *keys, int64_t n, uint64_t *out);

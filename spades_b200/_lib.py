@@ -30,6 +30,9 @@ SYMBOLS = [
     "sgpu_dist_open_peers", "sgpu_dist_scatter", "sgpu_dist_exchange", "sgpu_dist_sort", "sgpu_dist_end", "sgpu_dist_free", "sgpu_dist_plan_host",
     "sgpu_dist_cov_begin", "sgpu_dist_cov_ipc_handle", "sgpu_dist_cov_open_peers", "sgpu_dist_cov_bound", "sgpu_dist_cov_fill", "sgpu_dist_cov_filter",
     "sgpu_dist_cov_free", "sgpu_dist_cov_layout_host",
+    "sgpu_dist_ext_begin", "sgpu_dist_ext_local_counts", "sgpu_dist_ext_plan", "sgpu_dist_ext_free_bytes", "sgpu_dist_ext_next_pass",
+    "sgpu_dist_ext_ipc_handle", "sgpu_dist_ext_open_peers", "sgpu_dist_ext_scatter", "sgpu_dist_ext_apply", "sgpu_dist_ext_masks",
+    "sgpu_dist_ext_coverage", "sgpu_dist_ext_histogram", "sgpu_dist_ext_times", "sgpu_dist_ext_free", "sgpu_dist_ext_plan_host",
     "sgpu_selftest",
 ]
 
@@ -165,6 +168,21 @@ def load():
     L.sgpu_dist_cov_filter.restype = i32; L.sgpu_dist_cov_filter.argtypes = [vp, i32, vp, vp]
     L.sgpu_dist_cov_free.restype = None; L.sgpu_dist_cov_free.argtypes = [vp]
     L.sgpu_dist_cov_layout_host.restype = i32; L.sgpu_dist_cov_layout_host.argtypes = [i32, u64, vp, i64, vp, C.POINTER(u64)]
+    L.sgpu_dist_ext_begin.restype = i32; L.sgpu_dist_ext_begin.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, pp]
+    L.sgpu_dist_ext_local_counts.restype = i32; L.sgpu_dist_ext_local_counts.argtypes = [vp, vp]
+    L.sgpu_dist_ext_plan.restype = i32; L.sgpu_dist_ext_plan.argtypes = [vp, vp, C.POINTER(u64)]
+    L.sgpu_dist_ext_free_bytes.restype = i32; L.sgpu_dist_ext_free_bytes.argtypes = [vp, C.POINTER(u64)]
+    L.sgpu_dist_ext_next_pass.restype = i32; L.sgpu_dist_ext_next_pass.argtypes = [vp, u64, C.POINTER(i32)]
+    L.sgpu_dist_ext_ipc_handle.restype = i32; L.sgpu_dist_ext_ipc_handle.argtypes = [vp, vp]
+    L.sgpu_dist_ext_open_peers.restype = i32; L.sgpu_dist_ext_open_peers.argtypes = [vp, vp]
+    L.sgpu_dist_ext_scatter.restype = i32; L.sgpu_dist_ext_scatter.argtypes = [vp, i32]
+    L.sgpu_dist_ext_apply.restype = i32; L.sgpu_dist_ext_apply.argtypes = [vp, i32]
+    L.sgpu_dist_ext_masks.restype = i32; L.sgpu_dist_ext_masks.argtypes = [vp, vp, i64]
+    L.sgpu_dist_ext_coverage.restype = i32; L.sgpu_dist_ext_coverage.argtypes = [vp, vp, i64]
+    L.sgpu_dist_ext_histogram.restype = i64; L.sgpu_dist_ext_histogram.argtypes = [vp, vp, i64]
+    L.sgpu_dist_ext_times.restype = i32; L.sgpu_dist_ext_times.argtypes = [vp, vp]
+    L.sgpu_dist_ext_free.restype = None; L.sgpu_dist_ext_free.argtypes = [vp]
+    L.sgpu_dist_ext_plan_host.restype = i32; L.sgpu_dist_ext_plan_host.argtypes = [i32, i32, vp, vp, u64, i32, vp, C.POINTER(u64)]
     L.sgpu_selftest.restype = i32; L.sgpu_selftest.argtypes = [vp, i32, i32, i32, u64, vp, i64, vp]
     _lib = L
     return L

@@ -717,6 +717,90 @@ int sgpu_dist_cov_layout_host(int world, uint64_t cardinality_bound, const uint6
 }
 }  // extern "C"
 
+struct sgpu_dist_ext { ExtDist *d; Ctx *c; };
+extern "C" {
+int sgpu_dist_ext_begin(sgpu_ctx *ctx, const sgpu_kset *kpomers, const sgpu_mphf *kpomer_index, const sgpu_kset *kmers, const sgpu_mphf *kmer_index,
+                        const int32_t *owners, int world, int rank, sgpu_dist_ext **out) {
+    if (!ctx || !kpomers || !kmers || !kmer_index || !owners || !out) return SGPU_EINVAL;
+    *out = nullptr;
+    Ctx *c = &ctx->c;
+    API_TRY(c, {
+        SG_CHECK(world >= 1 && world <= 255 && rank >= 0 && rank < world, SGPU_EINVAL, "bad world/rank");
+        SG_CHECK(!kpomers->free_pending && !kmers->free_pending, SGPU_EINVAL, "a k-mer set has been freed");
+        SG_CUDA(cudaSetDevice(c->device));
+        ExtDist *d = ext_begin(c, kpomers->s, kpomer_index ? kpomer_index->m : nullptr, kmers->s, kmer_index->m, owners, world, rank);
+        *out = new sgpu_dist_ext{d, c};
+        child_add(c);
+    })
+}
+int sgpu_dist_ext_local_counts(const sgpu_dist_ext *d, uint64_t *out) {
+    if (!d || !out) return SGPU_EINVAL;
+    API_TRY(d->c, ext_local_counts(d->d, out))
+}
+int sgpu_dist_ext_plan(sgpu_dist_ext *d, const uint64_t *all_counts, uint64_t *total_records) {
+    if (!d || !all_counts || !total_records) return SGPU_EINVAL;
+    API_TRY(d->c, ext_plan(d->d, all_counts, total_records))
+}
+int sgpu_dist_ext_free_bytes(sgpu_dist_ext *d, uint64_t *out) {
+    if (!d || !out) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); *out = ext_free_bytes(d->d); })
+}
+int sgpu_dist_ext_next_pass(sgpu_dist_ext *d, uint64_t budget_bytes, int *pass) {
+    if (!d || !pass) return SGPU_EINVAL;
+    *pass = -1;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); *pass = ext_next_pass(d->d, budget_bytes); })
+}
+int sgpu_dist_ext_ipc_handle(sgpu_dist_ext *d, uint8_t *out) {
+    if (!d || !out) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); ext_ipc_handle(d->d, out); })
+}
+int sgpu_dist_ext_open_peers(sgpu_dist_ext *d, const uint8_t *descriptors) {
+    if (!d || !descriptors) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); ext_open_peers(d->d, descriptors); })
+}
+int sgpu_dist_ext_scatter(sgpu_dist_ext *d, int pass) {
+    if (!d) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); ext_scatter(d->d, pass); })
+}
+int sgpu_dist_ext_apply(sgpu_dist_ext *d, int pass) {
+    if (!d) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); ext_apply(d->d, pass); })
+}
+int sgpu_dist_ext_masks(const sgpu_dist_ext *d, uint8_t *out, int64_t n) {
+    if (!d || (n && !out)) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); ext_masks(d->d, out, n); })
+}
+int sgpu_dist_ext_coverage(const sgpu_dist_ext *d, uint32_t *out, int64_t n) {
+    if (!d || (n && !out)) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); ext_coverage(d->d, out, n); })
+}
+int64_t sgpu_dist_ext_histogram(const sgpu_dist_ext *d, uint64_t *out, int64_t cap) {
+    if (!d) return -1;
+    const std::vector<uint64_t> &h = ext_histogram(d->d);
+    if (out) for (int64_t i = 0; i < (int64_t)h.size() && i < cap; ++i) out[i] = h[i];
+    return (int64_t)h.size();
+}
+int sgpu_dist_ext_times(const sgpu_dist_ext *d, float *out5) {
+    if (!d || !out5) return SGPU_EINVAL;
+    ext_times(d->d, out5);
+    return SGPU_OK;
+}
+void sgpu_dist_ext_free(sgpu_dist_ext *d) {
+    if (!d) return;
+    Ctx *c = d->c;
+    cudaSetDevice(c->device);
+    ext_free(d->d);
+    delete d;
+    child_release(c);
+}
+int sgpu_dist_ext_plan_host(int world, int num_buckets, const int32_t *owners, const uint64_t *all_counts, uint64_t budget_bytes, int record_bytes,
+                            int *pass_bounds, uint64_t *max_records) {
+    if (world < 1 || num_buckets < 1 || !owners || !all_counts || !pass_bounds || !max_records) return -1;
+    try { return ext_plan_host(world, num_buckets, owners, all_counts, budget_bytes, record_bytes, pass_bounds, max_records); }
+    catch (...) { return -1; }
+}
+}  // extern "C"
+
 // ---- self test of kmer_dev.cuh on host and device -----------------------------------------------------------------------
 template <int NW>
 __host__ __device__ uint64_t selftest_one(int op, int K, uint64_t arg, const uint64_t *key) {

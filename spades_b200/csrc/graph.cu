@@ -9,6 +9,7 @@
 #include <optional>
 
 #include "graph.h"
+#include "masks_dev.cuh"
 #include "mphf_dev.cuh"
 
 namespace sg {
@@ -67,16 +68,15 @@ __global__ void masks_k(const uint64_t *__restrict__ kp, int64_t n, int K, MphfD
     Kmer<NWS> x;
 #pragma unroll
     for (int q = 0; q < NWS; ++q) x.w[q] = kp[i * NWS + q];
-    const int pnucl = (int)(x.w[0] & 3), nnucl = kmer_nuc<NWS>(x, K);          // kpomer[0], kpomer[K]
+    const int pnucl = kpomer_side_nucl<1, NWS>(x, K), nnucl = kpomer_side_nucl<0, NWS>(x, K);
+    auto slot = [&](const Kmer<NW> &key) { return mphf_lookup_dev<NW>(mk, key); };
     {
-        CanonIdx<NW> c = canon_lookup<NW>(mk, kmer_prefix<NW, NWS>(x, K), K);   // AddOutgoing(prefix, nnucl)
-        const unsigned bit = 1u << (c.is_min ? nnucl : 7 - nnucl);
-        atomicOr(&masks32[c.idx >> 2], bit << (8 * (c.idx & 3)));
+        const auto c = kpomer_side<0, NW, NWS>(x, K, slot);                       // AddOutgoing(prefix, nnucl)
+        mask_or(masks32, c.value, mask_bit<0>(c.is_min, nnucl));
     }
     {
-        CanonIdx<NW> c = canon_lookup<NW>(mk, kmer_suffix<NW, NWS>(x, K), K);   // AddIncoming(suffix, pnucl)
-        const unsigned bit = 1u << (c.is_min ? pnucl + 4 : 3 - pnucl);
-        atomicOr(&masks32[c.idx >> 2], bit << (8 * (c.idx & 3)));
+        const auto c = kpomer_side<1, NW, NWS>(x, K, slot);                       // AddIncoming(suffix, pnucl)
+        mask_or(masks32, c.value, mask_bit<1>(c.is_min, pnucl));
     }
 }
 
@@ -1025,19 +1025,38 @@ Graph *graph_build(Ctx *ctx, const KSet *kp, const KSet *km, const Mphf *mk, con
 }
 
 std::vector<uint64_t> graph_histogram(Ctx *ctx, const Graph *g) {
+    if (!g->cov.p) return {};
+    return coverage_histogram(ctx, g->cov.p, g->kp->n);
+}
+
+void coverage_fill(Ctx *ctx, ChunkStager &kpomers, const Mphf *mkp, uint32_t *cov) {
+    SG_CHECK(kpomers.with_counts, 2, "coverage: the (k+1)-mer set carries no multiplicities");
+    const MphfDev m = mphf_dev(mkp);
+    const int nws = kpomers.ks->nw;
+    kpomers.sweep([&](const Chunk &c, const uint64_t *keys, const uint32_t *counts) {
+        const int grid = div_up(c.n, 256);
+        if (nws == 1) cov_perm_k<1><<<grid, 256, 0, ctx->stream>>>(keys, counts, c.n, m, cov);
+        else if (nws == 2) cov_perm_k<2><<<grid, 256, 0, ctx->stream>>>(keys, counts, c.n, m, cov);
+        else if (nws == 3) cov_perm_k<3><<<grid, 256, 0, ctx->stream>>>(keys, counts, c.n, m, cov);
+        else cov_perm_k<4><<<grid, 256, 0, ctx->stream>>>(keys, counts, c.n, m, cov);
+        ctx->launches++;
+    });
+    SG_CUDA(cudaStreamSynchronize(ctx->stream));
+}
+
+std::vector<uint64_t> coverage_histogram(Ctx *ctx, const uint32_t *cov, int64_t n) {
     std::vector<uint64_t> h;
-    const int64_t n = g->kp->n;
-    if (!g->cov.p || n == 0) return h;
+    if (n == 0) return h;
     DArr<unsigned> mx(ctx, 1);
     SG_CUDA(cudaMemsetAsync(mx.p, 0, 4, ctx->stream));
-    hist_max_k<<<ctx->num_sms * 4, 256, 0, ctx->stream>>>(g->cov.p, n, mx.p);
+    hist_max_k<<<ctx->num_sms * 4, 256, 0, ctx->stream>>>(cov, n, mx.p);
     unsigned m = 0;
     SG_CUDA(cudaMemcpyAsync(&m, mx.p, 4, cudaMemcpyDeviceToHost, ctx->stream));
     SG_CUDA(cudaStreamSynchronize(ctx->stream));
     if (!m) return h;
     DArr<unsigned long long> dh(ctx, m);
     SG_CUDA(cudaMemsetAsync(dh.p, 0, dh.bytes(), ctx->stream));
-    hist_fill_k<<<ctx->num_sms * 4, 256, 0, ctx->stream>>>(g->cov.p, n, dh.p);
+    hist_fill_k<<<ctx->num_sms * 4, 256, 0, ctx->stream>>>(cov, n, dh.p);
     ctx->launches += 2;
     h.resize(m);
     SG_CUDA(cudaMemcpyAsync(h.data(), dh.p, (size_t)m * 8, cudaMemcpyDeviceToHost, ctx->stream));

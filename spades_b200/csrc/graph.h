@@ -35,6 +35,10 @@ struct GraphOptions {
 
 Graph *graph_build(Ctx *ctx, const KSet *kp, const KSet *km, const Mphf *mk, const Mphf *mkp, const GraphOptions &opt);
 std::vector<uint64_t> graph_histogram(Ctx *ctx, const Graph *g);
+// the same two steps outside a graph build: cov[mphf(kpomer)] = multiplicity over a sweep of the (k+1)-mers (cov zeroed by the
+// caller, one entry per key of the index), and the histogram of n coverage values (hist[c - 1] += 2, as long as the largest c)
+void coverage_fill(Ctx *ctx, ChunkStager &kpomers, const Mphf *mkp, uint32_t *cov);
+std::vector<uint64_t> coverage_histogram(Ctx *ctx, const uint32_t *cov, int64_t n);
 
 // edge_index.cu : KmerFreeEdgeIndex refill over the graph's own unitigs (alignment/edge_index.hpp, assembly_graph/index/edge_index_builders.hpp)
 struct EdgeIndex {

@@ -483,6 +483,25 @@ void dist_free(DistState *d);
 // pure host planning (exported for CPU tests): returns npass, fills pass boundaries / owner boundaries / totals
 int dist_plan_host(int world, int B, int rA, const uint64_t *cnt_all, uint64_t budget_bytes, int record_bytes, int *pass_b /*B+1 max*/, uint64_t *max_recv);
 
+// distributed extension masks, coverage and histogram (dist_ext.cu); owner: the rank owning each k-mer bucket (B entries)
+struct ExtDist;
+ExtDist *ext_begin(Ctx *ctx, const KSet *kp, const Mphf *mkp, const KSet *km, const Mphf *mk, const int *owner, int world, int rank);
+void ext_local_counts(const ExtDist *d, uint64_t *out);
+void ext_plan(ExtDist *d, const uint64_t *cnt_all, uint64_t *total);
+uint64_t ext_free_bytes(ExtDist *d);
+int ext_next_pass(ExtDist *d, uint64_t budget_bytes);
+void ext_ipc_handle(ExtDist *d, uint8_t *out96);
+void ext_open_peers(ExtDist *d, const uint8_t *descs);
+void ext_scatter(ExtDist *d, int p);
+void ext_apply(ExtDist *d, int p);
+void ext_masks(const ExtDist *d, uint8_t *out, int64_t n);
+void ext_coverage(const ExtDist *d, uint32_t *out, int64_t n);
+const std::vector<uint64_t> &ext_histogram(const ExtDist *d);
+void ext_times(const ExtDist *d, float *out5);
+void ext_free(ExtDist *d);
+// pure host planning (exported for CPU tests): returns npass, fills the pass boundaries and the most records of a pass
+int ext_plan_host(int world, int B, const int *owner, const uint64_t *cnt_all, uint64_t budget_bytes, int record_bytes, int *pass_b /*B+1 max*/, uint64_t *most);
+
 // mphf.cu
 Mphf *mphf_build(Ctx *ctx, const KSet *ks);
 size_t mphf_serialized_size(const Mphf *m);

@@ -8,7 +8,7 @@ import ctypes as C
 
 import numpy as np
 
-from .kmer_index import KMerDiskStorage, SGPU_CANONICAL, SGPU_RESULT_ON_HOST
+from .kmer_index import KMerDiskStorage, SGPU_CANONICAL, SGPU_RESULT_ON_HOST, _p
 
 SGPU_IPC_BYTES = 96
 
@@ -18,49 +18,87 @@ def _backend_device(group):
     return "cuda" if dist.get_backend(group) == "nccl" else "cpu"
 
 
+def _pass_budget(ctx, group, free_bytes, budget_bytes):
+    """the budget of the next pass: 90 % of the least any rank of `group` can allocate now (free_bytes(c_uint64 pointer) reads this
+    rank's), or a fixed budget_bytes (tests)"""
+    import torch
+    import torch.distributed as dist
+    if budget_bytes is not None:
+        return int(budget_bytes)
+    fb = C.c_uint64()
+    ctx.check(free_bytes(C.byref(fb)))
+    tb = torch.tensor([fb.value], dtype=torch.int64, device=_backend_device(group))
+    dist.all_reduce(tb, op=dist.ReduceOp.MIN, group=group)
+    return int(int(tb.item()) * 0.90)
+
+
+def _open_peers(ctx, group, ipc_handle, open_peers):
+    """all_gather of the ranks' SGPU_IPC_BYTES descriptors (ipc_handle(out) writes this rank's), handed to open_peers(descriptors)"""
+    import torch
+    import torch.distributed as dist
+    desc = np.zeros(SGPU_IPC_BYTES, np.uint8)
+    ctx.check(ipc_handle(desc.ctypes.data_as(C.c_void_p)))
+    t_h = torch.from_numpy(desc).to(_backend_device(group))
+    hs = [torch.empty_like(t_h) for _ in range(dist.get_world_size(group))]
+    dist.all_gather(hs, t_h, group=group)
+    descs = np.ascontiguousarray(torch.stack(hs).cpu().numpy())
+    ctx.check(open_peers(descs.ctypes.data_as(C.c_void_p)))
+
+
+def _all_gather_u64(local, group):
+    """world x len(local) table of every rank's u64 row"""
+    import torch
+    import torch.distributed as dist
+    t = torch.from_numpy(np.ascontiguousarray(local, np.uint64).view(np.int64)).to(_backend_device(group))
+    rows = [torch.empty_like(t) for _ in range(dist.get_world_size(group))]
+    dist.all_gather(rows, t, group=group)
+    return np.ascontiguousarray(torch.stack(rows).cpu().numpy().view(np.uint64))
+
+
+def _ownership(storage, group):
+    """(world x B bucket sizes, world x B owned flags) of the ranks' sets"""
+    import torch
+    import torch.distributed as dist
+    B = storage.num_buckets()
+    mine = torch.from_numpy(np.concatenate([storage.bucket_sizes(), storage.owned_buckets().astype(np.int64)])).to(_backend_device(group))
+    allv = [torch.empty_like(mine) for _ in range(dist.get_world_size(group))]
+    dist.all_gather(allv, mine, group=group)
+    allv = torch.stack(allv).cpu().numpy()
+    return allv[:, :B], allv[:, B:].astype(bool)
+
+
+def _check_owned_once(bsz_all, owned_all, what="k-mer"):
+    if not (owned_all.sum(axis=0) == 1).all():
+        raise ValueError("every %s bucket must be owned by exactly one rank (sets from one distributed count)" % what)
+    if (bsz_all[~owned_all] != 0).any():
+        raise ValueError("a rank holds %ss of a bucket it does not own" % what)
+
+
 def _distributed_count(ctx, group, begin, budget_bytes):
     """the pass loop of a distributed count over the ranks of `group`: begin(world, rank, handle pointer) starts it (sgpu_dist_begin
     or sgpu_dist_begin_kpomers); returns (this rank's KMerDiskStorage, passes)"""
-    import torch
     import torch.distributed as dist
     L = ctx.L
     world, rank = dist.get_world_size(group), dist.get_rank(group)
-    backend_dev = _backend_device(group)
     h = C.c_void_p()
     ctx.check(begin(world, rank, C.byref(h)))
     try:
         npart = L.sgpu_dist_num_partitions(h)
         local = np.zeros(npart, np.uint64)
         ctx.check(L.sgpu_dist_local_counts(h, local.ctypes.data_as(C.c_void_p)))
-        # all_gather of the per-partition record counts (world x npart x 8 bytes: small)
-        t_local = torch.from_numpy(local.view(np.int64)).to(backend_dev)
-        gathered = [torch.empty_like(t_local) for _ in range(world)]
-        dist.all_gather(gathered, t_local, group=group)
-        all_counts = np.ascontiguousarray(torch.stack(gathered).cpu().numpy().view(np.uint64))
+        all_counts = _all_gather_u64(local, group)     # the per-partition record counts (world x npart x 8 bytes: small)
         total = C.c_uint64()
         ctx.check(L.sgpu_dist_plan(h, all_counts.ctypes.data_as(C.c_void_p), C.byref(total)))
         npass = 0
         while True:
             # every pass is planned against what ALL ranks can allocate right now (earlier passes' outputs are resident)
-            if budget_bytes is None:
-                fb = C.c_uint64()
-                ctx.check(L.sgpu_dist_free_bytes(h, C.byref(fb)))
-                tb = torch.tensor([fb.value], dtype=torch.int64, device=backend_dev)
-                dist.all_reduce(tb, op=dist.ReduceOp.MIN, group=group)
-                budget = int(int(tb.item()) * 0.90)
-            else:
-                budget = int(budget_bytes)                 # tests: a fixed per-pass budget
+            budget = _pass_budget(ctx, group, lambda fb: L.sgpu_dist_free_bytes(h, fb), budget_bytes)
             p = C.c_int()
             ctx.check(L.sgpu_dist_next_pass(h, budget, C.byref(p)))
             if p.value < 0:
                 break
-            desc = np.zeros(SGPU_IPC_BYTES, np.uint8)
-            ctx.check(L.sgpu_dist_ipc_handle(h, desc.ctypes.data_as(C.c_void_p)))
-            t_h = torch.from_numpy(desc).to(backend_dev)
-            hs = [torch.empty_like(t_h) for _ in range(world)]
-            dist.all_gather(hs, t_h, group=group)
-            descs = np.ascontiguousarray(torch.stack(hs).cpu().numpy())
-            ctx.check(L.sgpu_dist_open_peers(h, descs.ctypes.data_as(C.c_void_p)))     # peers' arenas are mapped once per process
+            # peers' arenas are mapped once per process
+            _open_peers(ctx, group, lambda out: L.sgpu_dist_ipc_handle(h, out), lambda descs: L.sgpu_dist_open_peers(h, descs))
             ctx.check(L.sgpu_dist_scatter(h, p.value))    # local partition into the staging buffer
             dist.barrier(group=group)                     # every rank's staging buffer is complete
             ctx.check(L.sgpu_dist_exchange(h, p.value))   # one kernel: pull my pieces from all peers over NVLink + merge
@@ -127,20 +165,11 @@ def assemble_kmer_index(ctx, storage, mphf, group=None):
     count) and its index (`mphf`, KMerIndexBuilder.BuildIndex of it). A bucket's bytes depend on its own keys only, so each owner
     sends the serialized bytes of the buckets it owns; rank 0 writes num_segments, every bucket's bytes in bucket order and the
     segment_starts of the union's bucket sizes. Returns the bytes on rank 0, None elsewhere."""
-    import torch
     import torch.distributed as dist
     world, rank = dist.get_world_size(group), dist.get_rank(group)
-    backend_dev = _backend_device(group)
     B = storage.num_buckets()
-    mine = torch.from_numpy(np.concatenate([storage.bucket_sizes(), storage.owned_buckets().astype(np.int64)])).to(backend_dev)
-    allv = [torch.empty_like(mine) for _ in range(world)]
-    dist.all_gather(allv, mine, group=group)
-    allv = torch.stack(allv).cpu().numpy()
-    bsz_all, owned_all = allv[:, :B], allv[:, B:].astype(bool)
-    if not (owned_all.sum(axis=0) == 1).all():
-        raise ValueError("every bucket must be owned by exactly one rank (sets from one distributed count)")
-    if (bsz_all[~owned_all] != 0).any():
-        raise ValueError("a rank holds records of a bucket it does not own")
+    bsz_all, owned_all = _ownership(storage, group)
+    _check_owned_once(bsz_all, owned_all)
     own = owned_all[rank]
     runs, b = [], 0
     while b < B:                     # the serialized bytes of every maximal run of owned buckets
@@ -165,6 +194,158 @@ def assemble_kmer_index(ctx, storage, mphf, group=None):
     return np.uint64(B).tobytes() + b"".join(body) + starts.tobytes()
 
 
+class DistributedExtensionIndex:
+    """this rank's share of the union's extension masks and coverage (DistributedExtensionIndexBuilder.Build)"""
+
+    def __init__(self, ctx, h, kpomers, kmers, with_coverage):
+        self.ctx, self.h, self.kpomers, self.kmers, self.with_coverage = ctx, h, kpomers, kmers, with_coverage
+        self.npass = 0
+        self.local_counts = None          # this rank's mask contributions per destination k-mer bucket
+        self._hist = np.zeros(0, np.uint64)
+
+    def masks(self):
+        """the masks of this rank's k-mers, in the slot order of its k-mer index"""
+        n = self.kmers.total_kmers()
+        out = np.zeros(max(n, 1), np.uint8)
+        self.ctx.check(self.ctx.L.sgpu_dist_ext_masks(self.h, _p(out), n))
+        return out[:n]
+
+    def coverage(self):
+        """the multiplicities of this rank's (k+1)-mers, in the slot order of its (k+1)-mer index"""
+        n = self.kpomers.total_kmers()
+        out = np.zeros(max(n, 1), np.uint32)
+        self.ctx.check(self.ctx.L.sgpu_dist_ext_coverage(self.h, _p(out), n))
+        return out[:n]
+
+    def histogram(self):
+        """the union's coverage histogram (DeBruijnGraph.histogram of one GPU over the union)"""
+        if not self.with_coverage:
+            raise ValueError("built without a (k+1)-mer index: no coverage")
+        return self._hist.copy()
+
+    def times(self):
+        """milliseconds of this rank's contribution histogram, scatters, applies, coverage fill and coverage histogram"""
+        out = np.zeros(5, np.float32)
+        self.ctx.check(self.ctx.L.sgpu_dist_ext_times(self.h, _p(out)))
+        return dict(zip(("histogram", "scatter", "apply", "coverage", "coverage_histogram"), (float(x) for x in out)))
+
+    def free(self):
+        if self.h:
+            self.ctx.L.sgpu_dist_ext_free(self.h); self.h = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+class DistributedExtensionIndexBuilder:
+    """DeBruijnExtensionIndexBuilder and the coverage fill across the ranks of a torch.distributed process group. Every rank brings
+    its bucket-owned (k+1)-mer set with multiplicities (its shard of a DistributedKMerCounter count) and that set's index, and its
+    bucket-owned k-mer set (DistributedKmersFromKpomers) and that set's index. Build gives every rank the masks of the k-mers it
+    owns and the coverage of the (k+1)-mers it owns, each in its own indexes' slot order, and the union's histogram: what one GPU
+    computes over the union (assemble_masks / assemble_coverage lay the slices out in the union's order). kpomer_index=None builds
+    the masks only; the (k+1)-mer sets may then overlap. The sets and indexes must not be freed before the result."""
+
+    def __init__(self, ctx, kpomers, kpomer_index, kmers, kmer_index, group=None):
+        self.ctx, self.kpomers, self.kpomer_index, self.kmers, self.kmer_index, self.group = ctx, kpomers, kpomer_index, kmers, kmer_index, group
+
+    def Build(self, budget_bytes=None):
+        """budget_bytes: a fixed budget of every mask pass (tests); None plans each pass against the memory every rank has free"""
+        import torch
+        import torch.distributed as dist
+        ctx, L, group = self.ctx, self.ctx.L, self.group
+        world, rank = dist.get_world_size(group), dist.get_rank(group)
+        kp, km = self.kpomers, self.kmers
+        if not kp.h or not km.h:
+            raise ValueError("a k-mer set has been freed")
+        with_cov = self.kpomer_index is not None
+        # every rank takes part in the same collectives only for one k, one B and one choice of coverage
+        shape = (km.k(), km.num_buckets(), with_cov)
+        shapes = [None] * world
+        dist.all_gather_object(shapes, shape, group=group)
+        if any(tuple(x) != shape for x in shapes):
+            raise ValueError("the ranks' (k, num_buckets, coverage) differ: %s" % (shapes,))
+        if with_cov:
+            _check_owned_once(*_ownership(kp, group), what="(k+1)-mer")     # overlapping sources would count a (k+1)-mer twice
+        bsz_all, owned_all = _ownership(km, group)
+        _check_owned_once(bsz_all, owned_all)
+        owners = np.ascontiguousarray(owned_all.argmax(axis=0), np.int32)
+        h = C.c_void_p()
+        ctx.check(L.sgpu_dist_ext_begin(ctx.h, kp.h, self.kpomer_index.h if with_cov else None, km.h, self.kmer_index.h, _p(owners), world, rank,
+                                        C.byref(h)))
+        ext = DistributedExtensionIndex(ctx, h, kp, km, with_cov)
+        try:
+            local = np.zeros(km.num_buckets(), np.uint64)
+            ctx.check(L.sgpu_dist_ext_local_counts(h, _p(local)))
+            ext.local_counts = local
+            all_counts = _all_gather_u64(local, group)
+            total = C.c_uint64()
+            ctx.check(L.sgpu_dist_ext_plan(h, _p(all_counts), C.byref(total)))
+            while True:
+                budget = _pass_budget(ctx, group, lambda fb: L.sgpu_dist_ext_free_bytes(h, fb), budget_bytes)
+                p = C.c_int()
+                ctx.check(L.sgpu_dist_ext_next_pass(h, budget, C.byref(p)))
+                if p.value < 0:
+                    break
+                _open_peers(ctx, group, lambda out: L.sgpu_dist_ext_ipc_handle(h, out), lambda descs: L.sgpu_dist_ext_open_peers(h, descs))
+                ctx.check(L.sgpu_dist_ext_scatter(h, p.value))     # this rank's contributions to the pass, grouped by owner
+                dist.barrier(group=group)                          # every rank's staging buffer is complete
+                ctx.check(L.sgpu_dist_ext_apply(h, p.value))       # my pieces out of every peer's staging buffer, into my slice
+                dist.barrier(group=group)                          # nobody reads my staging buffer any more
+                ext.npass += 1
+            if with_cov:
+                # the union's histogram: the ranks' histograms summed, as long as the longest
+                n = L.sgpu_dist_ext_histogram(h, None, 0)
+                mine = np.zeros(max(n, 1), np.uint64)
+                L.sgpu_dist_ext_histogram(h, _p(mine), n)
+                dev = _backend_device(group)
+                t = torch.tensor([n], dtype=torch.int64, device=dev)
+                dist.all_reduce(t, op=dist.ReduceOp.MAX, group=group)
+                m = int(t.item())
+                hist = np.zeros(max(m, 1), np.uint64)
+                hist[:n] = mine[:n]
+                th = torch.from_numpy(hist.view(np.int64)).to(dev)
+                dist.all_reduce(th, group=group)
+                ext._hist = th.cpu().numpy().view(np.uint64)[:m].copy()
+        except BaseException:
+            ext.free()
+            raise
+        return ext
+
+
+def _assemble_slices(piece, storage, group, what):
+    """the union's array from the owners' slices (`piece`: this rank's, in the slot order of its index over `storage`): bucket b's
+    run of its owner's slice goes to the union's position of bucket b. Rank 0 gets the array, the others None."""
+    import torch.distributed as dist
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    bsz_all, owned_all = _ownership(storage, group)
+    _check_owned_once(bsz_all, owned_all, what)
+    pieces = [None] * world if rank == 0 else None
+    dist.gather_object(piece, pieces, dst=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
+    if rank != 0:
+        return None
+    bsz = bsz_all.sum(axis=0)
+    ustart = np.concatenate(([0], np.cumsum(bsz))).astype(np.int64)
+    lstart = np.concatenate((np.zeros((world, 1), np.int64), np.cumsum(bsz_all, axis=1)), axis=1)
+    out = np.zeros(int(ustart[-1]), piece.dtype)
+    for b in np.flatnonzero(bsz):
+        r = int(np.flatnonzero(owned_all[:, b])[0])
+        out[ustart[b]:ustart[b + 1]] = pieces[r][lstart[r, b]:lstart[r, b] + bsz[b]]
+    return out
+
+
+def assemble_masks(ext, group=None):
+    """DeBruijnGraph.masks of one GPU over the union (early clippers off), from the ranks' slices: on rank 0, None elsewhere"""
+    return _assemble_slices(ext.masks(), ext.kmers, group, "k-mer")
+
+
+def assemble_coverage(ext, group=None):
+    """DeBruijnGraph.coverage of one GPU over the union, from the ranks' slices: on rank 0, None elsewhere"""
+    return _assemble_slices(ext.coverage(), ext.kpomers, group, "(k+1)-mer")
+
+
 def distributed_cov_filter(ctx, k_plus_one, threshold, group=None, apply=True, phase_done=None):
     """reads_io.CovFilteringWrap over a read set sharded across the ranks of a torch.distributed process group: the verdicts, bound
     and key width are those of one GPU over the union of the shards (in rank order). Returns (keep flags of this rank's reads as
@@ -185,15 +366,9 @@ def distributed_cov_filter(ctx, k_plus_one, threshold, group=None, apply=True, p
     ctx.check(L.sgpu_dist_cov_begin(ctx.h, int(k_plus_one), int(threshold), world, rank, C.byref(h)))
     try:
         done("hll")
-        desc = np.zeros(SGPU_IPC_BYTES, np.uint8)
         for name, step in (("merge", L.sgpu_dist_cov_bound), ("fill", L.sgpu_dist_cov_fill)):
             # descriptors of the registers, then of the table slices; the all_gather also orders the steps across the ranks
-            ctx.check(L.sgpu_dist_cov_ipc_handle(h, desc.ctypes.data_as(C.c_void_p)))
-            t_h = torch.from_numpy(desc).to(backend_dev)
-            hs = [torch.empty_like(t_h) for _ in range(world)]
-            dist.all_gather(hs, t_h, group=group)
-            descs = np.ascontiguousarray(torch.stack(hs).cpu().numpy())
-            ctx.check(L.sgpu_dist_cov_open_peers(h, descs.ctypes.data_as(C.c_void_p)))
+            _open_peers(ctx, group, lambda out: L.sgpu_dist_cov_ipc_handle(h, out), lambda descs: L.sgpu_dist_cov_open_peers(h, descs))
             ctx.check(step(h))
             done(name)
         dist.barrier(group=group)                     # every rank's windows are in the owners' slices
@@ -232,6 +407,22 @@ def cov_pass_plan_host(cardinality_bound, nreads, budget_bytes):
     if rc:
         raise ValueError("bad arguments")
     return passes.value, int(cap.value)
+
+
+def ext_plan_host(world, owners, all_counts, budget_bytes, record_bytes):
+    """the mask passes' plan alone (pure host arithmetic): (passes, bucket boundaries, the most records any rank sends or any owner
+    receives in one pass) for owners[b] = the rank owning k-mer bucket b and all_counts = world x B contributions"""
+    from . import _lib
+    L = _lib.load()
+    owners = np.ascontiguousarray(owners, np.int32)
+    all_counts = np.ascontiguousarray(all_counts, np.uint64)
+    B = len(owners)
+    bounds = np.zeros(B + 1, np.int32)
+    mx = C.c_uint64()
+    n = L.sgpu_dist_ext_plan_host(world, B, _p(owners), _p(all_counts), budget_bytes, record_bytes, _p(bounds), C.byref(mx))
+    if n < 0:
+        raise ValueError("bad world size, owner table or arguments")
+    return n, bounds[: n + 1].copy(), int(mx.value)
 
 
 def plan_host(world, num_buckets, key_bits, all_counts, budget_bytes, record_bytes):
