@@ -388,6 +388,42 @@ void sgpu_dist_ext_free(sgpu_dist_ext *d);
 int sgpu_dist_ext_plan_host(int world, int num_buckets, const int32_t *owners, const uint64_t *all_counts, uint64_t budget_bytes, int record_bytes,
                             int *pass_bounds, uint64_t *max_records);
 
+/* ---- multi-GPU unitigs and perfect loops (one process per GPU), from a rank's sgpu_dist_ext after its passes: the edges one GPU's
+ * sgpu_graph_build gives over the union (early clippers off). Every rank walks from the junctions and the loop leaders among the
+ * k-mers it owns; a walk reads the index, masks, visited flags and coverage of whichever rank owns each k-mer it meets, in place,
+ * through cudaIpc mappings of the peers' arenas (the owners' per-bucket index rows are copied to every rank once). Link records
+ * carry union slots. kmer_owners[b] / kpomer_owners[b]: the rank whose k-mer / (k+1)-mer set holds bucket b (kpomer_owners may be
+ * NULL without coverage); kmer_bucket_sizes[b]: the union's k-mers in bucket b. budget_bytes sizes the junction batches (0: the
+ * memory left). The extension index, its sets and indexes must stay alive until sgpu_dist_graph_free.
+ *   begin (working copy of the masks, junction list) -> ipc_handle -> [all_gather descriptors] -> open_peers -> unitigs [barrier]
+ *   -> clear_visited [barrier] -> ipc_handle -> [all_gather] -> open_peers -> loops [barrier] -> edges / bucket_counts -> free
+ * (without perfect loops, stop after unitigs). A rank's edges are its unitigs in its final_kmers x out-edge order, then its loops
+ * in its leaders' order; bucket_counts gives per bucket the unitig edges that start at a junction of that bucket and the loop
+ * edges whose leader lies in it, so that the ranks' edges interleave into the single-GPU order: the unitig edges bucket by bucket,
+ * then the loop edges bucket by bucket. */
+#define SGPU_DIST_GRAPH_IPC_BYTES 256
+typedef struct sgpu_dist_graph sgpu_dist_graph;
+int sgpu_dist_graph_begin(sgpu_ctx *ctx, const sgpu_dist_ext *ext, const int32_t *kmer_owners, const int32_t *kpomer_owners,
+                          const uint64_t *kmer_bucket_sizes, uint64_t budget_bytes, sgpu_dist_graph **out);
+int sgpu_dist_graph_ipc_handle(sgpu_dist_graph *d, uint8_t *out /* SGPU_DIST_GRAPH_IPC_BYTES */);
+int sgpu_dist_graph_open_peers(sgpu_dist_graph *d, const uint8_t *descriptors /* world x SGPU_DIST_GRAPH_IPC_BYTES, rank-major */);
+int sgpu_dist_graph_unitigs(sgpu_dist_graph *d);
+int sgpu_dist_graph_clear_visited(sgpu_dist_graph *d);
+int sgpu_dist_graph_loops(sgpu_dist_graph *d);
+/* out4: this rank's edges, its unitig edges (the first ones), the bases of their text, its junction batches */
+int sgpu_dist_graph_stats(const sgpu_dist_graph *d, uint64_t *out4);
+/* this rank's edges: text (stats[2] bytes), lengths, link records (LinkRecord hash_and_mask, ~0 = self-conjugate end), raw coverage */
+int sgpu_dist_graph_edges(const sgpu_dist_graph *d, char *seq, uint32_t *lens, uint64_t *link_start, uint64_t *link_end, uint32_t *raw_cov);
+int sgpu_dist_graph_bucket_counts(const sgpu_dist_graph *d, uint64_t *unitig_counts /* num_buckets */, uint64_t *loop_counts /* num_buckets */);
+/* milliseconds spent so far in: begin (mask copy + junction list), unitigs, clear_visited, loops */
+int sgpu_dist_graph_times(const sgpu_dist_graph *d, float *out4);
+void sgpu_dist_graph_free(sgpu_dist_graph *d);
+/* a host-only graph from n assembled edges (text = the edges' bases concatenated, nbases = the sum of lens; every length >= k + 1):
+ * sgpu_graph_num_unitigs / _unitig_bases / _unitigs / _gfa / _write_gfa / _free work on it, the device accessors (masks, coverage,
+ * histogram, clipper statistics, sgpu_edge_index_build) return SGPU_EINVAL */
+int sgpu_graph_from_edges(int k, const char *seq, int64_t nbases, const uint32_t *lens, const uint64_t *link_start, const uint64_t *link_end,
+                          const uint32_t *raw_cov, int64_t n, sgpu_graph **out);
+
 /* self tests of the shared host/device arithmetic (tests only): op 0 = xxh3_64, 1 = xxh3_128 lo, 2 = xxh3_128 hi, 3 = bucket(arg),
  * 4 = is_minimal, 5.. = rc word j. keys: n records of ceil(K/32) words. on_device != 0 runs the same code in a kernel. */
 int sgpu_selftest(sgpu_ctx *ctx, int on_device, int op, int K, uint64_t arg, const uint64_t *keys, int64_t n, uint64_t *out);

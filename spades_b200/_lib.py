@@ -33,6 +33,9 @@ SYMBOLS = [
     "sgpu_dist_ext_begin", "sgpu_dist_ext_local_counts", "sgpu_dist_ext_plan", "sgpu_dist_ext_free_bytes", "sgpu_dist_ext_next_pass",
     "sgpu_dist_ext_ipc_handle", "sgpu_dist_ext_open_peers", "sgpu_dist_ext_scatter", "sgpu_dist_ext_apply", "sgpu_dist_ext_masks",
     "sgpu_dist_ext_coverage", "sgpu_dist_ext_histogram", "sgpu_dist_ext_times", "sgpu_dist_ext_free", "sgpu_dist_ext_plan_host",
+    "sgpu_dist_graph_begin", "sgpu_dist_graph_ipc_handle", "sgpu_dist_graph_open_peers", "sgpu_dist_graph_unitigs", "sgpu_dist_graph_clear_visited",
+    "sgpu_dist_graph_loops", "sgpu_dist_graph_stats", "sgpu_dist_graph_edges", "sgpu_dist_graph_bucket_counts", "sgpu_dist_graph_times",
+    "sgpu_dist_graph_free", "sgpu_graph_from_edges",
     "sgpu_selftest",
 ]
 
@@ -183,6 +186,18 @@ def load():
     L.sgpu_dist_ext_times.restype = i32; L.sgpu_dist_ext_times.argtypes = [vp, vp]
     L.sgpu_dist_ext_free.restype = None; L.sgpu_dist_ext_free.argtypes = [vp]
     L.sgpu_dist_ext_plan_host.restype = i32; L.sgpu_dist_ext_plan_host.argtypes = [i32, i32, vp, vp, u64, i32, vp, C.POINTER(u64)]
+    L.sgpu_dist_graph_begin.restype = i32; L.sgpu_dist_graph_begin.argtypes = [vp, vp, vp, vp, vp, u64, pp]
+    L.sgpu_dist_graph_ipc_handle.restype = i32; L.sgpu_dist_graph_ipc_handle.argtypes = [vp, vp]
+    L.sgpu_dist_graph_open_peers.restype = i32; L.sgpu_dist_graph_open_peers.argtypes = [vp, vp]
+    L.sgpu_dist_graph_unitigs.restype = i32; L.sgpu_dist_graph_unitigs.argtypes = [vp]
+    L.sgpu_dist_graph_clear_visited.restype = i32; L.sgpu_dist_graph_clear_visited.argtypes = [vp]
+    L.sgpu_dist_graph_loops.restype = i32; L.sgpu_dist_graph_loops.argtypes = [vp]
+    L.sgpu_dist_graph_stats.restype = i32; L.sgpu_dist_graph_stats.argtypes = [vp, vp]
+    L.sgpu_dist_graph_edges.restype = i32; L.sgpu_dist_graph_edges.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.sgpu_dist_graph_bucket_counts.restype = i32; L.sgpu_dist_graph_bucket_counts.argtypes = [vp, vp, vp]
+    L.sgpu_dist_graph_times.restype = i32; L.sgpu_dist_graph_times.argtypes = [vp, vp]
+    L.sgpu_dist_graph_free.restype = None; L.sgpu_dist_graph_free.argtypes = [vp]
+    L.sgpu_graph_from_edges.restype = i32; L.sgpu_graph_from_edges.argtypes = [i32, vp, i64, vp, vp, vp, vp, i64, pp]
     L.sgpu_selftest.restype = i32; L.sgpu_selftest.argtypes = [vp, i32, i32, i32, u64, vp, i64, vp]
     _lib = L
     return L

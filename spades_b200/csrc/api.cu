@@ -444,17 +444,17 @@ int sgpu_graph_build_streamed(sgpu_ctx *ctx, const sgpu_kset *kpomers, const sgp
     })
 }
 int sgpu_graph_at_clipper_stats(const sgpu_graph *g, uint64_t *out4) {
-    if (!g || !out4) return SGPU_EINVAL;
+    if (!g || !out4 || !g->g->ctx) return SGPU_EINVAL;
     for (int i = 0; i < 4; ++i) out4[i] = g->g->at_stats[i];
     return SGPU_OK;
 }
 int sgpu_graph_tip_clipper_stats(const sgpu_graph *g, uint64_t *out3) {
-    if (!g || !out3) return SGPU_EINVAL;
+    if (!g || !out3 || !g->g->ctx) return SGPU_EINVAL;
     for (int i = 0; i < 3; ++i) out3[i] = g->g->tc_stats[i];
     return SGPU_OK;
 }
 int sgpu_graph_masks(const sgpu_graph *g, uint8_t *out, int64_t n) {
-    if (!g || (n && !out)) return SGPU_EINVAL;
+    if (!g || (n && !out) || !g->g->ctx) return SGPU_EINVAL;
     Ctx *c = g->g->ctx;
     API_TRY(c, {
         SG_CHECK(n == g->g->km->n, SGPU_EINVAL, "mask array size != number of k-mers");
@@ -463,7 +463,7 @@ int sgpu_graph_masks(const sgpu_graph *g, uint8_t *out, int64_t n) {
     })
 }
 int sgpu_graph_coverage(const sgpu_graph *g, uint32_t *out, int64_t n) {
-    if (!g || (n && !out)) return SGPU_EINVAL;
+    if (!g || (n && !out) || !g->g->ctx) return SGPU_EINVAL;
     Ctx *c = g->g->ctx;
     API_TRY(c, {
         SG_CHECK(g->g->cov.p, SGPU_EINVAL, "graph was built without a (k+1)-mer index: no coverage");
@@ -473,7 +473,7 @@ int sgpu_graph_coverage(const sgpu_graph *g, uint32_t *out, int64_t n) {
     })
 }
 int64_t sgpu_graph_histogram(const sgpu_graph *g, uint64_t *out, int64_t cap) {
-    if (!g) return -1;
+    if (!g || !g->g->ctx) return -1;
     Ctx *c = g->g->ctx;
     try {
         cudaSetDevice(c->device);
@@ -496,7 +496,7 @@ int64_t sgpu_graph_gfa(const sgpu_graph *g, const char *version, char *out, int6
         std::string t = graph_gfa(g->g, version ? version : "SPAdes-4.3.0-dev");
         if (out && (int64_t)t.size() <= cap) memcpy(out, t.data(), t.size());
         return (int64_t)t.size();
-    } catch (const std::exception &e) { g->g->ctx->err = e.what(); return -1; }
+    } catch (const std::exception &e) { if (g->g->ctx) g->g->ctx->err = e.what(); return -1; }
 }
 int sgpu_graph_write_gfa(const sgpu_graph *g, const char *version, const char *path) {
     if (!g || !path) return SGPU_EINVAL;
@@ -529,6 +529,7 @@ int sgpu_graph_write_gfa(const sgpu_graph *g, const char *version, const char *p
 int sgpu_edge_index_build(sgpu_ctx *ctx, const sgpu_graph *g, int K, int num_buckets, sgpu_edge_index **out) {
     if (!ctx || !g || !out) return SGPU_EINVAL;
     *out = nullptr;
+    if (!g->g->ctx) return SGPU_EINVAL;
     Ctx *c = &ctx->c;
     API_TRY(c, {
         SG_CUDA(cudaSetDevice(c->device));
@@ -573,7 +574,8 @@ void sgpu_edge_index_free(sgpu_edge_index *e) {
 }
 void sgpu_graph_free(sgpu_graph *g) {
     if (!g) return;
-    if (g->g) { Ctx *c = g->g->ctx; cudaSetDevice(c->device); delete g->g; child_release(c); }
+    if (g->g && !g->g->ctx) delete g->g;                  // a host-only graph (sgpu_graph_from_edges)
+    else if (g->g) { Ctx *c = g->g->ctx; cudaSetDevice(c->device); delete g->g; child_release(c); }
     delete g;
 }
 
@@ -798,6 +800,105 @@ int sgpu_dist_ext_plan_host(int world, int num_buckets, const int32_t *owners, c
     if (world < 1 || num_buckets < 1 || !owners || !all_counts || !pass_bounds || !max_records) return -1;
     try { return ext_plan_host(world, num_buckets, owners, all_counts, budget_bytes, record_bytes, pass_bounds, max_records); }
     catch (...) { return -1; }
+}
+}  // extern "C"
+
+struct sgpu_dist_graph { DistGraph *d; Ctx *c; };
+extern "C" {
+int sgpu_dist_graph_begin(sgpu_ctx *ctx, const sgpu_dist_ext *ext, const int32_t *kmer_owners, const int32_t *kpomer_owners,
+                          const uint64_t *kmer_bucket_sizes, uint64_t budget_bytes, sgpu_dist_graph **out) {
+    if (!ctx || !ext || !kmer_owners || !kmer_bucket_sizes || !out) return SGPU_EINVAL;
+    *out = nullptr;
+    Ctx *c = &ctx->c;
+    API_TRY(c, {
+        SG_CUDA(cudaSetDevice(c->device));
+        DistGraph *d = dgraph_begin(c, ext->d, kmer_owners, kpomer_owners, kmer_bucket_sizes, budget_bytes);
+        *out = new sgpu_dist_graph{d, c};
+        child_add(c);
+    })
+}
+int sgpu_dist_graph_ipc_handle(sgpu_dist_graph *d, uint8_t *out) {
+    if (!d || !out) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dgraph_ipc_handle(d->d, out); })
+}
+int sgpu_dist_graph_open_peers(sgpu_dist_graph *d, const uint8_t *descriptors) {
+    if (!d || !descriptors) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dgraph_open_peers(d->d, descriptors); })
+}
+int sgpu_dist_graph_unitigs(sgpu_dist_graph *d) {
+    if (!d) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dgraph_unitigs(d->d); })
+}
+int sgpu_dist_graph_clear_visited(sgpu_dist_graph *d) {
+    if (!d) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dgraph_clear_visited(d->d); })
+}
+int sgpu_dist_graph_loops(sgpu_dist_graph *d) {
+    if (!d) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dgraph_loops(d->d); })
+}
+int sgpu_dist_graph_stats(const sgpu_dist_graph *d, uint64_t *out4) {
+    if (!d || !out4) return SGPU_EINVAL;
+    dgraph_stats(d->d, out4);
+    return SGPU_OK;
+}
+int sgpu_dist_graph_edges(const sgpu_dist_graph *d, char *seq, uint32_t *lens, uint64_t *link_start, uint64_t *link_end, uint32_t *raw_cov) {
+    if (!d) return SGPU_EINVAL;
+    const Graph &g = dgraph_edges(d->d);
+    const size_t n = g.edge_len.size();
+    if ((n && (!lens || !link_start || !link_end || !raw_cov)) || (!g.seq.empty() && !seq)) return SGPU_EINVAL;
+    if (!g.seq.empty()) memcpy(seq, g.seq.data(), g.seq.size());
+    if (n) {
+        memcpy(lens, g.edge_len.data(), n * 4);
+        memcpy(link_start, g.link_start.data(), n * 8);
+        memcpy(link_end, g.link_end.data(), n * 8);
+        memcpy(raw_cov, g.raw_cov.data(), n * 4);
+    }
+    return SGPU_OK;
+}
+int sgpu_dist_graph_bucket_counts(const sgpu_dist_graph *d, uint64_t *unitig_counts, uint64_t *loop_counts) {
+    if (!d || !unitig_counts || !loop_counts) return SGPU_EINVAL;
+    dgraph_bucket_counts(d->d, unitig_counts, loop_counts);
+    return SGPU_OK;
+}
+int sgpu_dist_graph_times(const sgpu_dist_graph *d, float *out4) {
+    if (!d || !out4) return SGPU_EINVAL;
+    dgraph_times(d->d, out4);
+    return SGPU_OK;
+}
+void sgpu_dist_graph_free(sgpu_dist_graph *d) {
+    if (!d) return;
+    Ctx *c = d->c;
+    cudaSetDevice(c->device);
+    dgraph_free(d->d);
+    delete d;
+    child_release(c);
+}
+int sgpu_graph_from_edges(int k, const char *seq, int64_t nbases, const uint32_t *lens, const uint64_t *link_start, const uint64_t *link_end,
+                          const uint32_t *raw_cov, int64_t n, sgpu_graph **out) {
+    if (!out) return SGPU_EINVAL;
+    *out = nullptr;
+    if (k < 1 || k > 127 || n < 0 || nbases < 0 || (nbases && !seq) || (n && (!lens || !link_start || !link_end || !raw_cov))) return SGPU_EINVAL;
+    uint64_t at = 0;
+    for (int64_t i = 0; i < n; ++i) {
+        if (lens[i] < (uint32_t)k + 1) return SGPU_EINVAL;                // an edge holds at least one (k+1)-mer
+        at += lens[i];
+        if (at > (uint64_t)nbases) return SGPU_EINVAL;                    // an edge reaching past the text
+    }
+    if (at != (uint64_t)nbases) return SGPU_EINVAL;                      // text and lengths disagree
+    try {
+        Graph *g = new Graph();
+        g->k = k;
+        g->seq.assign(seq ? seq : "", (size_t)nbases);
+        g->edge_len.assign(lens, lens + n);
+        g->edge_off.resize((size_t)n);
+        for (int64_t i = 0, o = 0; i < n; o += lens[i++]) g->edge_off[i] = (uint64_t)o;
+        g->link_start.assign(link_start, link_start + n);
+        g->link_end.assign(link_end, link_end + n);
+        g->raw_cov.assign(raw_cov, raw_cov + n);
+        *out = new sgpu_graph{g};
+    } catch (const std::bad_alloc &) { return SGPU_ENOMEM; }
+    return SGPU_OK;
 }
 }  // extern "C"
 

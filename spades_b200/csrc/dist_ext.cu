@@ -230,11 +230,6 @@ struct ExtDist {
     int record_bytes() const { return 8 * nw + 1; }
 };
 
-struct Stopwatch {
-    std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
-    float ms() const { return std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count(); }
-};
-
 template <int NW, int NWS>
 struct ExtDistNW : ExtDist {
     void histogram() override {
@@ -445,5 +440,8 @@ void ext_coverage(const ExtDist *d, uint32_t *out, int64_t n) {
 const std::vector<uint64_t> &ext_histogram(const ExtDist *d) { return d->hist; }
 void ext_times(const ExtDist *d, float *out5) { for (int i = 0; i < 5; ++i) out5[i] = d->ms[i]; }
 void ext_free(ExtDist *d) { delete d; }
+ExtSlices ext_slices(const ExtDist *d) {
+    return ExtSlices{d->ctx, d->kp, d->km, d->mkp, d->mk, d->masks.p, d->cov.p, d->owner.data(), d->world, d->rank};
+}
 
 }  // namespace sg

@@ -40,6 +40,23 @@ std::vector<uint64_t> graph_histogram(Ctx *ctx, const Graph *g);
 void coverage_fill(Ctx *ctx, ChunkStager &kpomers, const Mphf *mkp, uint32_t *cov);
 std::vector<uint64_t> coverage_histogram(Ctx *ctx, const uint32_t *cov, int64_t n);
 
+// dist_graph.cu : the unitigs and perfect loops of one rank's share of a distributed graph (DistributedGraphConstructor), from its
+// extension index slices (dist_ext.cu). Phases, with a barrier between them: begin (a working copy of the masks, the junction
+// list), ipc_handle / open_peers, unitigs, clear_visited, ipc_handle / open_peers again (the remaining slots' positions), loops.
+struct DistGraph;
+struct ExtDist;
+DistGraph *dgraph_begin(Ctx *ctx, const ExtDist *ext, const int *kmer_owner, const int *kpomer_owner, const uint64_t *kmer_bucket_sizes, uint64_t budget);
+void dgraph_ipc_handle(DistGraph *d, uint8_t *out256);
+void dgraph_open_peers(DistGraph *d, const uint8_t *descs);
+void dgraph_unitigs(DistGraph *d);
+void dgraph_clear_visited(DistGraph *d);
+void dgraph_loops(DistGraph *d);
+const Graph &dgraph_edges(const DistGraph *d);                   // its unitigs in its final_kmers order, then its loops
+void dgraph_stats(const DistGraph *d, uint64_t *out4);           // edges, unitig edges, bases, junction batches
+void dgraph_bucket_counts(const DistGraph *d, uint64_t *unitigs, uint64_t *loops);
+void dgraph_times(const DistGraph *d, float *out4);
+void dgraph_free(DistGraph *d);
+
 // edge_index.cu : KmerFreeEdgeIndex refill over the graph's own unitigs (alignment/edge_index.hpp, assembly_graph/index/edge_index_builders.hpp)
 struct EdgeIndex {
     Ctx *ctx = nullptr;

@@ -43,10 +43,9 @@ __device__ __forceinline__ uint64_t level_pos(const MphfDev &m, const Kmer<NW> &
     return pos;
 }
 
-// mphf::lookup (BooPHF.h:465-487) + bitVector::rank (:303-314) + KMerIndex::seq_idx (kmer_index.hpp:88-93)
+// mphf::lookup (BooPHF.h:465-487) + bitVector::rank (:303-314) + KMerIndex::seq_idx (kmer_index.hpp:88-93), for a key of bucket b
 template <int NW>
-__device__ __forceinline__ uint64_t mphf_lookup_dev(const MphfDev &m, const Kmer<NW> &k) {
-    const uint32_t b = kmer_bucket<NW>(k, m.B);
+__device__ __forceinline__ uint64_t mphf_lookup_dev(const MphfDev &m, const Kmer<NW> &k, uint32_t b) {
     LevelHasher lh(xxh3_128<NW>(k));
     for (int l = 0; l < kLevels - 1; ++l) {
         const uint64_t h = lh.next();
@@ -64,7 +63,10 @@ __device__ __forceinline__ uint64_t mphf_lookup_dev(const MphfDev &m, const Kmer
     }
     return ~0ull;
 }
-
+template <int NW>
+__device__ __forceinline__ uint64_t mphf_lookup_dev(const MphfDev &m, const Kmer<NW> &k) {
+    return mphf_lookup_dev<NW>(m, k, kmer_bucket<NW>(k, m.B));
+}
 
 MphfDev mphf_dev(const Mphf *m);
 

@@ -399,6 +399,12 @@ struct ChunkStager {
     }
 };
 
+// host milliseconds since construction
+struct Stopwatch {
+    std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
+    float ms() const { return std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count(); }
+};
+
 // SGPU_TRACE (user option, read once per process): wall-clock milliseconds between marks on stderr, one line per mark. A trace
 // given a stream (a context's is never null) waits for the work enqueued on it at every mark, so that a mark also times that work.
 struct Trace {
@@ -499,6 +505,17 @@ void ext_coverage(const ExtDist *d, uint32_t *out, int64_t n);
 const std::vector<uint64_t> &ext_histogram(const ExtDist *d);
 void ext_times(const ExtDist *d, float *out5);
 void ext_free(ExtDist *d);
+// what the distributed graph reads of an extension index: this rank's sets, indexes and slices (cov null without coverage)
+struct ExtSlices {
+    Ctx *ctx;
+    const KSet *kp, *km;
+    const Mphf *mkp, *mk;
+    const uint8_t *masks;
+    const uint32_t *cov;
+    const int *owner;              // B: the rank owning each k-mer bucket
+    int world, rank;
+};
+ExtSlices ext_slices(const ExtDist *d);
 // pure host planning (exported for CPU tests): returns npass, fills the pass boundaries and the most records of a pass
 int ext_plan_host(int world, int B, const int *owner, const uint64_t *cnt_all, uint64_t budget_bytes, int record_bytes, int *pass_b /*B+1 max*/, uint64_t *most);
 

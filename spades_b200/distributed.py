@@ -11,6 +11,7 @@ import numpy as np
 from .kmer_index import KMerDiskStorage, SGPU_CANONICAL, SGPU_RESULT_ON_HOST, _p
 
 SGPU_IPC_BYTES = 96
+SGPU_DIST_GRAPH_IPC_BYTES = 256
 
 
 def _backend_device(group):
@@ -32,11 +33,11 @@ def _pass_budget(ctx, group, free_bytes, budget_bytes):
     return int(int(tb.item()) * 0.90)
 
 
-def _open_peers(ctx, group, ipc_handle, open_peers):
-    """all_gather of the ranks' SGPU_IPC_BYTES descriptors (ipc_handle(out) writes this rank's), handed to open_peers(descriptors)"""
+def _open_peers(ctx, group, ipc_handle, open_peers, nbytes=SGPU_IPC_BYTES):
+    """all_gather of the ranks' nbytes descriptors (ipc_handle(out) writes this rank's), handed to open_peers(descriptors)"""
     import torch
     import torch.distributed as dist
-    desc = np.zeros(SGPU_IPC_BYTES, np.uint8)
+    desc = np.zeros(nbytes, np.uint8)
     ctx.check(ipc_handle(desc.ctypes.data_as(C.c_void_p)))
     t_h = torch.from_numpy(desc).to(_backend_device(group))
     hs = [torch.empty_like(t_h) for _ in range(dist.get_world_size(group))]
@@ -344,6 +345,203 @@ def assemble_masks(ext, group=None):
 def assemble_coverage(ext, group=None):
     """DeBruijnGraph.coverage of one GPU over the union, from the ranks' slices: on rank 0, None elsewhere"""
     return _assemble_slices(ext.coverage(), ext.kpomers, group, "(k+1)-mer")
+
+
+class DistributedGraph:
+    """this rank's share of the union's condensed graph (DistributedGraphConstructor.ConstructGraph): the unitigs that start at a
+    junction it owns, in its final_kmers x out-edge order, then the perfect loops whose leader it owns; with per-bucket counts of
+    both, so that assemble_graph can interleave the ranks' edges into one GPU's order"""
+
+    def __init__(self, ctx, h, k, num_buckets, owners):
+        self.ctx, self.h, self.k, self.num_buckets, self.owners = ctx, h, k, num_buckets, owners
+
+    def stats(self):
+        """(edges, unitig edges, bases, junction batches) of this rank"""
+        out = np.zeros(4, np.uint64)
+        self.ctx.check(self.ctx.L.sgpu_dist_graph_stats(self.h, _p(out)))
+        return tuple(int(x) for x in out)
+
+    def edges(self):
+        """this rank's edges: dict of text (bytes), lens, link_start, link_end, raw_cov, unitig_edges, unitig_counts, loop_counts"""
+        n, nu, nb, _ = self.stats()
+        seq = np.zeros(max(nb, 1), np.uint8)
+        lens = np.zeros(max(n, 1), np.uint32)
+        ls, le = np.zeros(max(n, 1), np.uint64), np.zeros(max(n, 1), np.uint64)
+        rc = np.zeros(max(n, 1), np.uint32)
+        self.ctx.check(self.ctx.L.sgpu_dist_graph_edges(self.h, _p(seq), _p(lens), _p(ls), _p(le), _p(rc)))
+        uc, lc = np.zeros(self.num_buckets, np.uint64), np.zeros(self.num_buckets, np.uint64)
+        self.ctx.check(self.ctx.L.sgpu_dist_graph_bucket_counts(self.h, _p(uc), _p(lc)))
+        return dict(text=seq[:nb].tobytes(), lens=lens[:n], link_start=ls[:n], link_end=le[:n], raw_cov=rc[:n], unitig_edges=nu,
+                    unitig_counts=uc, loop_counts=lc)
+
+    def times(self):
+        """milliseconds of this rank's mask copy + junction list, unitigs, visited clear and loops"""
+        out = np.zeros(4, np.float32)
+        self.ctx.check(self.ctx.L.sgpu_dist_graph_times(self.h, _p(out)))
+        return dict(zip(("junctions", "unitigs", "clear_visited", "loops"), (float(x) for x in out)))
+
+    def free(self):
+        if self.h:
+            self.ctx.L.sgpu_dist_graph_free(self.h); self.h = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+class DistributedGraphConstructor:
+    """UnbranchingPathExtractor over the ranks of a torch.distributed process group, from each rank's DistributedExtensionIndex
+    (its Build has run) and the indexes that built it: ConstructGraph gives every rank its share of the edges one GPU's
+    DeBruijnGraphConstructor.ConstructGraph gives over the union (early clippers off); assemble_graph puts them together. The walks
+    read the other ranks' indexes, masks and coverage in place; no rank holds more than its own slices and per-bucket tables. The
+    extension index, sets and indexes must not be freed before the result."""
+
+    def __init__(self, ctx, ext, kpomer_index, kmer_index, group=None):
+        self.ctx, self.ext, self.kpomer_index, self.kmer_index, self.group = ctx, ext, kpomer_index, kmer_index, group
+
+    def ConstructGraph(self, keep_perfect_loops=True, budget_bytes=None):
+        """budget_bytes: a fixed budget of the junction batches (tests); None sizes them from the memory left"""
+        import torch.distributed as dist
+        ctx, L, group, ext = self.ctx, self.ctx.L, self.group, self.ext
+        world = dist.get_world_size(group)
+        if not ext.h or not ext.kmers.h or not ext.kpomers.h:
+            raise ValueError("the extension index or one of its sets has been freed")
+        km, kp = ext.kmers, ext.kpomers
+        with_cov = self.kpomer_index is not None
+        if with_cov != ext.with_coverage:
+            raise ValueError("the (k+1)-mer index must be given exactly when the extension index has coverage")
+        # the same checks as DistributedExtensionIndexBuilder: every rank takes part in the same collectives
+        shape = (km.k(), km.num_buckets(), with_cov)
+        shapes = [None] * world
+        dist.all_gather_object(shapes, shape, group=group)
+        if any(tuple(x) != shape for x in shapes):
+            raise ValueError("the ranks' (k, num_buckets, coverage) differ: %s" % (shapes,))
+        bsz_all, owned_all = _ownership(km, group)
+        _check_owned_once(bsz_all, owned_all)
+        owners = np.ascontiguousarray(owned_all.argmax(axis=0), np.int32)
+        powners = None
+        if with_cov:
+            pbsz, powned = _ownership(kp, group)
+            _check_owned_once(pbsz, powned, what="(k+1)-mer")
+            powners = np.ascontiguousarray(powned.argmax(axis=0), np.int32)
+        ubsz = np.ascontiguousarray(bsz_all.sum(axis=0), np.uint64)
+        h = C.c_void_p()
+        ctx.check(L.sgpu_dist_graph_begin(ctx.h, ext.h, _p(owners), _p(powners) if with_cov else None, _p(ubsz), int(budget_bytes or 0), C.byref(h)))
+        g = DistributedGraph(ctx, h, km.k(), km.num_buckets(), owners)
+        try:
+            def open_peers():
+                _open_peers(ctx, group, lambda out: L.sgpu_dist_graph_ipc_handle(h, out), lambda descs: L.sgpu_dist_graph_open_peers(h, descs),
+                            SGPU_DIST_GRAPH_IPC_BYTES)
+            open_peers()
+            ctx.check(L.sgpu_dist_graph_unitigs(h))          # walks through every rank's masks; marks visited k-mers wherever they live
+            dist.barrier(group=group)                         # every rank's visited flags are final
+            if keep_perfect_loops:
+                ctx.check(L.sgpu_dist_graph_clear_visited(h))
+                dist.barrier(group=group)                     # every rank's masks are cleared and its remaining slots ranked
+                open_peers()                                  # the remaining slots' positions now exist
+                ctx.check(L.sgpu_dist_graph_loops(h))
+            dist.barrier(group=group)                         # nobody reads my arrays any more
+        except BaseException:
+            g.free()
+            raise
+        return g
+
+
+class AssembledGraph:
+    """the union's graph from the ranks' edges (assemble_graph): unitigs(), gfa() and write_gfa() as DeBruijnGraph has them"""
+
+    def __init__(self, ctx_lib, h):
+        self.L, self.h = ctx_lib, h
+
+    def _err(self):
+        from .kmer_index import SpadesGpuError
+        return SpadesGpuError("host-only graph call failed")
+
+    def unitigs(self):
+        ne, nb = self.L.sgpu_graph_num_unitigs(self.h), self.L.sgpu_graph_unitig_bases(self.h)
+        buf = np.zeros(max(nb, 1), np.uint8); lens = np.zeros(max(ne, 1), np.uint32)
+        if self.L.sgpu_graph_unitigs(self.h, _p(buf), _p(lens)):
+            raise self._err()
+        s = buf[:nb].tobytes().decode()
+        out, o = [], 0
+        for ln in lens[:ne]:
+            out.append(s[o:o + int(ln)]); o += int(ln)
+        return out
+
+    def gfa(self, version="SPAdes-4.3.0-dev"):
+        n = self.L.sgpu_graph_gfa(self.h, version.encode(), None, 0)
+        if n < 0:
+            raise self._err()
+        buf = np.zeros(max(n, 1), np.uint8)
+        self.L.sgpu_graph_gfa(self.h, version.encode(), _p(buf), n)
+        return buf[:n].tobytes().decode()
+
+    def write_gfa(self, path, version="SPAdes-4.3.0-dev"):
+        if self.L.sgpu_graph_write_gfa(self.h, version.encode(), str(path).encode()):
+            raise self._err()
+
+    def free(self):
+        if self.h:
+            self.L.sgpu_graph_free(self.h); self.h = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+def graph_from_edges(k, text, lens, link_start, link_end, raw_cov):
+    """a host-only graph (AssembledGraph) from edges laid end to end in `text`; refuses inconsistent edges with ValueError"""
+    from . import _lib
+    L = _lib.load()
+    lens = np.ascontiguousarray(lens, np.uint32)
+    ls, le = np.ascontiguousarray(link_start, np.uint64), np.ascontiguousarray(link_end, np.uint64)
+    rc = np.ascontiguousarray(raw_cov, np.uint32)
+    n = len(lens)
+    if not (len(ls) == len(le) == len(rc) == n):
+        raise ValueError("the edge arrays have different lengths")
+    buf = np.frombuffer(bytes(text) + b"\0", np.uint8)
+    h = C.c_void_p()
+    if L.sgpu_graph_from_edges(int(k), _p(buf), len(text), _p(lens), _p(ls), _p(le), _p(rc), n, C.byref(h)):
+        raise ValueError("inconsistent edges: a length below k + 1, or lengths that do not add up to the text")
+    return AssembledGraph(L, h)
+
+
+def assemble_graph(dg, group=None):
+    """the union's graph on rank 0 (None elsewhere): the ranks' edges interleaved into one GPU's order -- the unitig edges bucket by
+    bucket (each bucket's from its owner, in its order), then the loop edges bucket by bucket"""
+    import torch.distributed as dist
+    rank = dist.get_rank(group)
+    mine = dg.edges()
+    pieces = [None] * dist.get_world_size(group) if rank == 0 else None
+    dist.gather_object(mine, pieces, dst=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
+    if rank != 0:
+        return None
+    texts, lens, ls, le, rc = [], [], [], [], []
+    offs = [np.concatenate(([0], np.cumsum(p["lens"], dtype=np.uint64))).astype(np.int64) for p in pieces]
+    cur_u = [0] * len(pieces)
+    cur_l = [p["unitig_edges"] for p in pieces]
+
+    def take(r, a, n):
+        p = pieces[r]
+        texts.append(p["text"][offs[r][a]:offs[r][a + n]])
+        for dst, key in ((lens, "lens"), (ls, "link_start"), (le, "link_end"), (rc, "raw_cov")):
+            dst.append(p[key][a:a + n])
+    for counts, cur in (("unitig_counts", cur_u), ("loop_counts", cur_l)):
+        for b in range(dg.num_buckets):
+            r = int(dg.owners[b])
+            n = int(pieces[r][counts][b])
+            if n:
+                take(r, cur[r], n)
+                cur[r] += n
+    for r, p in enumerate(pieces):
+        if cur_u[r] != p["unitig_edges"] or cur_l[r] != len(p["lens"]):
+            raise ValueError("rank %d's bucket counts do not cover its edges" % r)
+    cat = lambda xs, dt: np.concatenate(xs).astype(dt) if xs else np.zeros(0, dt)     # noqa: E731
+    return graph_from_edges(dg.k, b"".join(texts), cat(lens, np.uint32), cat(ls, np.uint64), cat(le, np.uint64), cat(rc, np.uint32))
 
 
 def distributed_cov_filter(ctx, k_plus_one, threshold, group=None, apply=True, phase_done=None):
