@@ -389,7 +389,7 @@ int sgpu_dist_ext_plan_host(int world, int num_buckets, const int32_t *owners, c
                             int *pass_bounds, uint64_t *max_records);
 
 /* ---- multi-GPU unitigs and perfect loops (one process per GPU), from a rank's sgpu_dist_ext after its passes: the edges one GPU's
- * sgpu_graph_build gives over the union (early clippers off). Every rank walks from the junctions and the loop leaders among the
+ * sgpu_graph_build gives over the union (sgpu_dist_graph_begin_opts: the early clippers first, as sgpu_graph_build_opts). Every rank walks from the junctions and the loop leaders among the
  * k-mers it owns; a walk reads the index, masks, visited flags and coverage of whichever rank owns each k-mer it meets, in place,
  * through cudaIpc mappings of the peers' arenas (the owners' per-bucket index rows are copied to every rank once). Link records
  * carry union slots. kmer_owners[b] / kpomer_owners[b]: the rank whose k-mer / (k+1)-mer set holds bucket b (kpomer_owners may be
@@ -405,6 +405,36 @@ int sgpu_dist_ext_plan_host(int world, int num_buckets, const int32_t *owners, c
 typedef struct sgpu_dist_graph sgpu_dist_graph;
 int sgpu_dist_graph_begin(sgpu_ctx *ctx, const sgpu_dist_ext *ext, const int32_t *kmer_owners, const int32_t *kpomer_owners,
                           const uint64_t *kmer_bucket_sizes, uint64_t budget_bytes, sgpu_dist_graph **out);
+/* sgpu_dist_graph_begin with the Construction stage's early clippers (sgpu_graph_build_opts; keep_perfect_loops is the caller's
+ * choice of running clear_visited and loops). The options are refused with SGPU_EINVAL as sgpu_graph_build_opts refuses them,
+ * before anything is allocated; min_length > k is refused on every rank, whether it owns k-mers or not. Every rank passes the
+ * same options. With a clipper on, the phases between the first open_peers and the unitigs are, each followed by a barrier:
+ *   A/T clipper:  at_edges_probe, at_edges_apply, at_tips_probe, isolate, unlink
+ *   tip clipper:  tip_probe, isolate, unlink
+ *   then junctions (the junction list over the clipped masks)
+ * A phase called out of order, or for a clipper that is off, is refused with SGPU_EINVAL and changes nothing. Every probe reads
+ * the owners' masks as they were when the phase began: its flags are final on every rank before any rank's isolate or apply
+ * changes a mask. The probes set the IsolateVertex and root flags in the owners' slices; at_edges_apply clears the deleted links'
+ * bits in both k-mers' owners' masks (32-bit atomics: with the A/T clipper on, open_peers refuses a peer on another device
+ * without native peer atomics); isolate and unlink change only this rank's slice. A rank allocates 1 B per owned k-mer for the
+ * marks, 2 B for the tip clipper's flags and 4 B for the A/T clipper's, released by junctions. */
+int sgpu_dist_graph_begin_opts(sgpu_ctx *ctx, const sgpu_dist_ext *ext, const int32_t *kmer_owners, const int32_t *kpomer_owners,
+                               const uint64_t *kmer_bucket_sizes, uint64_t budget_bytes, const sgpu_graph_options *opts, sgpu_dist_graph **out);
+int sgpu_dist_graph_at_edges_probe(sgpu_dist_graph *d);
+int sgpu_dist_graph_at_edges_apply(sgpu_dist_graph *d);
+int sgpu_dist_graph_at_tips_probe(sgpu_dist_graph *d);
+int sgpu_dist_graph_tip_probe(sgpu_dist_graph *d);
+int sgpu_dist_graph_isolate(sgpu_dist_graph *d);
+int sgpu_dist_graph_unlink(sgpu_dist_graph *d);
+int sgpu_dist_graph_junctions(sgpu_dist_graph *d);
+/* after junctions: this rank's slice of what sgpu_graph_masks gives on one GPU over the union (the clipped masks, or the extension
+ * index's when no clipper is on), n = this rank's k-mers */
+int sgpu_dist_graph_masks(const sgpu_dist_graph *d, uint8_t *out, int64_t n);
+/* this rank's counters: at4 and tc3 as sgpu_graph_at_clipper_stats / _tip_clipper_stats (the union's are the sums over the ranks),
+ * remote3: the mark stores, root stores and bit clears that landed in another rank's slice */
+int sgpu_dist_graph_clipper_stats(const sgpu_dist_graph *d, uint64_t *at4, uint64_t *tc3, uint64_t *remote3);
+/* milliseconds spent so far in: A/T edges probe, A/T edges apply, A/T tips probe, tip probe, isolate (both clippers), unlink (both) */
+int sgpu_dist_graph_clipper_times(const sgpu_dist_graph *d, float *out6);
 int sgpu_dist_graph_ipc_handle(sgpu_dist_graph *d, uint8_t *out /* SGPU_DIST_GRAPH_IPC_BYTES */);
 int sgpu_dist_graph_open_peers(sgpu_dist_graph *d, const uint8_t *descriptors /* world x SGPU_DIST_GRAPH_IPC_BYTES, rank-major */);
 int sgpu_dist_graph_unitigs(sgpu_dist_graph *d);

@@ -3,7 +3,7 @@
 build's unitig and loop phases, at world size 1 on one GPU: every "remote" lookup is then local, so this measures what the
 DistView costs over the LocalView, not NVLink.
 
-    python scripts/bench_dist_graph.py [--reads 20000000] [--k 55] [--buckets 80] [--warmup 1] [--iters 3]
+    python scripts/bench_dist_graph.py [--reads 20000000] [--k 55] [--buckets 80] [--warmup 1] [--iters 3] [--early-tc 95] [--early-at]
 
 The reads come from bench.py's generator (150 bp, 1 % substitutions, seed 42, a genome as long as the read count). They go
 through the distributed (k+1)-mer count, the distributed k-mers of the (k+1)-mers, both indexes and the distributed extension
@@ -11,6 +11,10 @@ index. Every iteration then runs, alternately first and second, ConstructGraph (
 single-GPU graph build over the same sets and indexes with SGPU_TRACE on, whose junction, unitig and loop marks are summed. The
 warm-up iteration checks that both give a GFA with the same SHA-256. One JSON line: medians over the timed iterations, the card's
 name and power limit, and the context's device high-water mark over the whole run.
+
+--early-tc L / --early-at run the early tip clipper with length bound L / the A/T clipper (default parameters) in both builds. The
+line then also holds the distributed clipper phases (their sum as clipper_ms) next to the single-GPU build's "early clippers" mark
+over the same sets, and both builds' GFA SHA-256s.
 """
 import argparse
 import json
@@ -55,7 +59,11 @@ def main():
     ap.add_argument("--buckets", type=int, default=80)
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--iters", type=int, default=3)
+    ap.add_argument("--early-tc", type=int, default=0)
+    ap.add_argument("--early-at", action="store_true")
     args = ap.parse_args()
+    clip = bool(args.early_tc or args.early_at)
+    CLIP_PHASES = ("at_edges_probe", "at_edges_apply", "at_tips_probe", "tip_probe", "isolate", "unlink")
     os.environ["SGPU_TRACE"] = "1"              # read once by the library, at its first trace mark
     import ctypes as C
     import hashlib
@@ -92,8 +100,12 @@ def main():
         return r, (time.perf_counter() - t0) * 1e3
 
     def distributed(row, check):
-        dg, t = clock(lambda: DistributedGraphConstructor(ctx, ext, mkp, mk).ConstructGraph())
+        dg, t = clock(lambda: DistributedGraphConstructor(ctx, ext, mkp, mk).ConstructGraph(early_tip_clipper_length=args.early_tc,
+                                                                                         early_at_clipper=args.early_at))
         row.update(construct_ms=t, construct_phases_ms=dg.times())
+        if clip:
+            row["clipper_phases_ms"] = dg.clipper_times()
+            row["clipper_ms"] = sum(row["clipper_phases_ms"].values())
         if check:
             ag = assemble_graph(dg)
             row["_dist"] = hashlib.sha256(ag.gfa().encode()).hexdigest()
@@ -101,17 +113,19 @@ def main():
         dg.free()
 
     def single(row, check):
-        opts = SgpuGraphOptions(1, 0, 0, 0.8, 10, 200)
+        opts = SgpuGraphOptions(1, args.early_tc, 1 if args.early_at else 0, 0.8, 10, 200)
         h = C.c_void_p()
         _, marks = traced(lambda: ctx.check(ctx.L.sgpu_graph_build_opts(ctx.h, kp.h, km.h, mk.h, mkp.h, C.byref(opts), C.byref(h))))
         g = DeBruijnGraph(ctx, h, kp, km, mk, mkp)
         # the unitig and loop phases: everything after the early clippers' mark, up to the end of the build
         row.update(single_gpu_unitigs_ms=sum(marks.get(m, 0.0) for m in SINGLE_MARKS), single_gpu_marks_ms=marks)
+        if clip:
+            row["single_gpu_clipper_ms"] = marks.get("early clippers", 0.0)
         if check:
             row["_single"] = hashlib.sha256(g.gfa().encode()).hexdigest()
         g.free()
 
-    runs, same, sha = [], None, None
+    runs, same, sha, sha_single = [], None, None, None
     for it in range(args.warmup + args.iters):
         row = {}
         check = it == 0
@@ -120,8 +134,8 @@ def main():
         else:
             distributed(row, check); single(row, check)
         if check:
-            sha = row.pop("_dist")
-            same = sha == row.pop("_single")
+            sha, sha_single = row.pop("_dist"), row.pop("_single")
+            same = sha == sha_single
         if it >= args.warmup:
             runs.append(row)
     med = lambda xs: float(np.median(xs))     # noqa: E731
@@ -130,6 +144,10 @@ def main():
            "construct_phases_ms": {p: med([r["construct_phases_ms"][p] for r in runs]) for p in runs[0]["construct_phases_ms"]},
            "single_gpu_unitigs_ms": med([r["single_gpu_unitigs_ms"] for r in runs]),
            "gfa_sha256": sha, "same_gfa_as_single_gpu": same, "peak_bytes": ctx.times()["peak_bytes"], "runs": runs}
+    if clip:
+        out.update(early_tc=args.early_tc, early_at=args.early_at, clipper_ms=med([r["clipper_ms"] for r in runs]),
+                   clipper_phases_ms={p: med([r["clipper_phases_ms"][p] for r in runs]) for p in CLIP_PHASES},
+                   single_gpu_clipper_ms=med([r["single_gpu_clipper_ms"] for r in runs]), gfa_sha256_single_gpu=sha_single)
     print(json.dumps({"gpu": BN.gpu_facts(0), "result": out}))
     ext.free(); mk.free(); mkp.free(); km.free(); kp.free()
     ctx.close()

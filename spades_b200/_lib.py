@@ -36,6 +36,9 @@ SYMBOLS = [
     "sgpu_dist_graph_begin", "sgpu_dist_graph_ipc_handle", "sgpu_dist_graph_open_peers", "sgpu_dist_graph_unitigs", "sgpu_dist_graph_clear_visited",
     "sgpu_dist_graph_loops", "sgpu_dist_graph_stats", "sgpu_dist_graph_edges", "sgpu_dist_graph_bucket_counts", "sgpu_dist_graph_times",
     "sgpu_dist_graph_free", "sgpu_graph_from_edges",
+    "sgpu_dist_graph_begin_opts", "sgpu_dist_graph_at_edges_probe", "sgpu_dist_graph_at_edges_apply", "sgpu_dist_graph_at_tips_probe",
+    "sgpu_dist_graph_tip_probe", "sgpu_dist_graph_isolate", "sgpu_dist_graph_unlink", "sgpu_dist_graph_junctions", "sgpu_dist_graph_masks",
+    "sgpu_dist_graph_clipper_stats", "sgpu_dist_graph_clipper_times",
     "sgpu_selftest",
 ]
 
@@ -187,6 +190,13 @@ def load():
     L.sgpu_dist_ext_free.restype = None; L.sgpu_dist_ext_free.argtypes = [vp]
     L.sgpu_dist_ext_plan_host.restype = i32; L.sgpu_dist_ext_plan_host.argtypes = [i32, i32, vp, vp, u64, i32, vp, C.POINTER(u64)]
     L.sgpu_dist_graph_begin.restype = i32; L.sgpu_dist_graph_begin.argtypes = [vp, vp, vp, vp, vp, u64, pp]
+    L.sgpu_dist_graph_begin_opts.restype = i32; L.sgpu_dist_graph_begin_opts.argtypes = [vp, vp, vp, vp, vp, u64, C.POINTER(SgpuGraphOptions), pp]
+    for name in ("at_edges_probe", "at_edges_apply", "at_tips_probe", "tip_probe", "isolate", "unlink", "junctions"):
+        f = getattr(L, "sgpu_dist_graph_" + name)
+        f.restype = i32; f.argtypes = [vp]
+    L.sgpu_dist_graph_masks.restype = i32; L.sgpu_dist_graph_masks.argtypes = [vp, vp, i64]
+    L.sgpu_dist_graph_clipper_stats.restype = i32; L.sgpu_dist_graph_clipper_stats.argtypes = [vp, vp, vp, vp]
+    L.sgpu_dist_graph_clipper_times.restype = i32; L.sgpu_dist_graph_clipper_times.argtypes = [vp, vp]
     L.sgpu_dist_graph_ipc_handle.restype = i32; L.sgpu_dist_graph_ipc_handle.argtypes = [vp, vp]
     L.sgpu_dist_graph_open_peers.restype = i32; L.sgpu_dist_graph_open_peers.argtypes = [vp, vp]
     L.sgpu_dist_graph_unitigs.restype = i32; L.sgpu_dist_graph_unitigs.argtypes = [vp]

@@ -408,6 +408,17 @@ void sgpu_mphf_free(sgpu_mphf *m) {
 
 extern "C" {
 
+// the options of a graph build, refused with SGPU_EINVAL as sgpu_graph_build_opts documents (throws)
+static GraphOptions graph_options(const sgpu_graph_options *o) {
+    SG_CHECK(!o->early_at_clipper || (o->at_ratio > 0.0 && o->at_ratio <= 1.0 && o->at_max_length >= 1), SGPU_EINVAL, "bad A/T clipper parameters");
+    GraphOptions opt;
+    opt.keep_perfect_loops = o->keep_perfect_loops != 0;
+    opt.early_tip_length_bound = o->early_tip_length_bound;
+    opt.early_at = o->early_at_clipper != 0;
+    opt.at_ratio = o->at_ratio; opt.at_min_len = o->at_min_length; opt.at_max_len = o->at_max_length;
+    return opt;
+}
+
 int sgpu_graph_build(sgpu_ctx *ctx, const sgpu_kset *kpomers, const sgpu_kset *kmers, const sgpu_mphf *kmer_index, const sgpu_mphf *kpomer_index,
                      int keep_perfect_loops, sgpu_graph **out) {
     const sgpu_graph_options o = {keep_perfect_loops, 0, 0, 0.8, 10, 200};
@@ -431,13 +442,8 @@ int sgpu_graph_build_streamed(sgpu_ctx *ctx, const sgpu_kset *kpomers, const sgp
     *out = nullptr;
     Ctx *c = &ctx->c;
     API_TRY(c, {
-        SG_CHECK(!o->early_at_clipper || (o->at_ratio > 0.0 && o->at_ratio <= 1.0 && o->at_max_length >= 1), SGPU_EINVAL, "bad A/T clipper parameters");
+        const GraphOptions opt = graph_options(o);
         SG_CUDA(cudaSetDevice(c->device));
-        GraphOptions opt;
-        opt.keep_perfect_loops = o->keep_perfect_loops != 0;
-        opt.early_tip_length_bound = o->early_tip_length_bound;
-        opt.early_at = o->early_at_clipper != 0;
-        opt.at_ratio = o->at_ratio; opt.at_min_len = o->at_min_length; opt.at_max_len = o->at_max_length;
         Graph *g = graph_build(c, kpomers->s, kmers->s, kmer_index->m, kpomer_index ? kpomer_index->m : nullptr, opt);
         *out = new sgpu_graph{g};
         child_add(c);
@@ -807,12 +813,18 @@ struct sgpu_dist_graph { DistGraph *d; Ctx *c; };
 extern "C" {
 int sgpu_dist_graph_begin(sgpu_ctx *ctx, const sgpu_dist_ext *ext, const int32_t *kmer_owners, const int32_t *kpomer_owners,
                           const uint64_t *kmer_bucket_sizes, uint64_t budget_bytes, sgpu_dist_graph **out) {
-    if (!ctx || !ext || !kmer_owners || !kmer_bucket_sizes || !out) return SGPU_EINVAL;
+    const sgpu_graph_options o = {1, 0, 0, 0.8, 10, 200};
+    return sgpu_dist_graph_begin_opts(ctx, ext, kmer_owners, kpomer_owners, kmer_bucket_sizes, budget_bytes, &o, out);
+}
+int sgpu_dist_graph_begin_opts(sgpu_ctx *ctx, const sgpu_dist_ext *ext, const int32_t *kmer_owners, const int32_t *kpomer_owners,
+                               const uint64_t *kmer_bucket_sizes, uint64_t budget_bytes, const sgpu_graph_options *o, sgpu_dist_graph **out) {
+    if (!ctx || !ext || !kmer_owners || !kmer_bucket_sizes || !o || !out) return SGPU_EINVAL;
     *out = nullptr;
     Ctx *c = &ctx->c;
     API_TRY(c, {
+        const GraphOptions opt = graph_options(o);
         SG_CUDA(cudaSetDevice(c->device));
-        DistGraph *d = dgraph_begin(c, ext->d, kmer_owners, kpomer_owners, kmer_bucket_sizes, budget_bytes);
+        DistGraph *d = dgraph_begin(c, ext->d, kmer_owners, kpomer_owners, kmer_bucket_sizes, budget_bytes, opt);
         *out = new sgpu_dist_graph{d, c};
         child_add(c);
     })
@@ -824,6 +836,30 @@ int sgpu_dist_graph_ipc_handle(sgpu_dist_graph *d, uint8_t *out) {
 int sgpu_dist_graph_open_peers(sgpu_dist_graph *d, const uint8_t *descriptors) {
     if (!d || !descriptors) return SGPU_EINVAL;
     API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dgraph_open_peers(d->d, descriptors); })
+}
+static int dist_graph_phase(sgpu_dist_graph *d, int a, int b) {
+    if (!d) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dgraph_clip_phase(d->d, a, b); })
+}
+int sgpu_dist_graph_at_edges_probe(sgpu_dist_graph *d) { return dist_graph_phase(d, kAtEdgesProbe, kAtEdgesProbe); }
+int sgpu_dist_graph_at_edges_apply(sgpu_dist_graph *d) { return dist_graph_phase(d, kAtEdgesApply, kAtEdgesApply); }
+int sgpu_dist_graph_at_tips_probe(sgpu_dist_graph *d) { return dist_graph_phase(d, kAtTipsProbe, kAtTipsProbe); }
+int sgpu_dist_graph_tip_probe(sgpu_dist_graph *d) { return dist_graph_phase(d, kTipProbe, kTipProbe); }
+int sgpu_dist_graph_isolate(sgpu_dist_graph *d) { return dist_graph_phase(d, kAtIsolate, kTipIsolate); }
+int sgpu_dist_graph_unlink(sgpu_dist_graph *d) { return dist_graph_phase(d, kAtUnlink, kTipUnlink); }
+int sgpu_dist_graph_junctions(sgpu_dist_graph *d) { return dist_graph_phase(d, kJunctions, kJunctions); }
+int sgpu_dist_graph_masks(const sgpu_dist_graph *d, uint8_t *out, int64_t n) {
+    if (!d || n < 0 || (n && !out)) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dgraph_masks(d->d, out, n); })
+}
+int sgpu_dist_graph_clipper_stats(const sgpu_dist_graph *d, uint64_t *at4, uint64_t *tc3, uint64_t *remote3) {
+    if (!d || !at4 || !tc3 || !remote3) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dgraph_clip_stats(d->d, at4, tc3, remote3); })
+}
+int sgpu_dist_graph_clipper_times(const sgpu_dist_graph *d, float *out6) {
+    if (!d || !out6) return SGPU_EINVAL;
+    dgraph_clip_times(d->d, out6);
+    return SGPU_OK;
 }
 int sgpu_dist_graph_unitigs(sgpu_dist_graph *d) {
     if (!d) return SGPU_EINVAL;

@@ -120,222 +120,45 @@ __global__ void masks_clear_visited_k(uint8_t *__restrict__ masks, const uint8_t
     if (b && (threadIdx.x & 31) == 0) atomicAdd(remaining, (unsigned long long)__popc(b));
 }
 
-// ---- early tip clipper -------------------------------------------------------------------------------------------------
-// EarlyTipClipperProcessor (assembly_graph/construction/early_simplification.hpp:38-162), run by the pipeline between the
-// mask fill and the unitig extraction (stages/construction.cpp:289-302, length bound = read length - k). The reference walks
-// the junctions one after the other (or racily from several threads) on the live index; the result does not depend on the
-// order (a tip's vertices are reachable from exactly one junction orientation and removals only zero tip vertices -- checked
-// against the unmodified reference with 1 and 8 threads and against the oracle's sequential and snapshot modes, tests/), so
-// here every (k-mer, orientation) with >= 2 outgoing edges is one thread on a snapshot of the masks:
-//   tc_probe_k  FindForward per outgoing edge (:115-125), RemoveTips decision (:133-155), marks the vertices to isolate
-//   tc_apply_k  IsolateVertex for the marked vertices
-//   tc_links_k  RemoveInconsistentForwardLinks over the tipped junctions (:21-36) on the updated masks
-template <int NW, bool MARK>
-__device__ __forceinline__ uint32_t tc_find_forward(const MphfDev &mk, const uint8_t *masks, int K, Kmer<NW> kh, uint32_t bound, uint8_t *mark) {
-    uint32_t n = 0;
-    for (;;) {
-        uint64_t idx;
-        const uint8_t m = oriented_mask<NW>(LocalView{mk, masks}, kh, K, &idx);
-        const int uo = uniq4(m & 15), ui = uniq4(m >> 4);
-        if (MARK) mark[idx] = 1;
-        if (!(n < bound && ui >= 0 && uo >= 0)) {
-            ++n;                                                 // tip.push_back(kh) after the loop (:121)
-            return (ui < 0 || (m & 15) != 0) ? 0u : n;           // branching / not a dead end -> not a tip (:122-125)
-        }
-        ++n;
-        kmer_shl<NW>(kh, K, uo);
-    }
-}
+// ---- early clippers (graph_dev.cuh) over this GPU's index and masks ---------------------------------------------------------
 template <int NW>
 __global__ void tc_probe_k(const uint64_t *__restrict__ keys, int64_t base, int64_t n, int K, MphfDev mk, const uint8_t *__restrict__ masks, uint32_t bound,
                            uint8_t *__restrict__ mark, uint8_t *__restrict__ tipped /*[2 * all k-mers]*/, unsigned long long *__restrict__ stats) {
-    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (tid >= 2 * n) return;
-    const Kmer<NW> key = key_at<NW>(keys, tid >> 1);
-    tipped += 2 * base;
-    const int o = (int)(tid & 1);
-    const uint8_t mfw = masks[mphf_lookup_dev<NW>(mk, key)];
-    const uint8_t m = o ? inv_byte(mfw) : mfw;
-    tipped[tid] = 0;
-    if (__popc(m & 15) < 2) return;                              // OutgoingEdgeCount(kh) >= 2 (:72)
-    const Kmer<NW> kh = o ? kmer_rc<NW>(key, K) : key;
-    uint32_t sz[4] = {0, 0, 0, 0}, mx = 0;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-        if (!(m & (1u << c))) continue;
-        Kmer<NW> khc = kh;
-        kmer_shl<NW>(khc, K, c);
-        sz[c] = tc_find_forward<NW, false>(mk, masks, K, khc, bound, nullptr);
-        const uint32_t len = sz[c] ? sz[c] : 0xffffffffu;
-        if (len > mx) mx = len;
-    }
-    uint32_t removed = 0;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-        if (!sz[c] || sz[c] >= mx) continue;                     // RemoveTips: tip.size() < max (:136-141)
-        Kmer<NW> khc = kh;
-        kmer_shl<NW>(khc, K, c);
-        tc_find_forward<NW, true>(mk, masks, K, khc, bound, mark);
-        removed += sz[c];
-    }
-    if (removed) { tipped[tid] = 1; atomicAdd(&stats[0], (unsigned long long)removed); atomicAdd(&stats[1], 1ull); }
+    LocalView v{mk, masks};
+    v.marks = mark;
+    tc_probe<NW>(v, keys, base, n, K, bound, tipped, stats);
 }
 __global__ void tc_apply_k(uint8_t *__restrict__ masks, const uint8_t *__restrict__ mark, uint64_t n) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n && mark[i]) masks[i] = 0;
 }
 template <int NW>
-// flags_by_slot = 0: tipped[] is indexed by (k-mer position, orientation), as tc_probe_k writes it; 1: by (MPHF slot, orientation),
-// as at_tips_probe_k marks the roots it reaches by walking
 __global__ void tc_links_k(const uint64_t *__restrict__ keys, int64_t base, int64_t n, int K, MphfDev mk, uint8_t *__restrict__ masks,
                            const uint8_t *__restrict__ tipped, unsigned long long *__restrict__ stat_clipped, int flags_by_slot) {
-    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (tid >= 2 * n) return;
-    if (!flags_by_slot && !tipped[2 * base + tid]) return;
-    const Kmer<NW> key = key_at<NW>(keys, tid >> 1);
-    const Kmer<NW> kh = (tid & 1) ? kmer_rc<NW>(key, K) : key;
-    const CanonIdx<LocalView> ci = canon_lookup<NW>(LocalView{mk, masks}, kh, K);
-    if (flags_by_slot && !tipped[2 * ci.idx + (uint64_t)(tid & 1)]) return;
-    const uint8_t raw = masks[ci.idx];
-    const uint8_t m = ci.is_min ? raw : inv_byte(raw);
-    const int first = (int)(kh.w[0] & 3);                        // kh[0]
-    for (int c = 0; c < 4; ++c) {
-        if (!(m & (1u << c))) continue;
-        Kmer<NW> nx = kh;
-        kmer_shl<NW>(nx, K, c);
-        if (!(oriented_mask<NW>(LocalView{mk, masks}, nx, K) & (1u << (4 + first)))) {            // !CheckIncoming(next_kh, kh[0])
-            const unsigned bit = 1u << (ci.is_min ? c : 7 - c);                          // DeleteOutgoing(kh, c), inout_mask.hpp:108-114
-            atomicAnd(reinterpret_cast<unsigned *>(masks) + (ci.idx >> 2), ~(bit << (8 * (ci.idx & 3))));
-            atomicAdd(stat_clipped, 1ull);
-        }
-    }
+    LocalView v{mk, masks};
+    v.roots = const_cast<uint8_t *>(tipped);
+    tc_links<NW>(v, keys, base, n, K, tipped, stat_clipped, flags_by_slot);
 }
-
-// ---- early low-complexity (poly A/T) clipper ----------------------------------------------------------------------------------
-// EarlyLowComplexityClipperProcessor (assembly_graph/construction/early_simplification.hpp:164-347), the EarlyATClipper phase of the
-// RNA pipeline (stages/construction.cpp:317-340,447-448: at_ratio 0.8, min_length 10, max_length 200); runs before the tip clipper.
-//   RemoveATEdges (:185-256)  at_edges_probe_k : per (k-mer, orientation) on the untouched masks: junction + low-complexity k-mer ->
-//                                                 the outgoing edges of length 1 (next is a junction or a dead end) are flagged
-//                             at_edges_apply_k : every flagged link is deleted once (the reference deletes it through whichever of
-//                                                 its two representations comes first and skips the other, :237-238: here the
-//                                                 representation with the smaller (thread, nucleotide) pair acts)
-//   RemoveATTips  (:269-334)  at_tips_probe_k  : per dead end with a unique incoming edge: walk back to the junction (<= max_length),
-//                                                 complexity of the tip (+ the root's last nucleotides up to min_length), mark
-//                                                 the vertices and the root. The reference isolates tips while other threads
-//                                                 walk; the result does not depend on the order (tips are disjoint chains whose
-//                                                 decisions read only their own vertices and the root's mask -- checked: unmodified
-//                                                 reference with 1 and 8 threads == oracle sequential == oracle snapshot)
-//                             tc_apply_k, tc_links_k : IsolateVertex, RemoveInconsistentForwardLinks on the updated masks
-__device__ __forceinline__ bool almost_equals_f64(double a, double b) {     // gtest FloatingPoint<double>::AlmostEquals, 4 ULPs (math/xmath.h:283-299)
-    if (a != a || b != b) return false;
-    const unsigned long long x = (unsigned long long)__double_as_longlong(a), y = (unsigned long long)__double_as_longlong(b);
-    const unsigned long long sign = 0x8000000000000000ull;
-    const unsigned long long bx = (x & sign) ? (~x + 1ull) : (sign | x), by = (y & sign) ? (~y + 1ull) : (sign | y);
-    return (bx >= by ? bx - by : by - bx) <= 4ull;
-}
-__device__ __forceinline__ bool math_ls(double a, double b) { return !almost_equals_f64(a, b) && a < b; }      // math::ls, xmath.h:300-306
-__device__ __forceinline__ bool mask_is_junction(uint8_t m) { return uniq4(m & 15) < 0 || uniq4(m >> 4) < 0; }  // InOutMask::IsJunction
-
-struct AtParams { double ratio; uint32_t min_len, max_len; };
-
 template <int NW>
 __global__ void at_edges_probe_k(const uint64_t *__restrict__ keys, int64_t n, int K, MphfDev mk, const uint8_t *__restrict__ masks, AtParams ap,
                                  uint8_t *__restrict__ eflag /*[2 * all k-mers]*/, unsigned long long *__restrict__ stats) {
-    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (tid >= 2 * n) return;
-    const Kmer<NW> key = key_at<NW>(keys, tid >> 1);
-    const int o = (int)(tid & 1);
-    const uint64_t slot = mphf_lookup_dev<NW>(mk, key);
-    const int64_t fid = (int64_t)(2 * slot) + o;                        // flags are indexed by (MPHF slot, orientation), like the masks
-    eflag[fid] = 0;
-    const uint8_t mfw = masks[slot];
-    const uint8_t m = o ? inv_byte(mfw) : mfw;
-    if (!mask_is_junction(m)) return;
-    const Kmer<NW> kh = o ? kmer_rc<NW>(key, K) : key;
-    uint32_t cnt[4] = {0, 0, 0, 0};
-    for (int p = 0; p < K; ++p) cnt[kmer_nuc<NW>(kh, p)]++;
-    const uint32_t curm = max(max(cnt[0], cnt[1]), max(cnt[2], cnt[3]));
-    if (math_ls((double)curm, (double)K * ap.ratio)) return;
-    uint8_t f = 0;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-        if (!(m & (1u << c))) continue;
-        Kmer<NW> nx = kh;
-        kmer_shl<NW>(nx, K, c);
-        const uint8_t mn = oriented_mask<NW>(LocalView{mk, masks}, nx, K);
-        if (!mask_is_junction(mn) && (mn & 15) != 0) continue;          // an edge of length 1: next is a junction or a dead end
-        f |= (uint8_t)(1u << c);
-    }
-    eflag[fid] = f;
-    if (f) atomicAdd(&stats[0], (unsigned long long)__popc(f));
-}
-__device__ __forceinline__ void mask_clear_bit(uint8_t *masks, uint64_t idx, unsigned bit) {
-    atomicAnd(reinterpret_cast<unsigned *>(masks) + (idx >> 2), ~((1u << bit) << (8 * (idx & 3))));
+    LocalView v{mk, masks};
+    v.eflags = eflag;
+    at_edges_probe<NW>(v, keys, n, K, ap, stats);
 }
 template <int NW>
 __global__ void at_edges_apply_k(const uint64_t *__restrict__ keys, int64_t n, int K, MphfDev mk, uint8_t *__restrict__ masks, const uint8_t *__restrict__ eflag,
                                  unsigned long long *__restrict__ stats) {
-    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (tid >= 2 * n) return;
-    const Kmer<NW> key = key_at<NW>(keys, tid >> 1);
-    const Kmer<NW> kh = (tid & 1) ? kmer_rc<NW>(key, K) : key;
-    const CanonIdx<LocalView> ci = canon_lookup<NW>(LocalView{mk, masks}, kh, K);
-    const int64_t fid = (int64_t)(2 * ci.idx) + (tid & 1);               // kh is the table key (minimal form) iff the orientation bit is 0
-    const uint8_t mine = eflag[fid];
-    if (!mine) return;
-    const int first = (int)(kh.w[0] & 3);                                // kh[0]
-    for (int c = 0; c < 4; ++c) {
-        if (!(mine & (1u << c))) continue;
-        Kmer<NW> nx = kh;
-        kmer_shl<NW>(nx, K, c);
-        const CanonIdx<LocalView> cn = canon_lookup<NW>(LocalView{mk, masks}, nx, K);
-        // the same link seen from the other strand: (rc(next), complement of kh[0]); rc(next) is the table key iff next is NOT minimal
-        const int64_t fid2 = (int64_t)(2 * cn.idx) + (cn.is_min ? 1 : 0);
-        const int c2 = 3 - first;
-        if ((eflag[fid2] & (1u << c2)) && (fid2 < fid || (fid2 == fid && c2 < c))) continue;
-        mask_clear_bit(masks, ci.idx, (unsigned)(ci.is_min ? c : 7 - c));                        // DeleteOutgoing(kh, c)
-        mask_clear_bit(masks, cn.idx, (unsigned)(cn.is_min ? 4 + first : 7 - (4 + first)));      // DeleteIncoming(next, kh[0])
-        atomicAdd(&stats[1], 2ull);
-    }
+    LocalView v{mk, masks};
+    v.eflags = const_cast<uint8_t *>(eflag);
+    at_edges_apply<NW>(v, keys, n, K, stats);
 }
 template <int NW>
 __global__ void at_tips_probe_k(const uint64_t *__restrict__ keys, int64_t n, int K, MphfDev mk, const uint8_t *__restrict__ masks, AtParams ap,
                                 uint8_t *__restrict__ mark, uint8_t *__restrict__ rooted /*[2 * all k-mers]*/, unsigned long long *__restrict__ stats) {
-    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (tid >= 2 * n) return;
-    const Kmer<NW> key = key_at<NW>(keys, tid >> 1);
-    const int o = (int)(tid & 1);
-    const uint64_t idx0 = mphf_lookup_dev<NW>(mk, key);
-    const uint8_t mfw = masks[idx0];
-    const uint8_t m0 = o ? inv_byte(mfw) : mfw;
-    if ((m0 & 15) != 0 || uniq4(m0 >> 4) < 0) return;                   // IsDeadEnd && CheckUniqueIncoming
-    const Kmer<NW> start = o ? kmer_rc<NW>(key, K) : key;
-    Kmer<NW> kh = start;
-    uint32_t cnt[4] = {0, 0, 0, 0};
-    uint32_t tsz = 0;
-    uint8_t m = m0;
-    do {                                                                 // walk back to the junction, :292-296
-        ++tsz;
-        cnt[kmer_nuc<NW>(kh, K - 1)]++;
-        kmer_shr<NW>(kh, K, uniq4(m >> 4));
-        m = oriented_mask<NW>(LocalView{mk, masks}, kh, K);
-    } while (tsz < ap.max_len && !mask_is_junction(m));
-    if ((m >> 4) == 0 || !mask_is_junction(m)) return;                   // dead start (isolated short edge) or too long, :301-302
-    for (uint32_t p = tsz - 1; p < ap.min_len; ++p) cnt[kmer_nuc<NW>(kh, K - 1 - (int)p)]++;
-    const uint32_t curm = max(max(cnt[0], cnt[1]), max(cnt[2], cnt[3]));
-    if (math_ls((double)curm, (double)max(tsz, ap.min_len) * ap.ratio)) return;
-    // a low-complexity tip: mark its vertices (second walk) and its root
-    const CanonIdx<LocalView> cr = canon_lookup<NW>(LocalView{mk, masks}, kh, K);
-    rooted[2 * cr.idx + (cr.is_min ? 0 : 1)] = 1;
-    Kmer<NW> w = start;
-    uint8_t mw = m0;
-    for (uint32_t s2 = 0; s2 < tsz; ++s2) {
-        uint64_t idx;
-        if (s2) mw = oriented_mask<NW>(LocalView{mk, masks}, w, K, &idx); else idx = idx0;
-        mark[idx] = 1;
-        kmer_shr<NW>(w, K, uniq4(mw >> 4));
-    }
-    atomicAdd(&stats[2], (unsigned long long)tsz);
+    LocalView v{mk, masks};
+    v.marks = mark; v.roots = rooted;
+    at_tips_probe<NW>(v, keys, n, K, ap, stats);
 }
 
 // ---- perfect loops (CollectLoops :359-397) --------------------------------------------------------------------------
@@ -419,6 +242,12 @@ SG_INSTANTIATE_KEYS(2)
 SG_INSTANTIATE_KEYS(3)
 SG_INSTANTIATE_KEYS(4)
 
+void launch_isolate(Ctx *ctx, uint8_t *masks, const uint8_t *mark, uint64_t n) {
+    if (!n) return;
+    tc_apply_k<<<div_up((int64_t)n, 256), 256, 0, ctx->stream>>>(masks, mark, n);
+    ctx->launches++;
+}
+
 void launch_edge_table(Ctx *ctx, const uint32_t *len, const uint64_t *eidx, const uint64_t *eoff, int64_t nslots, uint64_t *out_off, uint32_t *out_len) {
     edge_table_k<<<div_up(nslots, 256), 256, 0, ctx->stream>>>(len, eidx, eoff, nslots, out_off, out_len);
     ctx->launches++;
@@ -493,8 +322,7 @@ struct GraphBuild {
     // tail: IsolateVertex for the marked k-mers, then one tc_links_k sweep (RemoveInconsistentForwardLinks) over the flagged
     // (k-mer, orientation) pairs, which counts the clipped links in stats[links]. Returns the clipper's four counters.
     std::array<unsigned long long, 4> isolate_and_unlink(const uint8_t *mark, const uint8_t *flags, int flags_by_slot, unsigned long long *stats, int links) {
-        tc_apply_k<<<div_up((int64_t)nk, 256), 256, 0, st>>>(g->masks.p, mark, nk);
-        ctx->launches++;
+        launch_isolate(ctx, g->masks.p, mark, nk);
         kmer_sweep([&](const Chunk &c, const uint64_t *keys) {
             tc_links_k<NW><<<div_up(2 * c.n, 128), 128, 0, st>>>(keys, c.first, c.n, K, mk, g->masks.p, flags, stats + links, flags_by_slot);
         });
@@ -507,7 +335,7 @@ struct GraphBuild {
     void at_clipper() {
         if (!opt.early_at || !nk) return;
         SG_CHECK(opt.at_min_len <= (uint64_t)K, 2, "early A/T clipper: min_length must not exceed k (the reference indexes kh[k - 1 - i])");
-        AtParams ap; ap.ratio = opt.at_ratio; ap.min_len = (uint32_t)std::min<uint64_t>(opt.at_min_len, 0x7fffffffu); ap.max_len = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(opt.at_max_len, 1), 0x7fffffffu);
+        const AtParams ap = at_params(opt);
         DArr<uint8_t> eflag(ctx, 2 * nk + 8), mark(ctx, nk + 8);
         DArr<uint8_t> rooted(ctx, 2 * nk + 8);
         DArr<unsigned long long> stats(ctx, 4);
@@ -534,7 +362,7 @@ struct GraphBuild {
         DArr<unsigned long long> stats(ctx, 4);
         SG_CUDA(cudaMemsetAsync(mark.p, 0, mark.bytes(), st));
         SG_CUDA(cudaMemsetAsync(stats.p, 0, 32, st));
-        const uint32_t bound = (uint32_t)std::min<uint64_t>(opt.early_tip_length_bound, 0x7fffffffu);
+        const uint32_t bound = tip_bound(opt);
         kmer_sweep([&](const Chunk &c, const uint64_t *keys) {
             tc_probe_k<NW><<<div_up(2 * c.n, 128), 128, 0, st>>>(keys, c.first, c.n, K, mk, g->masks.p, bound, mark.p, tipped.p, stats.p);
         });

@@ -40,14 +40,20 @@ std::vector<uint64_t> graph_histogram(Ctx *ctx, const Graph *g);
 void coverage_fill(Ctx *ctx, ChunkStager &kpomers, const Mphf *mkp, uint32_t *cov);
 std::vector<uint64_t> coverage_histogram(Ctx *ctx, const uint32_t *cov, int64_t n);
 
-// dist_graph.cu : the unitigs and perfect loops of one rank's share of a distributed graph (DistributedGraphConstructor), from its
-// extension index slices (dist_ext.cu). Phases, with a barrier between them: begin (a working copy of the masks, the junction
-// list), ipc_handle / open_peers, unitigs, clear_visited, ipc_handle / open_peers again (the remaining slots' positions), loops.
+// dist_graph.cu : the early clippers, unitigs and perfect loops of one rank's share of a distributed graph
+// (DistributedGraphConstructor), from its extension index slices (dist_ext.cu). Phases, with a barrier between them: begin (a
+// working copy of the masks; the junction list when no clipper is on), ipc_handle / open_peers, the clippers' phases and the
+// junction list (dgraph_clip_phase), unitigs, clear_visited, ipc_handle / open_peers again (the remaining slots' positions), loops.
 struct DistGraph;
 struct ExtDist;
-DistGraph *dgraph_begin(Ctx *ctx, const ExtDist *ext, const int *kmer_owner, const int *kpomer_owner, const uint64_t *kmer_bucket_sizes, uint64_t budget);
+DistGraph *dgraph_begin(Ctx *ctx, const ExtDist *ext, const int *kmer_owner, const int *kpomer_owner, const uint64_t *kmer_bucket_sizes, uint64_t budget,
+                        const GraphOptions &opt);
 void dgraph_ipc_handle(DistGraph *d, uint8_t *out256);
 void dgraph_open_peers(DistGraph *d, const uint8_t *descs);
+// the phases between begin and the unitigs, in the order they run (a clipper's phases only when it is on)
+enum { kAtEdgesProbe, kAtEdgesApply, kAtTipsProbe, kAtIsolate, kAtUnlink, kTipProbe, kTipIsolate, kTipUnlink, kJunctions };
+// the next of them, when it is phase a or b; refuses any other
+void dgraph_clip_phase(DistGraph *d, int a, int b);
 void dgraph_unitigs(DistGraph *d);
 void dgraph_clear_visited(DistGraph *d);
 void dgraph_loops(DistGraph *d);
@@ -55,6 +61,9 @@ const Graph &dgraph_edges(const DistGraph *d);                   // its unitigs 
 void dgraph_stats(const DistGraph *d, uint64_t *out4);           // edges, unitig edges, bases, junction batches
 void dgraph_bucket_counts(const DistGraph *d, uint64_t *unitigs, uint64_t *loops);
 void dgraph_times(const DistGraph *d, float *out4);
+void dgraph_clip_times(const DistGraph *d, float *out6);         // A/T edges probe, A/T edges apply, A/T tips probe, tip probe, isolate, unlink
+void dgraph_clip_stats(const DistGraph *d, uint64_t *at4, uint64_t *tc3, uint64_t *remote3);
+void dgraph_masks(const DistGraph *d, uint8_t *out, int64_t n);  // the clipped slice (the extension index's when no clipper ran)
 void dgraph_free(DistGraph *d);
 
 // edge_index.cu : KmerFreeEdgeIndex refill over the graph's own unitigs (alignment/edge_index.hpp, assembly_graph/index/edge_index_builders.hpp)

@@ -5,6 +5,7 @@
 //   DistView   one rank of many: a bucket's owner, the owner's index rows (copied locally) and its arrays as this process maps them.
 // The walk bodies are device functions templated on the view; each translation unit wraps them in kernels of its own.
 #pragma once
+#include <algorithm>
 #include <functional>
 
 #include "graph.h"
@@ -50,10 +51,18 @@ struct RemSlots {
     }
 };
 
+// DeleteOutgoing / DeleteIncoming: clears bit `bit` of mask byte idx with a 32-bit atomic on the word that holds it
+__device__ __forceinline__ void mask_clear_bit(uint8_t *masks, uint64_t idx, unsigned bit) {
+    atomicAnd(reinterpret_cast<unsigned *>(masks) + (idx >> 2), ~((1u << bit) << (8 * (idx & 3))));
+}
+
 // ---- views -----------------------------------------------------------------------------------------------------------------
 // Ref: where a k-mer's byte lives. slot(key of minimal form) -> Ref; mask / visit / rem_rank / rem_pos read or mark it;
 // link_idx(Ref) is the slot a link record carries; upos(Ref, p) turns the final_kmers position p of that k-mer in the set that
 // holds it into its position in the union's; lost(m): the walk cannot go on from mask m (only a view that can miss says so).
+// The early clippers' flags: mark(Ref) sets a k-mer's IsolateVertex flag, root(Ref, o) / is_root the flag of the (slot,
+// orientation) a clipped A/T tip hangs from, eflag / set_eflag the A/T edge flags of a (slot, orientation), clear_bit(Ref, bit)
+// deletes one edge of a k-mer's mask.
 struct LocalView {
     MphfDev mk;
     const uint8_t *masks;
@@ -62,6 +71,9 @@ struct LocalView {
     uint8_t *visited;
     RemSlots rs;
     const uint64_t *pos;
+    uint8_t *marks;            // the clippers' flags, per slot (marks) or per (slot, orientation)
+    uint8_t *eflags;
+    uint8_t *roots;
     typedef uint64_t Ref;
     template <int NW>
     __device__ __forceinline__ Ref slot(const Kmer<NW> &key) const { return mphf_lookup_dev<NW>(mk, key); }
@@ -75,21 +87,30 @@ struct LocalView {
     __device__ __forceinline__ uint64_t rem_pos(Ref, uint64_t rk) const { return pos[rk]; }
     __device__ __forceinline__ uint64_t upos(Ref, uint64_t p) const { return p; }
     __device__ __forceinline__ bool lost(uint8_t) const { return false; }
+    __device__ __forceinline__ void mark(Ref r) const { marks[r] = 1; }
+    __device__ __forceinline__ void root(Ref r, int o) const { roots[2 * r + o] = 1; }
+    __device__ __forceinline__ bool is_root(Ref r, int o) const { return roots[2 * r + o]; }
+    __device__ __forceinline__ uint8_t eflag(Ref r, int o) const { return eflags[2 * r + o]; }
+    __device__ __forceinline__ void set_eflag(Ref r, int o, uint8_t f) const { eflags[2 * r + o] = f; }
+    // only the clippers clear bits, and their kernels own a writable mask array
+    __device__ __forceinline__ void clear_bit(Ref r, unsigned bit) const { mask_clear_bit(const_cast<uint8_t *>(masks), r, bit); }
 };
 
 // one rank's arrays as this process maps them (its own arena, or a peer's through cudaIpc)
 struct DistPeer {
     const uint64_t *bits, *ranks;          // its k-mer index
-    const uint8_t *masks;                  // its mask slice (the walks' working copy)
+    uint8_t *masks;                        // its mask slice (the clippers' and the walks' working copy)
     uint8_t *visited;                      // its visited slice
     const uint64_t *pbits, *pranks;        // its (k+1)-mer index
     const uint32_t *cov;                   // its coverage slice
     const uint32_t *rem_bits;              // its remaining-slot tables (RemSlots) and their final_kmers positions
     const uint64_t *rem_base, *rem_pos;
+    uint8_t *mark, *eflag, *rooted;        // its clipper flags: per owned slot, per (owned slot, orientation) twice
 };
 // A k-mer's bucket b names its owner; the owner's index rows of bucket b (dom, woff for every level, its first slot lstart[b])
 // are copied here, so a lookup reads only the owner's bits and ranks remotely. The union's slot and final_kmers position are the
-// owner's shifted by ustart[b] - lstart[b]. A lookup no level answers counts in *err and ends the walk.
+// owner's shifted by ustart[b] - lstart[b]. A lookup no level answers counts in *err and ends the walk. The clippers' stores and
+// bit clears act on the owner's slice; those that land in another rank's slice are counted in remote[0, 3) (marks, roots, clears).
 struct DistView {
     const DistPeer *peers;
     const int *owner, *powner;             // B: owner of each k-mer bucket, of each (k+1)-mer bucket
@@ -98,6 +119,8 @@ struct DistView {
     uint32_t B;
     bool have_cov;
     unsigned long long *err;
+    int self;                              // this rank
+    unsigned long long *remote;
     struct Ref { uint64_t slot; uint32_t b; int g; };   // slot: in the owner's index, ~0 after a miss
     template <int NW>
     __device__ __forceinline__ Ref slot(const Kmer<NW> &key) const {
@@ -130,6 +153,25 @@ struct DistView {
     __device__ __forceinline__ uint64_t rem_pos(const Ref &r, uint64_t rk) const { return upos(r, peers[r.g].rem_pos[rk]); }
     __device__ __forceinline__ uint64_t upos(const Ref &r, uint64_t p) const { return ustart[r.b] + (p - lstart[r.b]); }
     __device__ __forceinline__ bool lost(uint8_t m) const { return uniq4(m & 15) < 0; }
+    __device__ __forceinline__ void mark(const Ref &r) const {
+        if (r.slot == ~0ull) return;
+        peers[r.g].mark[r.slot] = 1;
+        if (r.g != self) atomicAdd(&remote[0], 1ull);
+    }
+    __device__ __forceinline__ void root(const Ref &r, int o) const {
+        if (r.slot == ~0ull) return;
+        peers[r.g].rooted[2 * r.slot + o] = 1;
+        if (r.g != self) atomicAdd(&remote[1], 1ull);
+    }
+    __device__ __forceinline__ bool is_root(const Ref &r, int o) const { return r.slot != ~0ull && peers[r.g].rooted[2 * r.slot + o]; }
+    __device__ __forceinline__ uint8_t eflag(const Ref &r, int o) const { return r.slot == ~0ull ? 0 : peers[r.g].eflag[2 * r.slot + o]; }
+    __device__ __forceinline__ void set_eflag(const Ref &r, int o, uint8_t f) const { if (r.slot != ~0ull) peers[r.g].eflag[2 * r.slot + o] = f; }
+    // across devices, a 32-bit atomic on a peer's memory needs native peer atomics (dgraph_open_peers checks them)
+    __device__ __forceinline__ void clear_bit(const Ref &r, unsigned bit) const {
+        if (r.slot == ~0ull) return;
+        mask_clear_bit(peers[r.g].masks, r.slot, bit);
+        if (r.g != self) atomicAdd(&remote[2], 1ull);
+    }
 };
 
 // ---- lookups through a view --------------------------------------------------------------------------------------------------
@@ -441,7 +483,226 @@ __device__ __forceinline__ void loop_write(V vw, const LoopInfo *info, int64_t n
     }
 }
 
+// ---- early tip clipper -------------------------------------------------------------------------------------------------
+// EarlyTipClipperProcessor (assembly_graph/construction/early_simplification.hpp:38-162), run by the pipeline between the
+// mask fill and the unitig extraction (stages/construction.cpp:289-302, length bound = read length - k). The reference walks
+// the junctions one after the other (or racily from several threads) on the live index; the result does not depend on the
+// order (a tip's vertices are reachable from exactly one junction orientation and removals only zero tip vertices -- checked
+// against the unmodified reference with 1 and 8 threads and against the oracle's sequential and snapshot modes, tests/), so
+// here every (k-mer, orientation) with >= 2 outgoing edges is one thread on a snapshot of the masks:
+//   tc_probe   FindForward per outgoing edge (:115-125), RemoveTips decision (:133-155), marks the vertices to isolate
+//   tc_apply_k IsolateVertex for the marked vertices (graph.cu, over one array of marks)
+//   tc_links   RemoveInconsistentForwardLinks over the tipped junctions (:21-36) on the updated masks
+template <int NW, bool MARK, class V>
+__device__ __forceinline__ uint32_t tc_find_forward(const V &v, int K, Kmer<NW> kh, uint32_t bound) {
+    uint32_t n = 0;
+    for (;;) {
+        typename V::Ref idx;
+        const uint8_t m = oriented_mask<NW>(v, kh, K, &idx);
+        const int uo = uniq4(m & 15), ui = uniq4(m >> 4);
+        if (MARK) v.mark(idx);
+        if (!(n < bound && ui >= 0 && uo >= 0)) {
+            ++n;                                                 // tip.push_back(kh) after the loop (:121)
+            return (ui < 0 || (m & 15) != 0) ? 0u : n;           // branching / not a dead end -> not a tip (:122-125)
+        }
+        ++n;
+        kmer_shl<NW>(kh, K, uo);
+    }
+}
+// tipped: per (k-mer position of the keys' set, orientation), base = the position of keys[0]
+template <int NW, class V>
+__device__ __forceinline__ void tc_probe(const V &v, const uint64_t *keys, int64_t base, int64_t n, int K, uint32_t bound, uint8_t *tipped,
+                                         unsigned long long *stats) {
+    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (tid >= 2 * n) return;
+    const Kmer<NW> key = key_at<NW>(keys, tid >> 1);
+    tipped += 2 * base;
+    const int o = (int)(tid & 1);
+    const uint8_t mfw = v.mask(v.template slot<NW>(key));
+    const uint8_t m = o ? inv_byte(mfw) : mfw;
+    tipped[tid] = 0;
+    if (__popc(m & 15) < 2) return;                              // OutgoingEdgeCount(kh) >= 2 (:72)
+    const Kmer<NW> kh = o ? kmer_rc<NW>(key, K) : key;
+    uint32_t sz[4] = {0, 0, 0, 0}, mx = 0;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+        if (!(m & (1u << c))) continue;
+        Kmer<NW> khc = kh;
+        kmer_shl<NW>(khc, K, c);
+        sz[c] = tc_find_forward<NW, false>(v, K, khc, bound);
+        const uint32_t len = sz[c] ? sz[c] : 0xffffffffu;
+        if (len > mx) mx = len;
+    }
+    uint32_t removed = 0;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+        if (!sz[c] || sz[c] >= mx) continue;                     // RemoveTips: tip.size() < max (:136-141)
+        Kmer<NW> khc = kh;
+        kmer_shl<NW>(khc, K, c);
+        tc_find_forward<NW, true>(v, K, khc, bound);
+        removed += sz[c];
+    }
+    if (removed) { tipped[tid] = 1; atomicAdd(&stats[0], (unsigned long long)removed); atomicAdd(&stats[1], 1ull); }
+}
+// flags_by_slot = 0: tipped[] is indexed by (k-mer position, orientation), as tc_probe writes it; 1: the view's root flags, by
+// (slot, orientation), as at_tips_probe sets them by walking. The bits it clears are those of its own k-mer.
+template <int NW, class V>
+__device__ __forceinline__ void tc_links(const V &v, const uint64_t *keys, int64_t base, int64_t n, int K, const uint8_t *tipped,
+                                         unsigned long long *stat_clipped, int flags_by_slot) {
+    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (tid >= 2 * n) return;
+    if (!flags_by_slot && !tipped[2 * base + tid]) return;
+    const Kmer<NW> key = key_at<NW>(keys, tid >> 1);
+    const Kmer<NW> kh = (tid & 1) ? kmer_rc<NW>(key, K) : key;
+    const CanonIdx<V> ci = canon_lookup<NW>(v, kh, K);
+    if (flags_by_slot && !v.is_root(ci.idx, (int)(tid & 1))) return;
+    const uint8_t raw = v.mask(ci.idx);
+    const uint8_t m = ci.is_min ? raw : inv_byte(raw);
+    const int first = (int)(kh.w[0] & 3);                        // kh[0]
+    for (int c = 0; c < 4; ++c) {
+        if (!(m & (1u << c))) continue;
+        Kmer<NW> nx = kh;
+        kmer_shl<NW>(nx, K, c);
+        if (!(oriented_mask<NW>(v, nx, K) & (1u << (4 + first)))) {                  // !CheckIncoming(next_kh, kh[0])
+            v.clear_bit(ci.idx, (unsigned)(ci.is_min ? c : 7 - c));                  // DeleteOutgoing(kh, c), inout_mask.hpp:108-114
+            atomicAdd(stat_clipped, 1ull);
+        }
+    }
+}
+
+// ---- early low-complexity (poly A/T) clipper ----------------------------------------------------------------------------------
+// EarlyLowComplexityClipperProcessor (assembly_graph/construction/early_simplification.hpp:164-347), the EarlyATClipper phase of the
+// RNA pipeline (stages/construction.cpp:317-340,447-448: at_ratio 0.8, min_length 10, max_length 200); runs before the tip clipper.
+//   RemoveATEdges (:185-256)  at_edges_probe : per (k-mer, orientation) on the untouched masks: junction + low-complexity k-mer ->
+//                                               the outgoing edges of length 1 (next is a junction or a dead end) are flagged
+//                             at_edges_apply : every flagged link is deleted once (the reference deletes it through whichever of
+//                                               its two representations comes first and skips the other, :237-238: here the
+//                                               representation with the smaller (union slot, orientation, nucleotide) acts)
+//   RemoveATTips  (:269-334)  at_tips_probe  : per dead end with a unique incoming edge: walk back to the junction (<= max_length),
+//                                               complexity of the tip (+ the root's last nucleotides up to min_length), mark
+//                                               the vertices and the root. The reference isolates tips while other threads
+//                                               walk; the result does not depend on the order (tips are disjoint chains whose
+//                                               decisions read only their own vertices and the root's mask -- checked: unmodified
+//                                               reference with 1 and 8 threads == oracle sequential == oracle snapshot)
+//                             tc_apply_k, tc_links : IsolateVertex, RemoveInconsistentForwardLinks on the updated masks
+__device__ __forceinline__ bool almost_equals_f64(double a, double b) {     // gtest FloatingPoint<double>::AlmostEquals, 4 ULPs (math/xmath.h:283-299)
+    if (a != a || b != b) return false;
+    const unsigned long long x = (unsigned long long)__double_as_longlong(a), y = (unsigned long long)__double_as_longlong(b);
+    const unsigned long long sign = 0x8000000000000000ull;
+    const unsigned long long bx = (x & sign) ? (~x + 1ull) : (sign | x), by = (y & sign) ? (~y + 1ull) : (sign | y);
+    return (bx >= by ? bx - by : by - bx) <= 4ull;
+}
+__device__ __forceinline__ bool math_ls(double a, double b) { return !almost_equals_f64(a, b) && a < b; }      // math::ls, xmath.h:300-306
+__device__ __forceinline__ bool mask_is_junction(uint8_t m) { return uniq4(m & 15) < 0 || uniq4(m >> 4) < 0; }  // InOutMask::IsJunction
+
+struct AtParams { double ratio; uint32_t min_len, max_len; };
+inline AtParams at_params(const GraphOptions &o) {
+    AtParams ap;
+    ap.ratio = o.at_ratio;
+    ap.min_len = (uint32_t)std::min<uint64_t>(o.at_min_len, 0x7fffffffu);
+    ap.max_len = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(o.at_max_len, 1), 0x7fffffffu);
+    return ap;
+}
+inline uint32_t tip_bound(const GraphOptions &o) { return (uint32_t)std::min<uint64_t>(o.early_tip_length_bound, 0x7fffffffu); }
+
+template <int NW, class V>
+__device__ __forceinline__ void at_edges_probe(const V &v, const uint64_t *keys, int64_t n, int K, AtParams ap, unsigned long long *stats) {
+    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (tid >= 2 * n) return;
+    const Kmer<NW> key = key_at<NW>(keys, tid >> 1);
+    const int o = (int)(tid & 1);
+    const typename V::Ref slot = v.template slot<NW>(key);      // flags are indexed by (slot, orientation), like the masks
+    v.set_eflag(slot, o, 0);
+    const uint8_t mfw = v.mask(slot);
+    const uint8_t m = o ? inv_byte(mfw) : mfw;
+    if (!mask_is_junction(m)) return;
+    const Kmer<NW> kh = o ? kmer_rc<NW>(key, K) : key;
+    uint32_t cnt[4] = {0, 0, 0, 0};
+    for (int p = 0; p < K; ++p) cnt[kmer_nuc<NW>(kh, p)]++;
+    const uint32_t curm = max(max(cnt[0], cnt[1]), max(cnt[2], cnt[3]));
+    if (math_ls((double)curm, (double)K * ap.ratio)) return;
+    uint8_t f = 0;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+        if (!(m & (1u << c))) continue;
+        Kmer<NW> nx = kh;
+        kmer_shl<NW>(nx, K, c);
+        const uint8_t mn = oriented_mask<NW>(v, nx, K);
+        if (!mask_is_junction(mn) && (mn & 15) != 0) continue;          // an edge of length 1: next is a junction or a dead end
+        f |= (uint8_t)(1u << c);
+    }
+    v.set_eflag(slot, o, f);
+    if (f) atomicAdd(&stats[0], (unsigned long long)__popc(f));
+}
+template <int NW, class V>
+__device__ __forceinline__ void at_edges_apply(const V &v, const uint64_t *keys, int64_t n, int K, unsigned long long *stats) {
+    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (tid >= 2 * n) return;
+    const Kmer<NW> key = key_at<NW>(keys, tid >> 1);
+    const Kmer<NW> kh = (tid & 1) ? kmer_rc<NW>(key, K) : key;
+    const CanonIdx<V> ci = canon_lookup<NW>(v, kh, K);
+    const int o = (int)(tid & 1);                                        // kh is the table key (minimal form) iff o == 0
+    const int64_t fid = (int64_t)(2 * v.link_idx(ci.idx)) + o;
+    const uint8_t mine = v.eflag(ci.idx, o);
+    if (!mine) return;
+    const int first = (int)(kh.w[0] & 3);                                // kh[0]
+    for (int c = 0; c < 4; ++c) {
+        if (!(mine & (1u << c))) continue;
+        Kmer<NW> nx = kh;
+        kmer_shl<NW>(nx, K, c);
+        const CanonIdx<V> cn = canon_lookup<NW>(v, nx, K);
+        // the same link seen from the other strand: (rc(next), complement of kh[0]); rc(next) is the table key iff next is NOT minimal
+        const int o2 = cn.is_min ? 1 : 0;
+        const int64_t fid2 = (int64_t)(2 * v.link_idx(cn.idx)) + o2;
+        const int c2 = 3 - first;
+        if ((v.eflag(cn.idx, o2) & (1u << c2)) && (fid2 < fid || (fid2 == fid && c2 < c))) continue;
+        v.clear_bit(ci.idx, (unsigned)(ci.is_min ? c : 7 - c));                        // DeleteOutgoing(kh, c)
+        v.clear_bit(cn.idx, (unsigned)(cn.is_min ? 4 + first : 7 - (4 + first)));      // DeleteIncoming(next, kh[0])
+        atomicAdd(&stats[1], 2ull);
+    }
+}
+template <int NW, class V>
+__device__ __forceinline__ void at_tips_probe(const V &v, const uint64_t *keys, int64_t n, int K, AtParams ap, unsigned long long *stats) {
+    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (tid >= 2 * n) return;
+    const Kmer<NW> key = key_at<NW>(keys, tid >> 1);
+    const int o = (int)(tid & 1);
+    const typename V::Ref idx0 = v.template slot<NW>(key);
+    const uint8_t mfw = v.mask(idx0);
+    const uint8_t m0 = o ? inv_byte(mfw) : mfw;
+    if ((m0 & 15) != 0 || uniq4(m0 >> 4) < 0) return;                   // IsDeadEnd && CheckUniqueIncoming
+    const Kmer<NW> start = o ? kmer_rc<NW>(key, K) : key;
+    Kmer<NW> kh = start;
+    uint32_t cnt[4] = {0, 0, 0, 0};
+    uint32_t tsz = 0;
+    uint8_t m = m0;
+    do {                                                                 // walk back to the junction, :292-296
+        ++tsz;
+        cnt[kmer_nuc<NW>(kh, K - 1)]++;
+        kmer_shr<NW>(kh, K, uniq4(m >> 4));
+        m = oriented_mask<NW>(v, kh, K);
+    } while (tsz < ap.max_len && !mask_is_junction(m));
+    if ((m >> 4) == 0 || !mask_is_junction(m)) return;                   // dead start (isolated short edge) or too long, :301-302
+    for (uint32_t p = tsz - 1; p < ap.min_len; ++p) cnt[kmer_nuc<NW>(kh, K - 1 - (int)p)]++;
+    const uint32_t curm = max(max(cnt[0], cnt[1]), max(cnt[2], cnt[3]));
+    if (math_ls((double)curm, (double)max(tsz, ap.min_len) * ap.ratio)) return;
+    // a low-complexity tip: mark its vertices (second walk) and its root
+    const CanonIdx<V> cr = canon_lookup<NW>(v, kh, K);
+    v.root(cr.idx, cr.is_min ? 0 : 1);
+    Kmer<NW> w = start;
+    uint8_t mw = m0;
+    for (uint32_t s2 = 0; s2 < tsz; ++s2) {
+        typename V::Ref idx;
+        if (s2) mw = oriented_mask<NW>(v, w, K, &idx); else idx = idx0;
+        v.mark(idx);
+        kmer_shr<NW>(w, K, uniq4(mw >> 4));
+    }
+    atomicAdd(&stats[2], (unsigned long long)tsz);
+}
+
 // ---- host pieces shared by both builds (graph.cu) ---------------------------------------------------------------------------
+// IsolateVertex for the n marked k-mers of one array of masks (tc_apply_k)
+void launch_isolate(Ctx *ctx, uint8_t *masks, const uint8_t *mark, uint64_t n);
 // the keys of a sweep's flagged records, in final_kmers order, as one compacted list per chunk that has any (so they are never
 // held twice, as a join would)
 struct KeyParts {

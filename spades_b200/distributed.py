@@ -338,7 +338,8 @@ def _assemble_slices(piece, storage, group, what):
 
 
 def assemble_masks(ext, group=None):
-    """DeBruijnGraph.masks of one GPU over the union (early clippers off), from the ranks' slices: on rank 0, None elsewhere"""
+    """DeBruijnGraph.masks of one GPU over the union, from the ranks' slices of a DistributedExtensionIndex (the masks before any
+    clipper) or of a DistributedGraph (after its early clippers): on rank 0, None elsewhere"""
     return _assemble_slices(ext.masks(), ext.kmers, group, "k-mer")
 
 
@@ -350,10 +351,37 @@ def assemble_coverage(ext, group=None):
 class DistributedGraph:
     """this rank's share of the union's condensed graph (DistributedGraphConstructor.ConstructGraph): the unitigs that start at a
     junction it owns, in its final_kmers x out-edge order, then the perfect loops whose leader it owns; with per-bucket counts of
-    both, so that assemble_graph can interleave the ranks' edges into one GPU's order"""
+    both, so that assemble_graph can interleave the ranks' edges into one GPU's order. masks() is this rank's slice of the masks
+    after the early clippers (assemble_masks lays the slices out on rank 0), and the clipper statistics are the union's."""
 
-    def __init__(self, ctx, h, k, num_buckets, owners):
-        self.ctx, self.h, self.k, self.num_buckets, self.owners = ctx, h, k, num_buckets, owners
+    def __init__(self, ctx, h, k, num_buckets, owners, kmers):
+        self.ctx, self.h, self.k, self.num_buckets, self.owners, self.kmers = ctx, h, k, num_buckets, owners, kmers
+        self._tc, self._at = (0, 0, 0), [0, 0, 0, 0]
+
+    def masks(self):
+        """the masks of this rank's k-mers after the early clippers (the extension index's when they were off), in the slot order of
+        its k-mer index"""
+        n = self.kmers.total_kmers()
+        out = np.zeros(max(n, 1), np.uint8)
+        self.ctx.check(self.ctx.L.sgpu_dist_graph_masks(self.h, _p(out), n))
+        return out[:n]
+
+    def tip_clipper_stats(self):
+        """the union's (removed k-mers, tipped junctions, clipped links) of the early tip clipper, as DeBruijnGraph has them"""
+        return self._tc
+
+    def at_clipper_stats(self):
+        """the union's (edges collected, links removed, k-mers removed, clipped tips) of the early A/T clipper, as DeBruijnGraph has them"""
+        return list(self._at)
+
+    def _clipper_counters(self):
+        at, tc, remote = np.zeros(4, np.uint64), np.zeros(3, np.uint64), np.zeros(3, np.uint64)
+        self.ctx.check(self.ctx.L.sgpu_dist_graph_clipper_stats(self.h, _p(at), _p(tc), _p(remote)))
+        return at, tc, remote
+
+    def remote_clipper_stores(self):
+        """this rank's clipper stores that landed in another rank's slice: {"marks", "roots", "clears"}"""
+        return dict(zip(("marks", "roots", "clears"), (int(x) for x in self._clipper_counters()[2])))
 
     def stats(self):
         """(edges, unitig edges, bases, junction batches) of this rank"""
@@ -380,6 +408,12 @@ class DistributedGraph:
         self.ctx.check(self.ctx.L.sgpu_dist_graph_times(self.h, _p(out)))
         return dict(zip(("junctions", "unitigs", "clear_visited", "loops"), (float(x) for x in out)))
 
+    def clipper_times(self):
+        """milliseconds of this rank's early clipper phases (isolate and unlink summed over both clippers)"""
+        out = np.zeros(6, np.float32)
+        self.ctx.check(self.ctx.L.sgpu_dist_graph_clipper_times(self.h, _p(out)))
+        return dict(zip(("at_edges_probe", "at_edges_apply", "at_tips_probe", "tip_probe", "isolate", "unlink"), (float(x) for x in out)))
+
     def free(self):
         if self.h:
             self.ctx.L.sgpu_dist_graph_free(self.h); self.h = None
@@ -392,17 +426,21 @@ class DistributedGraph:
 
 
 class DistributedGraphConstructor:
-    """UnbranchingPathExtractor over the ranks of a torch.distributed process group, from each rank's DistributedExtensionIndex
-    (its Build has run) and the indexes that built it: ConstructGraph gives every rank its share of the edges one GPU's
-    DeBruijnGraphConstructor.ConstructGraph gives over the union (early clippers off); assemble_graph puts them together. The walks
-    read the other ranks' indexes, masks and coverage in place; no rank holds more than its own slices and per-bucket tables. The
-    extension index, sets and indexes must not be freed before the result."""
+    """The Construction stage's early clippers and UnbranchingPathExtractor over the ranks of a torch.distributed process group,
+    from each rank's DistributedExtensionIndex (its Build has run) and the indexes that built it: ConstructGraph gives every rank its
+    share of the edges one GPU's DeBruijnGraphConstructor.ConstructGraph gives over the union with the same options;
+    assemble_graph puts them together. The clippers and the walks read the other ranks' indexes, masks and coverage in place; no
+    rank holds more than its own slices and per-bucket tables. The extension index is not changed (its masks stay the unclipped
+    slice). The extension index, sets and indexes must not be freed before the result."""
 
     def __init__(self, ctx, ext, kpomer_index, kmer_index, group=None):
         self.ctx, self.ext, self.kpomer_index, self.kmer_index, self.group = ctx, ext, kpomer_index, kmer_index, group
 
-    def ConstructGraph(self, keep_perfect_loops=True, budget_bytes=None):
-        """budget_bytes: a fixed budget of the junction batches (tests); None sizes them from the memory left"""
+    def ConstructGraph(self, keep_perfect_loops=True, early_tip_clipper_length=0, early_at_clipper=False, at_ratio=0.8, at_min_length=10,
+                       at_max_length=200, budget_bytes=None):
+        """the options of DeBruijnGraphConstructor.ConstructGraph (every rank passes the same ones); budget_bytes: a fixed budget of
+        the junction batches (tests); None sizes them from the memory left"""
+        import torch
         import torch.distributed as dist
         ctx, L, group, ext = self.ctx, self.ctx.L, self.group, self.ext
         world = dist.get_world_size(group)
@@ -412,12 +450,15 @@ class DistributedGraphConstructor:
         with_cov = self.kpomer_index is not None
         if with_cov != ext.with_coverage:
             raise ValueError("the (k+1)-mer index must be given exactly when the extension index has coverage")
-        # the same checks as DistributedExtensionIndexBuilder: every rank takes part in the same collectives
-        shape = (km.k(), km.num_buckets(), with_cov)
+        from ._lib import SgpuGraphOptions
+        opts = SgpuGraphOptions(1 if keep_perfect_loops else 0, int(early_tip_clipper_length), 1 if early_at_clipper else 0, float(at_ratio),
+                                int(at_min_length), int(at_max_length))
+        # the same checks as DistributedExtensionIndexBuilder: every rank takes part in the same collectives, so the options agree too
+        shape = (km.k(), km.num_buckets(), with_cov) + tuple(getattr(opts, f) for f, _ in opts._fields_)
         shapes = [None] * world
         dist.all_gather_object(shapes, shape, group=group)
         if any(tuple(x) != shape for x in shapes):
-            raise ValueError("the ranks' (k, num_buckets, coverage) differ: %s" % (shapes,))
+            raise ValueError("the ranks' (k, num_buckets, coverage, graph options) differ: %s" % (shapes,))
         bsz_all, owned_all = _ownership(km, group)
         _check_owned_once(bsz_all, owned_all)
         owners = np.ascontiguousarray(owned_all.argmax(axis=0), np.int32)
@@ -428,13 +469,29 @@ class DistributedGraphConstructor:
             powners = np.ascontiguousarray(powned.argmax(axis=0), np.int32)
         ubsz = np.ascontiguousarray(bsz_all.sum(axis=0), np.uint64)
         h = C.c_void_p()
-        ctx.check(L.sgpu_dist_graph_begin(ctx.h, ext.h, _p(owners), _p(powners) if with_cov else None, _p(ubsz), int(budget_bytes or 0), C.byref(h)))
-        g = DistributedGraph(ctx, h, km.k(), km.num_buckets(), owners)
+        ctx.check(L.sgpu_dist_graph_begin_opts(ctx.h, ext.h, _p(owners), _p(powners) if with_cov else None, _p(ubsz), int(budget_bytes or 0),
+                                               C.byref(opts), C.byref(h)))
+        g = DistributedGraph(ctx, h, km.k(), km.num_buckets(), owners, km)
         try:
             def open_peers():
                 _open_peers(ctx, group, lambda out: L.sgpu_dist_graph_ipc_handle(h, out), lambda descs: L.sgpu_dist_graph_open_peers(h, descs),
                             SGPU_DIST_GRAPH_IPC_BYTES)
             open_peers()
+            # the clippers' phases: every rank's probe is over before any rank changes a mask (the snapshot of one GPU's build)
+            phases = []
+            if early_at_clipper:
+                phases += ["at_edges_probe", "at_edges_apply", "at_tips_probe", "isolate", "unlink"]
+            if early_tip_clipper_length:
+                phases += ["tip_probe", "isolate", "unlink"]
+            if phases:
+                for name in phases + ["junctions"]:
+                    ctx.check(getattr(L, "sgpu_dist_graph_" + name)(h))
+                    dist.barrier(group=group)
+                at, tc, _ = g._clipper_counters()            # the union's counters: the sums of the ranks'
+                t = torch.from_numpy(np.concatenate((at, tc)).view(np.int64)).to(_backend_device(group))
+                dist.all_reduce(t, group=group)
+                tot = t.cpu().numpy().view(np.uint64)
+                g._at, g._tc = [int(x) for x in tot[:4]], tuple(int(x) for x in tot[4:])
             ctx.check(L.sgpu_dist_graph_unitigs(h))          # walks through every rank's masks; marks visited k-mers wherever they live
             dist.barrier(group=group)                         # every rank's visited flags are final
             if keep_perfect_loops:
