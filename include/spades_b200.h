@@ -454,6 +454,59 @@ void sgpu_dist_graph_free(sgpu_dist_graph *d);
 int sgpu_graph_from_edges(int k, const char *seq, int64_t nbases, const uint32_t *lens, const uint64_t *link_start, const uint64_t *link_end,
                           const uint32_t *raw_cov, int64_t n, sgpu_graph **out);
 
+/* ---- multi-GPU EdgeIndex refill (one process per GPU): sgpu_edge_index_build over the union of the ranks' edges, from each rank's
+ * sgpu_dist_graph after its walks. Every rank ends with the union's index (serialize, lookup and size give one GPU's bytes and slots)
+ * and the values of its slot range [n r / W, n (r+1) / W) (values: as sgpu_edge_index_values gives them, with the union's edge ids).
+ * K and num_buckets as sgpu_edge_index_build; every rank passes the same ones. unitig_counts_all / loop_counts_all: world x B
+ * (rank-major; B = the graph's k-mer buckets) of every rank's sgpu_dist_graph_bucket_counts, from which each rank numbers its edges
+ * in the order assemble_graph lays them out (more than 2^31 - 2 union edges: SGPU_EUNSUPPORTED).
+ *   begin -> count_begin (an ordinary distributed count, sgpu_dist_*, over this rank's edges; free it before the index) ->
+ *   keys -> ipc_handle -> [all_gather descriptors] -> open_peers ->
+ *   repeat: [barrier] merge [barrier] advance -> [all_reduce SUM live] -> level_done (more = 0: placed) ->
+ *   ranks [barrier] fill [barrier] -> values / serialize / lookup / size / slot_range / times -> free
+ * count_begin: K = k + 1 counts into the graph's k-mer buckets (they only decide which rank owns a key; the index has one segment),
+ * any other K into num_buckets (at most 8192). keys: this rank's set from that count (in HBM), the union's size of each of its
+ * buckets (the sums of every rank's sgpu_kset_bucket_sizes), and, for K = k + 1, whether the index is serialized as the reference's
+ * single-index branch (num_buckets > 1 and at least num_buckets / 2 distinct edge ends in the union; sgpu_edge_index_vertex_prefix_host
+ * gives each rank's part of that decision). keys lays out the union's index on every rank, allocates this rank's slot slice and
+ * inserts its keys into level 0 of its copy. merge: every rank's copy of the current level and of its collision words, read through
+ * the peer mappings, merged into scratch; advance: the merge becomes the level, this rank's keys whose bit was cleared go into the
+ * next level (live: this rank's keys still unplaced); level_done: the union's live keys (SGPU_EUNSUPPORTED when keys remain after
+ * the last level). fill: every window of this rank's edges is put into its slot's owner's slice with a 64-bit system-scope CAS
+ * (open_peers refuses a peer on another device without native peer atomics). Steps out of order are refused with SGPU_EINVAL.
+ * Every rank holds the union's index (about 0.65 B per union key) and, until ranks, collision and merge words of the largest level
+ * (about 1 B per union key). */
+#define SGPU_DIST_EDGE_INDEX_IPC_BYTES 128
+typedef struct sgpu_dist_edge_index sgpu_dist_edge_index;
+int sgpu_dist_edge_index_begin(sgpu_ctx *ctx, const sgpu_dist_graph *dg, int K, int num_buckets, const uint64_t *unitig_counts_all,
+                               const uint64_t *loop_counts_all, sgpu_dist_edge_index **out);
+int sgpu_dist_edge_index_count_begin(sgpu_dist_edge_index *d, int world, int rank, sgpu_dist **out);
+int sgpu_dist_edge_index_keys(sgpu_dist_edge_index *d, const sgpu_kset *keys, const uint64_t *union_bucket_sizes, int single);
+int sgpu_dist_edge_index_ipc_handle(sgpu_dist_edge_index *d, uint8_t *out /* SGPU_DIST_EDGE_INDEX_IPC_BYTES */);
+int sgpu_dist_edge_index_open_peers(sgpu_dist_edge_index *d, const uint8_t *descriptors /* world x SGPU_DIST_EDGE_INDEX_IPC_BYTES */);
+int sgpu_dist_edge_index_merge(sgpu_dist_edge_index *d);
+int sgpu_dist_edge_index_advance(sgpu_dist_edge_index *d, uint64_t *live);
+int sgpu_dist_edge_index_level_done(sgpu_dist_edge_index *d, uint64_t union_live, int *more);
+int sgpu_dist_edge_index_ranks(sgpu_dist_edge_index *d);
+int sgpu_dist_edge_index_fill(sgpu_dist_edge_index *d);
+int sgpu_dist_edge_index_values(const sgpu_dist_edge_index *d, uint64_t *edge_ids, uint32_t *offsets, int64_t n);   /* n = this rank's slots */
+int sgpu_dist_edge_index_k(const sgpu_dist_edge_index *d);
+int64_t sgpu_dist_edge_index_size(const sgpu_dist_edge_index *d);                     /* the union's K-mers (after ranks) */
+int sgpu_dist_edge_index_slot_range(const sgpu_dist_edge_index *d, int64_t *lo, int64_t *hi);
+int64_t sgpu_dist_edge_index_serialized_size(const sgpu_dist_edge_index *d);
+int sgpu_dist_edge_index_serialize(const sgpu_dist_edge_index *d, uint8_t *out, int64_t cap);
+int sgpu_dist_edge_index_lookup(const sgpu_dist_edge_index *d, const uint64_t *keys, int64_t n, uint64_t *out_idx);
+/* host milliseconds spent so far in: begin (edge numbers and packing), keys, the levels (merges and advances), ranks, fill, values */
+int sgpu_dist_edge_index_times(const sgpu_dist_edge_index *d, float *out6);
+void sgpu_dist_edge_index_free(sgpu_dist_edge_index *d);
+/* pure host arithmetic (no GPU): the union number of each of a rank's edges (unitig edges first, then loops, as its sgpu_dist_graph
+ * lists them), as above; the sorted distinct vertex slots (LinkRecord >> 2; an end of ~0 is none) of n edges, the first
+ * ceil(num_buckets / 2) of them into out (returns how many, -1 for bad arguments); a rank's slot range of n slots */
+int sgpu_dist_edge_numbers_host(int world, int rank, int num_buckets, const int32_t *owners, const uint64_t *unitig_counts_all,
+                                const uint64_t *loop_counts_all, uint64_t unitig_edges, uint64_t edges, uint64_t *out);
+int64_t sgpu_edge_index_vertex_prefix_host(const uint64_t *link_start, const uint64_t *link_end, int64_t n, int num_buckets, uint64_t *out);
+int sgpu_dist_slot_range_host(uint64_t n, int world, int rank, uint64_t *lo, uint64_t *hi);
+
 /* self tests of the shared host/device arithmetic (tests only): op 0 = xxh3_64, 1 = xxh3_128 lo, 2 = xxh3_128 hi, 3 = bucket(arg),
  * 4 = is_minimal, 5.. = rc word j. keys: n records of ceil(K/32) words. on_device != 0 runs the same code in a kernel. */
 int sgpu_selftest(sgpu_ctx *ctx, int on_device, int op, int K, uint64_t arg, const uint64_t *keys, int64_t n, uint64_t *out);

@@ -39,6 +39,12 @@ SYMBOLS = [
     "sgpu_dist_graph_begin_opts", "sgpu_dist_graph_at_edges_probe", "sgpu_dist_graph_at_edges_apply", "sgpu_dist_graph_at_tips_probe",
     "sgpu_dist_graph_tip_probe", "sgpu_dist_graph_isolate", "sgpu_dist_graph_unlink", "sgpu_dist_graph_junctions", "sgpu_dist_graph_masks",
     "sgpu_dist_graph_clipper_stats", "sgpu_dist_graph_clipper_times",
+    "sgpu_dist_edge_index_begin", "sgpu_dist_edge_index_count_begin", "sgpu_dist_edge_index_keys", "sgpu_dist_edge_index_ipc_handle",
+    "sgpu_dist_edge_index_open_peers", "sgpu_dist_edge_index_merge", "sgpu_dist_edge_index_advance", "sgpu_dist_edge_index_level_done",
+    "sgpu_dist_edge_index_ranks", "sgpu_dist_edge_index_fill", "sgpu_dist_edge_index_values", "sgpu_dist_edge_index_k", "sgpu_dist_edge_index_size",
+    "sgpu_dist_edge_index_slot_range", "sgpu_dist_edge_index_serialized_size", "sgpu_dist_edge_index_serialize", "sgpu_dist_edge_index_lookup",
+    "sgpu_dist_edge_index_times", "sgpu_dist_edge_index_free", "sgpu_dist_edge_numbers_host", "sgpu_edge_index_vertex_prefix_host",
+    "sgpu_dist_slot_range_host",
     "sgpu_selftest",
 ]
 
@@ -207,6 +213,27 @@ def load():
     L.sgpu_dist_graph_bucket_counts.restype = i32; L.sgpu_dist_graph_bucket_counts.argtypes = [vp, vp, vp]
     L.sgpu_dist_graph_times.restype = i32; L.sgpu_dist_graph_times.argtypes = [vp, vp]
     L.sgpu_dist_graph_free.restype = None; L.sgpu_dist_graph_free.argtypes = [vp]
+    L.sgpu_dist_edge_index_begin.restype = i32; L.sgpu_dist_edge_index_begin.argtypes = [vp, vp, i32, i32, vp, vp, pp]
+    L.sgpu_dist_edge_index_count_begin.restype = i32; L.sgpu_dist_edge_index_count_begin.argtypes = [vp, i32, i32, pp]
+    L.sgpu_dist_edge_index_keys.restype = i32; L.sgpu_dist_edge_index_keys.argtypes = [vp, vp, vp, i32]
+    for name in ("ipc_handle", "open_peers", "advance", "times"):
+        f = getattr(L, "sgpu_dist_edge_index_" + name)
+        f.restype = i32; f.argtypes = [vp, vp]
+    for name in ("merge", "ranks", "fill"):
+        f = getattr(L, "sgpu_dist_edge_index_" + name)
+        f.restype = i32; f.argtypes = [vp]
+    L.sgpu_dist_edge_index_level_done.restype = i32; L.sgpu_dist_edge_index_level_done.argtypes = [vp, u64, vp]
+    L.sgpu_dist_edge_index_values.restype = i32; L.sgpu_dist_edge_index_values.argtypes = [vp, vp, vp, i64]
+    L.sgpu_dist_edge_index_k.restype = i32; L.sgpu_dist_edge_index_k.argtypes = [vp]
+    L.sgpu_dist_edge_index_size.restype = i64; L.sgpu_dist_edge_index_size.argtypes = [vp]
+    L.sgpu_dist_edge_index_slot_range.restype = i32; L.sgpu_dist_edge_index_slot_range.argtypes = [vp, vp, vp]
+    L.sgpu_dist_edge_index_serialized_size.restype = i64; L.sgpu_dist_edge_index_serialized_size.argtypes = [vp]
+    L.sgpu_dist_edge_index_serialize.restype = i32; L.sgpu_dist_edge_index_serialize.argtypes = [vp, vp, i64]
+    L.sgpu_dist_edge_index_lookup.restype = i32; L.sgpu_dist_edge_index_lookup.argtypes = [vp, vp, i64, vp]
+    L.sgpu_dist_edge_index_free.restype = None; L.sgpu_dist_edge_index_free.argtypes = [vp]
+    L.sgpu_dist_edge_numbers_host.restype = i32; L.sgpu_dist_edge_numbers_host.argtypes = [i32, i32, i32, vp, vp, vp, u64, u64, vp]
+    L.sgpu_edge_index_vertex_prefix_host.restype = i64; L.sgpu_edge_index_vertex_prefix_host.argtypes = [vp, vp, i64, i32, vp]
+    L.sgpu_dist_slot_range_host.restype = i32; L.sgpu_dist_slot_range_host.argtypes = [u64, i32, i32, vp, vp]
     L.sgpu_graph_from_edges.restype = i32; L.sgpu_graph_from_edges.argtypes = [i32, vp, i64, vp, vp, vp, vp, i64, pp]
     L.sgpu_selftest.restype = i32; L.sgpu_selftest.argtypes = [vp, i32, i32, i32, u64, vp, i64, vp]
     _lib = L

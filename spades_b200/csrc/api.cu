@@ -1019,3 +1019,132 @@ extern "C" int sgpu_selftest(sgpu_ctx *ctx, int on_device, int op, int K, uint64
         }
     })
 }
+
+struct sgpu_dist_edge_index { DistEdgeIndex *d; Ctx *c; };
+extern "C" {
+int sgpu_dist_edge_index_begin(sgpu_ctx *ctx, const sgpu_dist_graph *dg, int K, int num_buckets, const uint64_t *unitig_counts_all,
+                               const uint64_t *loop_counts_all, sgpu_dist_edge_index **out) {
+    if (!ctx || !dg || !unitig_counts_all || !loop_counts_all || !out) return SGPU_EINVAL;
+    *out = nullptr;
+    Ctx *c = &ctx->c;
+    API_TRY(c, {
+        SG_CUDA(cudaSetDevice(c->device));
+        DistEdgeIndex *d = dei_begin(c, dg->d, K, num_buckets, unitig_counts_all, loop_counts_all);
+        *out = new sgpu_dist_edge_index{d, c};
+        child_add(c);
+    })
+}
+int sgpu_dist_edge_index_count_begin(sgpu_dist_edge_index *d, int world, int rank, sgpu_dist **out) {
+    if (!d || !out) return SGPU_EINVAL;
+    *out = nullptr;
+    API_TRY(d->c, {
+        SG_CUDA(cudaSetDevice(d->c->device));
+        DistState *s = dei_count_begin(d->d, world, rank);
+        *out = new sgpu_dist{s, d->c, nullptr};
+        child_add(d->c);
+    })
+}
+int sgpu_dist_edge_index_keys(sgpu_dist_edge_index *d, const sgpu_kset *keys, const uint64_t *union_bucket_sizes, int single) {
+    if (!d || !keys || !union_bucket_sizes) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dei_keys(d->d, keys->s, union_bucket_sizes, single); })
+}
+int sgpu_dist_edge_index_ipc_handle(sgpu_dist_edge_index *d, uint8_t *out) {
+    if (!d || !out) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dei_ipc_handle(d->d, out); })
+}
+int sgpu_dist_edge_index_open_peers(sgpu_dist_edge_index *d, const uint8_t *descriptors) {
+    if (!d || !descriptors) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dei_open_peers(d->d, descriptors); })
+}
+int sgpu_dist_edge_index_merge(sgpu_dist_edge_index *d) {
+    if (!d) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dei_merge(d->d); })
+}
+int sgpu_dist_edge_index_advance(sgpu_dist_edge_index *d, uint64_t *live) {
+    if (!d || !live) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); *live = dei_advance(d->d); })
+}
+int sgpu_dist_edge_index_level_done(sgpu_dist_edge_index *d, uint64_t union_live, int *more) {
+    if (!d || !more) return SGPU_EINVAL;
+    API_TRY(d->c, { *more = dei_level_done(d->d, union_live); })
+}
+int sgpu_dist_edge_index_ranks(sgpu_dist_edge_index *d) {
+    if (!d) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dei_ranks(d->d); })
+}
+int sgpu_dist_edge_index_fill(sgpu_dist_edge_index *d) {
+    if (!d) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dei_fill(d->d); })
+}
+int sgpu_dist_edge_index_values(const sgpu_dist_edge_index *d, uint64_t *edge_ids, uint32_t *offsets, int64_t n) {
+    if (!d || n < 0 || (n && (!edge_ids || !offsets))) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); dei_values(d->d, edge_ids, offsets, n); })
+}
+int sgpu_dist_edge_index_k(const sgpu_dist_edge_index *d) { return d ? dei_k(d->d) : -1; }
+int64_t sgpu_dist_edge_index_size(const sgpu_dist_edge_index *d) {
+    if (!d) return -1;
+    try { return dei_index(d->d)->n; } catch (const sg::Error &e) { d->c->err = e.what(); return -1; }
+}
+int sgpu_dist_edge_index_slot_range(const sgpu_dist_edge_index *d, int64_t *lo, int64_t *hi) {
+    if (!d || !lo || !hi) return SGPU_EINVAL;
+    API_TRY(d->c, {
+        uint64_t a = 0, b = 0;
+        dei_slot_range(d->d, &a, &b);
+        *lo = (int64_t)a; *hi = (int64_t)b;
+    })
+}
+int64_t sgpu_dist_edge_index_serialized_size(const sgpu_dist_edge_index *d) {
+    if (!d) return -1;
+    try { return (int64_t)mphf_serialized_size(dei_index(d->d)); } catch (const sg::Error &e) { d->c->err = e.what(); return -1; }
+}
+int sgpu_dist_edge_index_serialize(const sgpu_dist_edge_index *d, uint8_t *out, int64_t cap) {
+    if (!d || !out || cap < 0) return SGPU_EINVAL;
+    API_TRY(d->c, {
+        SG_CUDA(cudaSetDevice(d->c->device));
+        const Mphf *m = dei_index(d->d);
+        mphf_serialize_to(m, out, (size_t)cap);
+        if (dei_single(d->d)) memset(out + mphf_serialized_size(m) - 8, 0, 8);     // segment_starts_[1] of the single-index branch, as sgpu_edge_index_serialize
+    })
+}
+int sgpu_dist_edge_index_lookup(const sgpu_dist_edge_index *d, const uint64_t *keys, int64_t n, uint64_t *out_idx) {
+    if (!d || n < 0 || (n && (!keys || !out_idx))) return SGPU_EINVAL;
+    API_TRY(d->c, { SG_CUDA(cudaSetDevice(d->c->device)); mphf_lookup_host_keys(d->c, dei_index(d->d), keys, n, out_idx); })
+}
+int sgpu_dist_edge_index_times(const sgpu_dist_edge_index *d, float *out6) {
+    if (!d || !out6) return SGPU_EINVAL;
+    dei_times(d->d, out6);
+    return SGPU_OK;
+}
+void sgpu_dist_edge_index_free(sgpu_dist_edge_index *d) {
+    if (!d) return;
+    Ctx *c = d->c;
+    cudaSetDevice(c->device);
+    dei_free(d->d);
+    delete d;
+    child_release(c);
+}
+int sgpu_dist_edge_numbers_host(int world, int rank, int num_buckets, const int32_t *owners, const uint64_t *unitig_counts_all,
+                                const uint64_t *loop_counts_all, uint64_t unitig_edges, uint64_t edges, uint64_t *out) {
+    if (!owners || !unitig_counts_all || !loop_counts_all || (edges && !out)) return SGPU_EINVAL;
+    try { dist_edge_numbers(world, rank, num_buckets, owners, unitig_counts_all, loop_counts_all, unitig_edges, edges, out); }
+    catch (const sg::Error &e) { return e.code; }
+    return SGPU_OK;
+}
+int64_t sgpu_edge_index_vertex_prefix_host(const uint64_t *link_start, const uint64_t *link_end, int64_t n, int num_buckets, uint64_t *out) {
+    if (n < 0 || num_buckets < 1 || (n && (!link_start || !link_end)) || !out) return -1;
+    try {
+        Graph g;
+        g.link_start.assign(link_start, link_start + n);
+        g.link_end.assign(link_end, link_end + n);
+        g.edge_len.assign((size_t)n, 0);
+        const std::vector<uint64_t> v = edge_vertex_slots(&g, ((uint64_t)num_buckets + 1) / 2);
+        std::copy(v.begin(), v.end(), out);
+        return (int64_t)v.size();
+    } catch (...) { return -1; }
+}
+int sgpu_dist_slot_range_host(uint64_t n, int world, int rank, uint64_t *lo, uint64_t *hi) {
+    if (world < 1 || rank < 0 || rank >= world || !lo || !hi) return SGPU_EINVAL;
+    *lo = dist_slot_lo(n, world, rank); *hi = dist_slot_lo(n, world, rank + 1);
+    return SGPU_OK;
+}
+}  // extern "C"

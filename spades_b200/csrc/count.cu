@@ -2372,6 +2372,26 @@ DistState *dist_begin(Ctx *ctx, int K, int B, int mode, int world, int rank, boo
     return dist_start(d, ctx, K, B, world, rank, mode == kCanonical, mode == kCanonical && K % 2 == 0, result_on_host, nullptr);
 }
 
+// dist_begin's canonical count over packed sequences other than the context's reads (the edges of a distributed EdgeIndex refill,
+// dist_edge_index.cu); they must stay on the device until the count is freed
+DistState *dist_begin_packed(Ctx *ctx, const uint64_t *words, uint64_t nwords, const uint64_t *offs, const uint32_t *lens, int64_t n, int K, int B,
+                             int world, int rank) {
+    SG_CHECK(K >= 1 && K <= 128, 2, "K must be in [1,128]");
+    check_dist_args(B, world, rank);
+    ctx->times = PhaseTimes();
+    ReadsSrc src;
+    src.words = words; src.offs = offs; src.lens = lens; src.n = n; src.nwords = nwords; src.K = K;
+    std::vector<ReadsSrc> srcs{src};
+    DistState *d = nullptr;
+    switch (nwords_of(K)) {
+        case 1: d = dist_state_of<1, ReadsSrc, false>(srcs); break;
+        case 2: d = dist_state_of<2, ReadsSrc, false>(srcs); break;
+        case 3: d = dist_state_of<3, ReadsSrc, false>(srcs); break;
+        default: d = dist_state_of<4, ReadsSrc, false>(srcs); break;
+    }
+    return dist_start(d, ctx, K, B, world, rank, true, K % 2 == 0, false, nullptr);
+}
+
 // the k-mers of this rank's (k+1)-mer set, bucket-owned like dist_begin's count; the records are those of kmers_from_kpomers
 // (no multiplicities). The ranks' sets may overlap: every owner's sort removes the duplicates its pieces bring.
 DistState *dist_begin_kpomers(Ctx *ctx, const KSet *kp, int B, int world, int rank, bool result_on_host) {

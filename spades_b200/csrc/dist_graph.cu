@@ -378,7 +378,7 @@ static void merge_rows(const uint64_t *peer, int levels, int B, int g, const std
 }
 
 // the visible device with this UUID, -1 if none
-static int device_of(const cudaUUID_t &u) {
+int device_of(const cudaUUID_t &u) {
     int n = 0;
     SG_CUDA(cudaGetDeviceCount(&n));
     for (int i = 0; i < n; ++i) {
@@ -509,6 +509,9 @@ void dgraph_masks(const DistGraph *d, uint8_t *out, int64_t n) {
     SG_CHECK(d->next == d->phases.size(), 2, "the early clippers and the junction list have not run");
     SG_CHECK((uint64_t)n == d->nk, 2, "mask array size != number of this rank's k-mers");
     if (n) SG_CUDA(cudaMemcpy(out, d->clip ? d->masks_final.p : d->ext.masks, (size_t)n, cudaMemcpyDeviceToHost));
+}
+DistGraphInfo dgraph_info(const DistGraph *d) {
+    return DistGraphInfo{d->ctx, d->world, d->rank, d->B, d->K, &d->owner, &d->ucnt, &d->lcnt, d->unitig_edges, &d->edges};
 }
 void dgraph_free(DistGraph *d) { delete d; }
 

@@ -19,45 +19,10 @@
 #include <thread>
 #include <vector>
 
-#include "graph.h"
+#include "edge_dev.cuh"
 #include "host_par.h"
-#include "mphf_dev.cuh"
 
 namespace sg {
-
-static const uint32_t kEdgeInfoTombstone = 0x7ffffffeu;       // EdgeInfo::TOMBSTONE: -2u without the PicoSpinLock bit (edge_position_index.hpp:29-30)
-static const uint32_t kEdgeInfoCleared = 0x7fffffffu;         // EdgeInfo::CLEARED
-
-struct UnitigTable {
-    const uint64_t *words;      // 2-bit packed primary strands, each on a word boundary
-    const uint64_t *woff;       // [E] first word
-    const uint32_t *len;        // [E] nucleotides
-    const uint8_t *selfc;       // [E] the edge is its own conjugate
-    const uint64_t *wstart;     // [E+1] exclusive prefix of the windows per edge (both strands counted, self-conjugate once)
-    int64_t E;
-};
-
-// work item -> (edge, strand, offset); K-mer of the conjugate strand at offset j = rc of the primary window at L - K - j
-template <int NW>
-__device__ __forceinline__ bool edge_window(const UnitigTable &u, int K, uint64_t w, uint32_t *edge, int *strand, uint32_t *off, Kmer<NW> *k) {
-    int64_t lo = 0, hi = u.E - 1;
-    while (lo < hi) {                                                   // last edge whose first window index is <= w
-        const int64_t mid = (lo + hi + 1) >> 1;
-        if (u.wstart[mid] <= w) lo = mid; else hi = mid - 1;
-    }
-    const uint32_t L = u.len[lo];
-    if (L < (uint32_t)K) return false;
-    const uint32_t nwin = L - (uint32_t)K + 1;
-    uint32_t j = (uint32_t)(w - u.wstart[lo]);
-    int s = 0;
-    if (j >= nwin) { j -= nwin; s = 1; }
-    const uint64_t *seq = u.words + u.woff[lo];
-    const Kmer<NW> f = kmer_window<NW>(seq, (int64_t)(s == 0 ? j : nwin - 1 - j), K);
-    const Kmer<NW> r = kmer_rc<NW>(f, K);
-    *k = s == 0 ? f : r;                                                // the window as it stands on this strand
-    *edge = (uint32_t)lo; *strand = s; *off = j;
-    return s == 0 ? kmer_is_minimal<NW>(f, r) : kmer_is_minimal<NW>(r, f);      // kwh.is_minimal(): only minimal windows are put
-}
 
 template <int NW>
 __global__ void edge_occ_k(UnitigTable u, int K, uint64_t nwork, MphfDev m, uint32_t *__restrict__ occ) {
@@ -104,27 +69,20 @@ __global__ void fill_u32_k(uint32_t *__restrict__ p, uint64_t n, uint32_t v) {
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) p[i] = v;
 }
 
-EdgeIndex *edge_index_build(Ctx *ctx, const Graph *g, int K, int B) {
-    if (K == 0) K = g->k + 1;
-    SG_CHECK(K >= 1 && K <= g->k + 1 && K <= 128, 2, "edge index: K must be in [1, k+1]");
-    SG_CHECK(B >= 1, 2, "edge index: num_buckets must be >= 1");
-    // K == k+1: the reference takes the K-mers straight from the edges (KMerFullGraphStorage: the edges of `num_buckets` = 10 x threads
-    // vertex chunks, ONE index segment). With more than one chunk KMerIndexBuilder takes its "single index parallel over buckets" branch
-    // (kmer_index_builder.hpp:481-493), which never fills segment_starts_[1] -> it serializes as 0; a graph with fewer vertices than
-    // chunks yields one chunk (graph_iterators.hpp:471-498) and the segmented branch, which stores n there.
-    bool single = false;
-    if (K == g->k + 1) {
-        std::vector<uint64_t> vk;
-        vk.reserve(2 * g->edge_len.size());
-        for (size_t i = 0; i < g->edge_len.size(); ++i) {
-            vk.push_back(g->link_start[i] >> 2);
-            if (g->link_end[i] != ~0ull) vk.push_back(g->link_end[i] >> 2);
-        }
-        par_sort(vk, [](uint64_t a, uint64_t b) { return a < b; });
-        const uint64_t vertices = 2 * (uint64_t)(std::unique(vk.begin(), vk.end()) - vk.begin());      // every vertex and its conjugate (k is odd)
-        single = B > 1 && vertices / (uint64_t)B > 0;
-        B = 1;
+std::vector<uint64_t> edge_vertex_slots(const Graph *g, uint64_t cap) {
+    std::vector<uint64_t> vk;
+    vk.reserve(2 * g->edge_len.size());
+    for (size_t i = 0; i < g->edge_len.size(); ++i) {
+        vk.push_back(g->link_start[i] >> 2);
+        if (g->link_end[i] != ~0ull) vk.push_back(g->link_end[i] >> 2);
     }
+    par_sort(vk, [](uint64_t a, uint64_t b) { return a < b; });
+    vk.erase(std::unique(vk.begin(), vk.end()), vk.end());
+    if (vk.size() > cap) vk.resize(cap);
+    return vk;
+}
+
+void edge_pack(Ctx *ctx, const Graph *g, int K, EdgePack *out) {
     cudaStream_t st = ctx->stream;
     const size_t E = g->edge_len.size();
     // ---- unitigs -> 2-bit packed "reads" (primary strand), self-conjugate flags, window prefix
@@ -171,22 +129,43 @@ EdgeIndex *edge_index_build(Ctx *ctx, const Graph *g, int K, int B) {
             for (auto &x : th) x.join();
         }
     }
+    out->words.alloc(ctx, words.size()); out->woff.alloc(ctx, E + 1); out->wstart.alloc(ctx, E + 1);
+    out->lens.alloc(ctx, E + 1);
+    out->selfc.alloc(ctx, E + 8);
+    SG_CUDA(cudaMemcpyAsync(out->words.p, words.data(), words.size() * 8, cudaMemcpyHostToDevice, st));
+    SG_CUDA(cudaMemcpyAsync(out->woff.p, woff.data(), (E + 1) * 8, cudaMemcpyHostToDevice, st));
+    SG_CUDA(cudaMemcpyAsync(out->wstart.p, wstart.data(), (E + 1) * 8, cudaMemcpyHostToDevice, st));
+    SG_CUDA(cudaMemcpyAsync(out->lens.p, lens.data(), (E + 1) * 4, cudaMemcpyHostToDevice, st));
+    SG_CUDA(cudaMemcpyAsync(out->selfc.p, selfc.data(), E + 1, cudaMemcpyHostToDevice, st));
+    SG_CUDA(cudaStreamSynchronize(st));
+    out->nwords = words.size(); out->nwork = wstart[E]; out->E = (int64_t)E;
+}
+
+EdgeIndex *edge_index_build(Ctx *ctx, const Graph *g, int K, int B) {
+    if (K == 0) K = g->k + 1;
+    SG_CHECK(K >= 1 && K <= g->k + 1 && K <= 128, 2, "edge index: K must be in [1, k+1]");
+    SG_CHECK(B >= 1, 2, "edge index: num_buckets must be >= 1");
+    // K == k+1: the reference takes the K-mers straight from the edges (KMerFullGraphStorage: the edges of `num_buckets` = 10 x threads
+    // vertex chunks, ONE index segment). With more than one chunk KMerIndexBuilder takes its "single index parallel over buckets" branch
+    // (kmer_index_builder.hpp:481-493), which never fills segment_starts_[1] -> it serializes as 0; a graph with fewer vertices than
+    // chunks yields one chunk (graph_iterators.hpp:471-498) and the segmented branch, which stores n there.
+    bool single = false;
+    if (K == g->k + 1) {
+        const uint64_t vertices = 2 * (uint64_t)edge_vertex_slots(g, ~0ull).size();      // every vertex and its conjugate (k is odd)
+        single = B > 1 && vertices / (uint64_t)B > 0;
+        B = 1;
+    }
+    cudaStream_t st = ctx->stream;
+    EdgePack pk;
+    edge_pack(ctx, g, K, &pk);
+    const size_t E = (size_t)pk.E;
     EdgeIndex *ei = new EdgeIndex();
     ei->ctx = ctx; ei->K = K; ei->single_segment = single;
     try {
-        DArr<uint64_t> d_words(ctx, words.size()), d_woff(ctx, E + 1), d_wstart(ctx, E + 1);
-        DArr<uint32_t> d_lens(ctx, E + 1);
-        DArr<uint8_t> d_selfc(ctx, E + 8);
-        SG_CUDA(cudaMemcpyAsync(d_words.p, words.data(), words.size() * 8, cudaMemcpyHostToDevice, st));
-        SG_CUDA(cudaMemcpyAsync(d_woff.p, woff.data(), (E + 1) * 8, cudaMemcpyHostToDevice, st));
-        SG_CUDA(cudaMemcpyAsync(d_wstart.p, wstart.data(), (E + 1) * 8, cudaMemcpyHostToDevice, st));
-        SG_CUDA(cudaMemcpyAsync(d_lens.p, lens.data(), (E + 1) * 4, cudaMemcpyHostToDevice, st));
-        SG_CUDA(cudaMemcpyAsync(d_selfc.p, selfc.data(), E + 1, cudaMemcpyHostToDevice, st));
-        SG_CUDA(cudaStreamSynchronize(st));
         // ---- keys: the canonical count over the unitigs (the context's read set is swapped for the duration of the call)
         const uint64_t *sv_w = ctx->d_words, *sv_o = ctx->d_offs; const uint32_t *sv_l = ctx->d_lens;
         const int64_t sv_n = ctx->n_reads; const uint64_t sv_nw = ctx->n_words; const bool sv_dirty = ctx->staged_dirty;
-        ctx->d_words = d_words.p; ctx->d_offs = d_woff.p; ctx->d_lens = d_lens.p; ctx->n_reads = (int64_t)E; ctx->n_words = words.size(); ctx->staged_dirty = false;
+        ctx->d_words = pk.words.p; ctx->d_offs = pk.woff.p; ctx->d_lens = pk.lens.p; ctx->n_reads = (int64_t)E; ctx->n_words = pk.nwords; ctx->staged_dirty = false;
         try { ei->ks = count_from_reads(ctx, K, B, kCanonical); } catch (...) {
             ctx->d_words = sv_w; ctx->d_offs = sv_o; ctx->d_lens = sv_l; ctx->n_reads = sv_n; ctx->n_words = sv_nw; ctx->staged_dirty = sv_dirty;
             throw;
@@ -199,15 +178,13 @@ EdgeIndex *edge_index_build(Ctx *ctx, const Graph *g, int K, int B) {
         ei->offset.alloc(ctx, n + 1, true);
         fill_u32_k<<<ctx->num_sms * 4, 256, 0, st>>>(ei->offset.p, n + 1, kEdgeInfoCleared);
         ctx->launches++;
-        UnitigTable u;
-        u.words = d_words.p; u.woff = d_woff.p; u.len = d_lens.p; u.selfc = d_selfc.p; u.wstart = d_wstart.p; u.E = (int64_t)E;
-        const uint64_t nwork = wstart[E];
+        const UnitigTable u = pk.table();
         if (E) {
             switch (nwords_of(K)) {
-                case 1: edge_index_fill_nw<1>(ctx, ei, u, nwork); break;
-                case 2: edge_index_fill_nw<2>(ctx, ei, u, nwork); break;
-                case 3: edge_index_fill_nw<3>(ctx, ei, u, nwork); break;
-                default: edge_index_fill_nw<4>(ctx, ei, u, nwork); break;
+                case 1: edge_index_fill_nw<1>(ctx, ei, u, pk.nwork); break;
+                case 2: edge_index_fill_nw<2>(ctx, ei, u, pk.nwork); break;
+                case 3: edge_index_fill_nw<3>(ctx, ei, u, pk.nwork); break;
+                default: edge_index_fill_nw<4>(ctx, ei, u, pk.nwork); break;
             }
         }
     } catch (...) { delete ei; throw; }

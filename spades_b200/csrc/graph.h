@@ -64,7 +64,19 @@ void dgraph_times(const DistGraph *d, float *out4);
 void dgraph_clip_times(const DistGraph *d, float *out6);         // A/T edges probe, A/T edges apply, A/T tips probe, tip probe, isolate, unlink
 void dgraph_clip_stats(const DistGraph *d, uint64_t *at4, uint64_t *tc3, uint64_t *remote3);
 void dgraph_masks(const DistGraph *d, uint8_t *out, int64_t n);  // the clipped slice (the extension index's when no clipper ran)
+// what the distributed EdgeIndex refill reads of a rank's share of the graph
+struct DistGraphInfo {
+    Ctx *ctx;
+    int world, rank, B, k;
+    const std::vector<int> *owner;                    // B: the rank owning each k-mer bucket
+    const std::vector<uint64_t> *ucnt, *lcnt;         // B: this rank's unitig edges by start junction's bucket, loop edges by leader's
+    uint64_t unitig_edges;
+    const Graph *edges;
+};
+DistGraphInfo dgraph_info(const DistGraph *d);
 void dgraph_free(DistGraph *d);
+// the visible device with this UUID, -1 if none
+int device_of(const cudaUUID_t &u);
 
 // edge_index.cu : KmerFreeEdgeIndex refill over the graph's own unitigs (alignment/edge_index.hpp, assembly_graph/index/edge_index_builders.hpp)
 struct EdgeIndex {
@@ -78,6 +90,34 @@ struct EdgeIndex {
     ~EdgeIndex();
 };
 EdgeIndex *edge_index_build(Ctx *ctx, const Graph *g, int K, int num_buckets);
+// the sorted distinct vertex slots (LinkRecord >> 2) of g's edge ends, the first `cap` of them
+std::vector<uint64_t> edge_vertex_slots(const Graph *g, uint64_t cap);
+
+// dist_edge_index.cu : the EdgeIndex refill across GPUs (DistributedEdgeIndex), from each rank's share of a distributed graph. Every
+// rank ends with the union's index and the values of its slot range.
+struct DistEdgeIndex;
+DistEdgeIndex *dei_begin(Ctx *ctx, const DistGraph *dg, int K, int num_buckets, const uint64_t *ucnt_all, const uint64_t *lcnt_all);
+DistState *dei_count_begin(DistEdgeIndex *d, int world, int rank);
+void dei_keys(DistEdgeIndex *d, const KSet *ks, const uint64_t *union_bucket_sizes, int single);
+void dei_ipc_handle(DistEdgeIndex *d, uint8_t *out128);
+void dei_open_peers(DistEdgeIndex *d, const uint8_t *descs);
+void dei_merge(DistEdgeIndex *d);
+uint64_t dei_advance(DistEdgeIndex *d);
+int dei_level_done(DistEdgeIndex *d, uint64_t union_live);     // 1: another level follows
+void dei_ranks(DistEdgeIndex *d);
+void dei_fill(DistEdgeIndex *d);
+void dei_values(const DistEdgeIndex *d, uint64_t *ids, uint32_t *offs, int64_t n);
+const Mphf *dei_index(const DistEdgeIndex *d);
+bool dei_single(const DistEdgeIndex *d);
+int dei_k(const DistEdgeIndex *d);
+void dei_slot_range(const DistEdgeIndex *d, uint64_t *lo, uint64_t *hi);
+void dei_times(const DistEdgeIndex *d, float *out6);
+void dei_free(DistEdgeIndex *d);
+// pure host arithmetic (exported for CPU tests): the union number of each of a rank's edges, in assemble_graph's order (the unitig
+// edges bucket by bucket, each bucket's from its owner, then the loop edges bucket by bucket); and a rank's slot range
+void dist_edge_numbers(int world, int rank, int B, const int *owner, const uint64_t *ucnt_all, const uint64_t *lcnt_all, uint64_t unitig_edges,
+                       uint64_t edges, uint64_t *out);
+__host__ __device__ inline uint64_t dist_slot_lo(uint64_t n, int world, int r) { return n * (uint64_t)r / (uint64_t)world; }
 
 // host_graph.cpp : FastGraphFromSequencesConstructor::ConstructGraph + GFAWriter
 std::string graph_gfa(const Graph *g, const char *version);

@@ -181,11 +181,9 @@ MphfDev mphf_dev(const Mphf *m) {
     return d;
 }
 
-template <int NW>
-static void build_nw(Ctx *ctx, const KSet *ks, Mphf *m) {
+std::vector<uint64_t> mphf_geometry(Ctx *ctx, Mphf *m, const std::vector<int64_t> &bsz) {
     cudaStream_t st = ctx->stream;
-    const int B = ks->B;
-    const uint64_t n = (uint64_t)ks->n;
+    const int B = m->B;
     // ---- level geometry on the host, same libm as the reference (BooPHF.h:582-595)
     m->dom.assign((size_t)kLevels * B, 0); m->nchar.assign((size_t)kLevels * B, 0); m->woff.assign((size_t)kLevels * B + 1, 0);
     std::vector<uint64_t> level_start(kLevels + 1, 0);
@@ -194,7 +192,7 @@ static void build_nw(Ctx *ctx, const KSet *ks, Mphf *m) {
         std::vector<double> pcol(B);
         std::vector<uint64_t> hd(B);
         for (int b = 0; b < B; ++b) {
-            uint64_t nb = (uint64_t)ks->bsz[b];
+            uint64_t nb = (uint64_t)bsz[b];
             double gamma = 4.0;
             hd[b] = (uint64_t)ceil((double)nb * gamma);
             pcol[b] = nb ? 1.0 - pow(((gamma * (double)nb - 1) / (gamma * (double)nb)), (double)(nb - 1)) : 0.0;
@@ -204,7 +202,7 @@ static void build_nw(Ctx *ctx, const KSet *ks, Mphf *m) {
             for (int b = 0; b < B; ++b) {
                 const size_t p = (size_t)l * B + b;
                 m->woff[p] = off;
-                if (ks->bsz[b] == 0) { m->dom[p] = 64; m->nchar[p] = 0; continue; }   // empty buckets own no words
+                if (bsz[b] == 0) { m->dom[p] = 64; m->nchar[p] = 0; continue; }   // empty buckets own no words
                 uint64_t d = (((uint64_t)((double)hd[b] * pow(pcol[b], l)) + 63) / 64) * 64;
                 if (d == 0) d = 64;
                 m->dom[p] = d;
@@ -217,9 +215,9 @@ static void build_nw(Ctx *ctx, const KSet *ks, Mphf *m) {
         m->total_words = off;
     }
     m->starts.assign(B + 1, 0);
-    for (int b = 0; b < B; ++b) m->starts[b + 1] = (uint64_t)ks->bsz[b];
+    for (int b = 0; b < B; ++b) m->starts[b + 1] = (uint64_t)bsz[b];
     for (int i = 1; i < B; ++i) m->starts[i] += m->starts[i - 1];            // kmer_index_builder.hpp:492-493 (stops before B)
-    m->bsz = ks->bsz;
+    m->bsz = bsz;
     m->lastrank.assign(B, 0);
     const uint64_t total_words = m->total_words;
     const uint64_t nblocks = total_words / 8;
@@ -230,7 +228,35 @@ static void build_nw(Ctx *ctx, const KSet *ks, Mphf *m) {
     SG_CUDA(cudaMemcpyAsync(m->d_dom.p, m->dom.data(), m->dom.size() * 8, cudaMemcpyHostToDevice, st));
     SG_CUDA(cudaMemcpyAsync(m->d_woff.p, m->woff.data(), m->woff.size() * 8, cudaMemcpyHostToDevice, st));
     SG_CUDA(cudaMemcpyAsync(m->d_starts.p, m->starts.data(), m->starts.size() * 8, cudaMemcpyHostToDevice, st));
-    if (n == 0 || total_words == 0) { SG_CUDA(cudaStreamSynchronize(st)); return; }
+    return level_start;
+}
+
+void mphf_ranks(Ctx *ctx, Mphf *m) {
+    cudaStream_t st = ctx->stream;
+    const int B = m->B;
+    const uint64_t nblocks = m->total_words / 8;
+    DArr<uint32_t> pop(ctx, nblocks + 1);
+    DArr<uint64_t> gscan(ctx, nblocks + 1), piece_base(ctx, (size_t)kLevels * B), d_last(ctx, B);
+    SG_CUDA(cudaMemsetAsync(pop.p + nblocks, 0, 4, st));
+    mphf_blockpop_k<<<div_up((int64_t)nblocks, 256), 256, 0, st>>>(m->bits.p, nblocks, pop.p);
+    ctx->launches++;
+    exclusive_scan_u32_to_u64(ctx, pop.p, gscan.p, nblocks + 1);
+    mphf_piecebase_k<<<div_up(B, 128), 128, 0, st>>>(gscan.p, m->d_woff.p, (uint32_t)B, nblocks, piece_base.p, d_last.p);
+    mphf_ranks_k<<<div_up((int64_t)nblocks, 256), 256, 0, st>>>(gscan.p, m->d_woff.p, piece_base.p, (uint32_t)(kLevels * B), nblocks, m->ranks.p);
+    ctx->launches += 2;
+    SG_CUDA(cudaGetLastError());
+    SG_CUDA(cudaMemcpyAsync(m->lastrank.data(), d_last.p, (size_t)B * 8, cudaMemcpyDeviceToHost, st));
+    SG_CUDA(cudaStreamSynchronize(st));
+    for (int b = 0; b < B; ++b) SG_CHECK(m->lastrank[b] == (uint64_t)m->bsz[b], 6, "internal: MPHF is not minimal (rank total != bucket size)");
+}
+
+template <int NW>
+static void build_nw(Ctx *ctx, const KSet *ks, Mphf *m) {
+    cudaStream_t st = ctx->stream;
+    const int B = ks->B;
+    const uint64_t n = (uint64_t)ks->n;
+    const std::vector<uint64_t> level_start = mphf_geometry(ctx, m, ks->bsz);
+    if (n == 0 || m->total_words == 0) { SG_CUDA(cudaStreamSynchronize(st)); return; }
 
     MphfDev md = mphf_dev(m);
     const uint64_t l0_words = level_start[1] - level_start[0];
@@ -284,20 +310,7 @@ static void build_nw(Ctx *ctx, const KSet *ks, Mphf *m) {
             place(t, (uint64_t)ch.n, ch.b_lo, ch.b_hi);
         });
     }
-    // ---- ranks
-    DArr<uint32_t> pop(ctx, nblocks + 1);
-    DArr<uint64_t> gscan(ctx, nblocks + 1), piece_base(ctx, (size_t)kLevels * B), d_last(ctx, B);
-    SG_CUDA(cudaMemsetAsync(pop.p + nblocks, 0, 4, st));
-    mphf_blockpop_k<<<div_up((int64_t)nblocks, 256), 256, 0, st>>>(m->bits.p, nblocks, pop.p);
-    ctx->launches++;
-    exclusive_scan_u32_to_u64(ctx, pop.p, gscan.p, nblocks + 1);
-    mphf_piecebase_k<<<div_up(B, 128), 128, 0, st>>>(gscan.p, m->d_woff.p, (uint32_t)B, nblocks, piece_base.p, d_last.p);
-    mphf_ranks_k<<<div_up((int64_t)nblocks, 256), 256, 0, st>>>(gscan.p, m->d_woff.p, piece_base.p, (uint32_t)(kLevels * B), nblocks, m->ranks.p);
-    ctx->launches += 2;
-    SG_CUDA(cudaGetLastError());
-    SG_CUDA(cudaMemcpyAsync(m->lastrank.data(), d_last.p, (size_t)B * 8, cudaMemcpyDeviceToHost, st));
-    SG_CUDA(cudaStreamSynchronize(st));
-    for (int b = 0; b < B; ++b) SG_CHECK(m->lastrank[b] == (uint64_t)ks->bsz[b], 6, "internal: MPHF is not minimal (rank total != bucket size)");
+    mphf_ranks(ctx, m);
 }
 
 Mphf *mphf_build(Ctx *ctx, const KSet *ks) {
@@ -431,6 +444,97 @@ void mphf_lookup_host_keys(Ctx *ctx, const Mphf *m, const uint64_t *h_keys, int6
     SG_CUDA(cudaGetLastError());
     SG_CUDA(cudaMemcpyAsync(h_out, dout.p, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->stream));
     SG_CUDA(cudaStreamSynchronize(ctx->stream));
+}
+
+
+// ---- an index over the union of the ranks' keys, placed by every rank together (dist_edge_index.cu drives the steps). A level's
+// bit is set iff exactly one still-unplaced key of the union hashed to it: each rank inserts its own keys into its copy of the
+// level, then the copies are merged (a bit seen twice, within a rank or across ranks, collides), and every rank filters its keys
+// against the merged level before inserting the survivors into the next one.
+__global__ void mphf_merge_k(const uint64_t *const *__restrict__ bits, const uint64_t *const *__restrict__ coll, int world, uint64_t w0, uint64_t nwords,
+                             uint64_t *__restrict__ out) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nwords) return;
+    uint64_t seen = 0, c = 0;
+    for (int r = 0; r < world; ++r) {
+        const uint64_t s = bits[r][w0 + i];
+        c |= coll[r][i] | (seen & s);
+        seen |= s;
+    }
+    out[i] = seen & ~c;
+}
+
+void mphf_place_begin(Ctx *ctx, Mphf *m, MphfPlacer *pl, const KeyTable &t, uint64_t n, const std::vector<uint64_t> &level_start) {
+    cudaStream_t st = ctx->stream;
+    pl->t = t; pl->n_alive = n; pl->alive = nullptr; pl->level = 0; pl->level_start = level_start;
+    const uint64_t l0_words = level_start[1] - level_start[0];
+    pl->coll.alloc(ctx, l0_words + 8, true);
+    pl->scratch.alloc(ctx, l0_words + 8);
+    pl->cnt.alloc(ctx, 1);
+    SG_CUDA(cudaMemsetAsync(pl->coll.p, 0, pl->coll.bytes(), st));
+    if (n) {
+        const MphfDev md = mphf_dev(m);
+        switch (m->nw) {
+            case 1: mphf_insert_k<1><<<div_up((int64_t)n, 256), 256, 0, st>>>(t, nullptr, n, 0, md, level_start[0], pl->coll.p); break;
+            case 2: mphf_insert_k<2><<<div_up((int64_t)n, 256), 256, 0, st>>>(t, nullptr, n, 0, md, level_start[0], pl->coll.p); break;
+            case 3: mphf_insert_k<3><<<div_up((int64_t)n, 256), 256, 0, st>>>(t, nullptr, n, 0, md, level_start[0], pl->coll.p); break;
+            default: mphf_insert_k<4><<<div_up((int64_t)n, 256), 256, 0, st>>>(t, nullptr, n, 0, md, level_start[0], pl->coll.p); break;
+        }
+        ctx->launches++;
+        SG_CUDA(cudaGetLastError());
+    }
+    SG_CUDA(cudaStreamSynchronize(st));
+}
+
+void mphf_place_merge(Ctx *ctx, Mphf *m, MphfPlacer *pl, const uint64_t *const *d_bits, const uint64_t *const *d_coll, int world) {
+    cudaStream_t st = ctx->stream;
+    const int l = pl->level;
+    const uint64_t w0 = pl->level_start[l], nw = pl->level_start[l + 1] - w0;
+    if (nw) {
+        mphf_merge_k<<<div_up((int64_t)nw, 256), 256, 0, st>>>(d_bits, d_coll, world, w0, nw, pl->scratch.p);
+        ctx->launches++;
+        SG_CUDA(cudaGetLastError());
+    }
+    SG_CUDA(cudaStreamSynchronize(st));
+}
+
+uint64_t mphf_place_advance(Ctx *ctx, Mphf *m, MphfPlacer *pl) {
+    cudaStream_t st = ctx->stream;
+    const int l = pl->level;
+    const bool last = (l == kLevels - 2);              // level 23 has no successor bitset: only count what is left
+    const uint64_t w0 = pl->level_start[l], nw = pl->level_start[l + 1] - w0;
+    // the merged level replaces this rank's copy, and its collisions are spent (no peer reads either any more)
+    if (nw) SG_CUDA(cudaMemcpyAsync(m->bits.p + w0, pl->scratch.p, nw * 8, cudaMemcpyDeviceToDevice, st));
+    SG_CUDA(cudaMemsetAsync(pl->coll.p, 0, pl->coll.bytes(), st));
+    const uint64_t n_alive = pl->n_alive;
+    uint64_t c = 0;
+    if (n_alive) {
+        DArr<uint64_t> &next = (l & 1) ? pl->aliveA : pl->aliveB;
+        const uint64_t cap = (l == 0) ? n_alive / 2 + 1024 : n_alive;
+        if (next.n < cap) next.alloc(ctx, cap);
+        SG_CUDA(cudaMemsetAsync(pl->cnt.p, 0, 8, st));
+        const MphfDev md = mphf_dev(m);
+        const int grid = div_up((int64_t)n_alive, 256);
+        const uint64_t nls = last ? 0 : pl->level_start[l + 1];
+        switch (m->nw) {
+            case 1: mphf_advance_k<1><<<grid, 256, 0, st>>>(pl->t, pl->alive, n_alive, l, md, next.p, (uint64_t)next.n, pl->cnt.p, last ? 0 : 1, nls, pl->coll.p); break;
+            case 2: mphf_advance_k<2><<<grid, 256, 0, st>>>(pl->t, pl->alive, n_alive, l, md, next.p, (uint64_t)next.n, pl->cnt.p, last ? 0 : 1, nls, pl->coll.p); break;
+            case 3: mphf_advance_k<3><<<grid, 256, 0, st>>>(pl->t, pl->alive, n_alive, l, md, next.p, (uint64_t)next.n, pl->cnt.p, last ? 0 : 1, nls, pl->coll.p); break;
+            default: mphf_advance_k<4><<<grid, 256, 0, st>>>(pl->t, pl->alive, n_alive, l, md, next.p, (uint64_t)next.n, pl->cnt.p, last ? 0 : 1, nls, pl->coll.p); break;
+        }
+        ctx->launches++;
+        SG_CUDA(cudaGetLastError());
+        unsigned long long h = 0;
+        SG_CUDA(cudaMemcpyAsync(&h, pl->cnt.p, 8, cudaMemcpyDeviceToHost, st));
+        SG_CUDA(cudaStreamSynchronize(st));
+        SG_CHECK(h <= next.n, 6, "internal: MPHF survivor list overflow");
+        pl->alive = next.p;
+        c = h;
+    }
+    SG_CUDA(cudaStreamSynchronize(st));
+    pl->n_alive = c;
+    pl->level = l + 1;
+    return c;
 }
 
 }  // namespace sg

@@ -80,4 +80,21 @@ inline KeyTable make_table(const KSet *ks) {
     return t;
 }
 
+// one rank's placement of its own keys into an index over the union (mphf.cu). begin inserts them into level 0 of its copy; then,
+// level by level: merge (every rank's copy of the level and collision words, read through d_bits / d_coll, device arrays of world
+// pointers to the ranks' bits and collision words, into scratch), advance (the merge replaces the level; the keys whose bit was
+// cleared go on into the next level). advance returns the keys of this rank still unplaced.
+struct MphfPlacer {
+    KeyTable t;
+    const uint64_t *alive = nullptr;
+    uint64_t n_alive = 0;
+    int level = 0;
+    std::vector<uint64_t> level_start;
+    DArr<uint64_t> coll, scratch, aliveA, aliveB;   // coll: peers read it
+    DArr<unsigned long long> cnt;
+};
+void mphf_place_begin(Ctx *ctx, Mphf *m, MphfPlacer *pl, const KeyTable &t, uint64_t n, const std::vector<uint64_t> &level_start);
+void mphf_place_merge(Ctx *ctx, Mphf *m, MphfPlacer *pl, const uint64_t *const *d_bits, const uint64_t *const *d_coll, int world);
+uint64_t mphf_place_advance(Ctx *ctx, Mphf *m, MphfPlacer *pl);
+
 }  // namespace sg

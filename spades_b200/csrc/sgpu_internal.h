@@ -474,6 +474,8 @@ struct DistState;
 struct DistPlan;
 DistState *dist_begin(Ctx *ctx, int K, int B, int mode, int world, int rank, bool result_on_host = false);
 DistState *dist_begin_kpomers(Ctx *ctx, const KSet *kp, int B, int world, int rank, bool result_on_host);
+DistState *dist_begin_packed(Ctx *ctx, const uint64_t *words, uint64_t nwords, const uint64_t *offs, const uint32_t *lens, int64_t n, int K, int B,
+                             int world, int rank);
 uint32_t dist_num_partitions(const DistState *d);
 void dist_local_counts(DistState *d, uint64_t *h_out);
 void dist_plan(DistState *d, const uint64_t *cnt_all, uint64_t *total_records);
@@ -527,6 +529,11 @@ void mphf_serialize_to(const Mphf *m, uint8_t *out, size_t cap);
 size_t mphf_serialized_size_buckets(const Mphf *m, int b_lo, int b_hi);
 void mphf_serialize_buckets_to(const Mphf *m, int b_lo, int b_hi, uint8_t *out, size_t cap);
 void mphf_lookup_host_keys(Ctx *ctx, const Mphf *m, const uint64_t *h_keys, int64_t n, uint64_t *h_out);
+// the steps of mphf_build, for an index whose keys are spread over several ranks: the level geometry of B = m->B buckets of these
+// sizes (device tables allocated, bits zeroed; returns the first word of every level, kLevels + 1 entries), and the ranks once
+// every level is placed (each bucket's rank total is checked against its size)
+std::vector<uint64_t> mphf_geometry(Ctx *ctx, Mphf *m, const std::vector<int64_t> &bsz);
+void mphf_ranks(Ctx *ctx, Mphf *m);
 
 static inline int div_up(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 

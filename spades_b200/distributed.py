@@ -12,6 +12,7 @@ from .kmer_index import KMerDiskStorage, SGPU_CANONICAL, SGPU_RESULT_ON_HOST, _p
 
 SGPU_IPC_BYTES = 96
 SGPU_DIST_GRAPH_IPC_BYTES = 256
+SGPU_DIST_EDGE_INDEX_IPC_BYTES = 128
 
 
 def _backend_device(group):
@@ -599,6 +600,195 @@ def assemble_graph(dg, group=None):
             raise ValueError("rank %d's bucket counts do not cover its edges" % r)
     cat = lambda xs, dt: np.concatenate(xs).astype(dt) if xs else np.zeros(0, dt)     # noqa: E731
     return graph_from_edges(dg.k, b"".join(texts), cat(lens, np.uint32), cat(ls, np.uint64), cat(le, np.uint64), cat(rc, np.uint32))
+
+
+def edge_index_vertex_prefix(link_start, link_end, num_buckets):
+    """the sorted distinct vertex slots of edges with these link records, the first ceil(num_buckets / 2) of them (pure host
+    arithmetic): a rank's part of the single-index decision of a DistributedEdgeIndex"""
+    from . import _lib
+    L = _lib.load()
+    ls, le = np.ascontiguousarray(link_start, np.uint64), np.ascontiguousarray(link_end, np.uint64)
+    if len(ls) != len(le) or int(num_buckets) < 1:
+        raise ValueError("link arrays of different lengths, or num_buckets < 1")
+    out = np.zeros((int(num_buckets) + 1) // 2 + 1, np.uint64)
+    n = L.sgpu_edge_index_vertex_prefix_host(_p(ls), _p(le), len(ls), int(num_buckets), _p(out))
+    if n < 0:
+        raise ValueError("bad arguments")
+    return out[:n].copy()
+
+
+def edge_index_single(prefixes, num_buckets):
+    """the single-index flag of the (k+1)-mer EdgeIndex over the union (num_buckets > 1 and 2 x distinct vertex slots >= num_buckets),
+    from every rank's edge_index_vertex_prefix: a rank holding ceil(B / 2) vertices decides it alone, otherwise the lists are whole"""
+    B = int(num_buckets)
+    union = np.unique(np.concatenate([np.asarray(p, np.uint64) for p in prefixes])) if len(prefixes) else np.zeros(0, np.uint64)
+    return B > 1 and len(union) >= (B + 1) // 2
+
+
+def dist_edge_numbers(world, rank, owners, unitig_counts_all, loop_counts_all, unitig_edges, edges):
+    """the union number of each of a rank's edges in assemble_graph's order (pure host arithmetic)"""
+    from . import _lib
+    L = _lib.load()
+    owners = np.ascontiguousarray(owners, np.int32)
+    uc, lc = np.ascontiguousarray(unitig_counts_all, np.uint64), np.ascontiguousarray(loop_counts_all, np.uint64)
+    out = np.zeros(max(int(edges), 1), np.uint64)
+    rc = L.sgpu_dist_edge_numbers_host(int(world), int(rank), len(owners), _p(owners), _p(uc), _p(lc), int(unitig_edges), int(edges), _p(out))
+    if rc:
+        raise ValueError("inconsistent bucket counts (code %d)" % rc)
+    return out[:int(edges)]
+
+
+def slot_range_host(n, world, rank):
+    """[lo, hi): the slots of rank `rank` of a DistributedEdgeIndex over n slots (pure host arithmetic)"""
+    from . import _lib
+    L = _lib.load()
+    lo, hi = C.c_uint64(), C.c_uint64()
+    if L.sgpu_dist_slot_range_host(int(n), int(world), int(rank), C.byref(lo), C.byref(hi)):
+        raise ValueError("bad world size or rank")
+    return int(lo.value), int(hi.value)
+
+
+class DistributedEdgeIndex:
+    """EdgeIndex (graph.EdgeIndex) over the union of the ranks' edges of a DistributedGraph, built across the ranks of a
+    torch.distributed process group. Every rank holds the union's index: K, size(), serialize() and seq_idx() are one GPU's over the
+    union (assembled graph); values() are the (edge id, offset) of this rank's slots, slot_range() = [n r / W, n (r+1) / W), with
+    the union's edge ids (assemble_edge_index_values gathers them). k and num_buckets as graph.EdgeIndex; every rank passes the same
+    arguments. budget_bytes: a fixed budget of every pass of the key count (tests); None plans each pass against the memory every
+    rank has free. The graph may be freed afterwards."""
+    REMOVED, TOMBSTONE = (1 << 64) - 2, 0x7FFFFFFE
+
+    def __init__(self, dg, k=None, num_buckets=None, group=None, budget_bytes=None):
+        import torch
+        import torch.distributed as dist
+        ctx, L = dg.ctx, dg.ctx.L
+        self.ctx, self.h, self.group = ctx, None, group
+        world, rank = dist.get_world_size(group), dist.get_rank(group)
+        K = 0 if k is None else int(k)
+        B = 1 if num_buckets is None else int(num_buckets)
+        # every rank takes part in the same collectives only for one K and one B
+        shape = (K, B, dg.k, dg.num_buckets)
+        shapes = [None] * world
+        dist.all_gather_object(shapes, shape, group=group)
+        if any(tuple(x) != shape for x in shapes):
+            raise ValueError("the ranks' (k, num_buckets) differ: %s" % ([x[:2] for x in shapes],))
+        if not dg.h:
+            raise ValueError("the distributed graph has been freed")
+        e = dg.edges()
+        uc, lc = _all_gather_u64(e["unitig_counts"], group), _all_gather_u64(e["loop_counts"], group)
+        h = C.c_void_p()
+        ctx.check(L.sgpu_dist_edge_index_begin(ctx.h, dg.h, K, B, _p(uc), _p(lc), C.byref(h)))
+        self.h = h
+        self.K = L.sgpu_dist_edge_index_k(h)
+        self.nw = (self.K + 31) // 32
+        self.count_ms = 0.0
+        try:
+            import time
+            t0 = time.perf_counter()
+            keys, self.npass = _distributed_count(ctx, group, lambda w, r, out: L.sgpu_dist_edge_index_count_begin(h, w, r, out), budget_bytes)
+            self.count_ms = (time.perf_counter() - t0) * 1e3
+            try:
+                single = False
+                if self.K == dg.k + 1:
+                    prefixes = [None] * world
+                    dist.all_gather_object(prefixes, edge_index_vertex_prefix(e["link_start"], e["link_end"], B), group=group)
+                    single = edge_index_single(prefixes, B)
+                ubsz = np.ascontiguousarray(_all_gather_u64(keys.bucket_sizes().astype(np.uint64), group).sum(axis=0), np.uint64)
+                ctx.check(L.sgpu_dist_edge_index_keys(h, keys.h, _p(ubsz), 1 if single else 0))
+                _open_peers(ctx, group, lambda out: L.sgpu_dist_edge_index_ipc_handle(h, out), lambda descs: L.sgpu_dist_edge_index_open_peers(h, descs),
+                            SGPU_DIST_EDGE_INDEX_IPC_BYTES)
+                dev = _backend_device(group)
+                self.levels = 0
+                while True:
+                    dist.barrier(group=group)                  # every rank's copy of the level is complete
+                    ctx.check(L.sgpu_dist_edge_index_merge(h))
+                    dist.barrier(group=group)                  # nobody reads my level or collision words any more
+                    live = C.c_uint64()
+                    ctx.check(L.sgpu_dist_edge_index_advance(h, C.byref(live)))
+                    t = torch.tensor([live.value], dtype=torch.int64, device=dev)
+                    dist.all_reduce(t, group=group)
+                    more = C.c_int()
+                    ctx.check(L.sgpu_dist_edge_index_level_done(h, int(t.item()), C.byref(more)))
+                    self.levels += 1
+                    if not more.value:
+                        break
+                ctx.check(L.sgpu_dist_edge_index_ranks(h))
+            finally:
+                keys.free()
+            dist.barrier(group=group)                          # every rank's slice is cleared and its copy of the index complete
+            ctx.check(L.sgpu_dist_edge_index_fill(h))
+            dist.barrier(group=group)                          # every put has landed
+        except BaseException:
+            self.free()
+            raise
+
+    def size(self):
+        return int(self.ctx.L.sgpu_dist_edge_index_size(self.h))
+
+    def slot_range(self):
+        lo, hi = C.c_int64(), C.c_int64()
+        self.ctx.check(self.ctx.L.sgpu_dist_edge_index_slot_range(self.h, C.byref(lo), C.byref(hi)))
+        return int(lo.value), int(hi.value)
+
+    def serialize(self) -> bytes:
+        n = self.ctx.L.sgpu_dist_edge_index_serialized_size(self.h)
+        buf = np.zeros(max(n, 1), np.uint8)
+        self.ctx.check(self.ctx.L.sgpu_dist_edge_index_serialize(self.h, _p(buf), n))
+        return buf[:n].tobytes()
+
+    def values(self):
+        """(edge ids u64, offsets u32) of this rank's slots, slot_range() in slot order"""
+        lo, hi = self.slot_range()
+        n = hi - lo
+        ids = np.zeros(max(n, 1), np.uint64); offs = np.zeros(max(n, 1), np.uint32)
+        self.ctx.check(self.ctx.L.sgpu_dist_edge_index_values(self.h, _p(ids), _p(offs), n))
+        return ids[:n], offs[:n]
+
+    def seq_idx(self, keys):
+        keys = np.ascontiguousarray(keys, np.uint64).reshape(-1, self.nw)
+        out = np.zeros(max(len(keys), 1), np.uint64)
+        self.ctx.check(self.ctx.L.sgpu_dist_edge_index_lookup(self.h, _p(keys), len(keys), _p(out)))
+        return out[: len(keys)]
+
+    def times(self):
+        """milliseconds of this rank's begin (edge numbers, packing), key count, keys, levels, ranks, fill and values"""
+        out = np.zeros(6, np.float32)
+        self.ctx.check(self.ctx.L.sgpu_dist_edge_index_times(self.h, _p(out)))
+        t = dict(zip(("pack", "keys", "levels", "ranks", "fill", "values"), (float(x) for x in out)))
+        t["count"] = self.count_ms
+        return t
+
+    def free(self):
+        if self.h:
+            self.ctx.L.sgpu_dist_edge_index_free(self.h); self.h = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+def assemble_edge_index_values(dei, group=None):
+    """graph.EdgeIndex.values of one GPU over the union, from the ranks' slot ranges of a DistributedEdgeIndex: (ids, offsets) on
+    rank 0, None elsewhere"""
+    import torch.distributed as dist
+    rank = dist.get_rank(group)
+    mine = dei.values()
+    pieces = [None] * dist.get_world_size(group) if rank == 0 else None
+    dist.gather_object((dei.slot_range(), mine), pieces, dst=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
+    if rank != 0:
+        return None
+    n = dei.size()
+    ids, offs = np.zeros(n, np.uint64), np.zeros(n, np.uint32)
+    at = 0
+    for (lo, hi), (i, o) in pieces:
+        if lo != at:
+            raise ValueError("the ranks' slot ranges do not tile the index")
+        ids[lo:hi], offs[lo:hi] = i, o
+        at = hi
+    if at != n:
+        raise ValueError("the ranks' slot ranges do not tile the index")
+    return ids, offs
 
 
 def distributed_cov_filter(ctx, k_plus_one, threshold, group=None, apply=True, phase_done=None):
