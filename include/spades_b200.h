@@ -265,6 +265,30 @@ int sgpu_graph_unitigs(const sgpu_graph *g, char *out, uint32_t *lens);
 int64_t sgpu_graph_gfa(const sgpu_graph *g, const char *version, char *out, int64_t cap);   /* returns the text size */
 int sgpu_graph_write_gfa(const sgpu_graph *g, const char *version, const char *path);
 void sgpu_graph_free(sgpu_graph *g);
+/* The graph as FASTG (io::FastgWriter::WriteSegmentsAndLinks, io/graph/fastg_writer.cpp:21-46) and its unitigs as spades-gbuilder's
+ * FASTA (projects/spades_tools/gbuilder.cpp:191-200), formatted on ctx's device. FASTG: one record per edge 3 + 2i, then one for its
+ * conjugate 4 + 2i unless it is self-conjugate; header ">EDGE_<3+2i>_length_<bases>_cov_<%f of raw / (bases - k)>" ("'" on the
+ * conjugate), then ':' and the end vertex's outgoing edges' names in byte order, then ";"; the sequence wrapped at 60. Unitigs:
+ * ">EDGE_<i+1>_length_<bases>" and the sequence wrapped at 60. The text is built in runs of whole records in a device buffer sized
+ * from the memory the context may still use (one record larger than a third of it fails with SGPU_ENOMEM); each run is copied out
+ * through pinned host memory while the next is formatted. A device graph must be given its own context; a host-only graph
+ * (sgpu_graph_from_edges) any context. _fastg / _unitigs_fasta return the text size (-1 on error) and fill out when it holds the
+ * text, in one pass; with out NULL or too small the text is only measured. */
+int64_t sgpu_graph_fastg(sgpu_ctx *ctx, const sgpu_graph *g, char *out, int64_t cap);
+int sgpu_graph_write_fastg(sgpu_ctx *ctx, const sgpu_graph *g, const char *path);
+int64_t sgpu_graph_unitigs_fasta(sgpu_ctx *ctx, const sgpu_graph *g, char *out, int64_t cap);
+int sgpu_graph_write_unitigs_fasta(sgpu_ctx *ctx, const sgpu_graph *g, const char *path);
+/* the last of those four calls on g: runs formatted (0 when the text only was measured), records, text bytes, device milliseconds
+ * of the formatting kernels and of the copies to pinned host memory, host milliseconds handing the runs to the file or buffer,
+ * building the vertex structure (FASTG only), and from there to the record sizes (record table, upload, size kernel, scans) */
+typedef struct sgpu_format_stats {
+    uint64_t runs, records, bytes;
+    float format_ms, d2h_ms, write_ms, vertices_ms, sizes_ms;
+} sgpu_format_stats;
+int sgpu_graph_format_stats(const sgpu_graph *g, sgpu_format_stats *out);
+/* the formatter's coverage text, std::to_string(raw[i] / den[i]) (den[i] >= 1), into out + 32 i, NUL-terminated: compiled for the
+ * host (on_device = 0, ctx may be NULL) or run on ctx's device */
+int sgpu_format_coverage(sgpu_ctx *ctx, int on_device, const uint32_t *raw, const uint32_t *den, int64_t n, char *out);
 
 /* ---- EdgeIndex refill (the next consumer of the graph in the pipeline): debruijn_graph::EdgeIndex<Graph>::Refill
  * (alignment/edge_index.hpp:88-110, modules/graph_construction.hpp:74-82) = GraphPositionFillingIndexBuilder::BuildIndexFromGraph

@@ -17,10 +17,15 @@
 // This only works because the GPU's MPHF is bit-identical to the one the reference builds: the mask / coverage arrays are indexed
 // by it. Exit code 0 iff the reference, fed with the GPU's arrays, extracts the GPU's unitigs and writes the GPU's GFA.
 //
-//   spades_gbuilder_gpu <reads (FASTA/FASTQ[.gz] or one read per line)> <k> <workdir> [num_buckets=16] [early_tip_length_bound=0] [--host-result]
+//   spades_gbuilder_gpu <reads (FASTA/FASTQ[.gz] or one read per line)> <k> <workdir> [num_buckets=16] [early_tip_length_bound=0]
+//                       [--host-result] [--fastg]
 //
 // --host-result: both counts keep their sets in host memory (SGPU_RESULT_ON_HOST), so they may be larger than the device, and the
 // graph comes from sgpu_graph_build_streamed, which reads the sets chunk by chunk. The checks against the reference are the same.
+// --fastg: also gbuilder's other two outputs. The GPU writes graph.fastg (sgpu_graph_write_fastg) and unitigs.fasta
+// (sgpu_graph_write_unitigs_fasta); the reference writes graph_ref.fastg with io::FastgWriter over its own graph, graph_nocov_ref.fastg
+// with it before FillCoverageAndFlankingFromPHM (what gbuilder without -c writes), and unitigs_ref.fasta with gbuilder's unitig loop
+// (gbuilder.cpp:191-200) over its own unitigs. graph.fastg and unitigs.fasta must equal the reference's byte for byte.
 #include "gpu_kmer_counter.hpp"
 
 #include "kmer_index/ph_map/kmer_maps.hpp"
@@ -31,6 +36,9 @@
 #include "assembly_graph/construction/early_simplification.hpp"
 #include "assembly_graph/graph_support/coverage_filling.hpp"
 #include "io/graph/gfa_writer.hpp"
+#include "io/graph/fastg_writer.hpp"
+#include "io/reads/header_naming.hpp"
+#include "io/reads/osequencestream.hpp"
 #include "utils/logger/log_writers.hpp"
 #include "utils/filesystem/temporary.hpp"
 #include "version.hpp"
@@ -86,10 +94,23 @@ class GpuKmersFromKpomersCounter : public kmers::KMerCounter<RtSeq> {
 
 #define CK(call) do { if (int rc_ = (call)) { fprintf(stderr, "spades_b200 error %d: %s\n", rc_, sgpu_last_error(ctx)); return 4; } } while (0)
 
+static std::string file_text(const std::filesystem::path &p) {
+    std::ifstream f(p, std::ios::binary);
+    std::ostringstream s;
+    s << f.rdbuf();
+    return s.str();
+}
+
 int main(int argc, char **argv) {
-    const bool host_result = argc > 4 && std::string(argv[argc - 1]) == "--host-result";
-    if (host_result) --argc;
-    if (argc < 4) { fprintf(stderr, "usage: %s reads k workdir [num_buckets] [early_tip_length_bound] [--host-result]\n", argv[0]); return 2; }
+    bool host_result = false, fastg = false;
+    while (argc > 4) {                                   // trailing flags, in any order
+        const std::string a = argv[argc - 1];
+        if (a == "--host-result") host_result = true;
+        else if (a == "--fastg") fastg = true;
+        else break;
+        --argc;
+    }
+    if (argc < 4) { fprintf(stderr, "usage: %s reads k workdir [num_buckets] [early_tip_length_bound] [--host-result] [--fastg]\n", argv[0]); return 2; }
     const std::string reads_path = argv[1];
     const unsigned k = (unsigned)atoi(argv[2]);
     const std::filesystem::path workdir = argv[3];
@@ -157,8 +178,27 @@ int main(int argc, char **argv) {
         kmers::BuildIndex(coverage_map, kpomers, 1);                  // the reference's MPHF over the GPU-written (k+1)-mer buckets
         if (coverage_map.values().size() != (size_t)sgpu_kset_size(kpomer_counter.device_set())) { ERROR("(k+1)-mer count differs"); ++bad; }
         else CK(sgpu_graph_coverage(gg, coverage_map.values().data(), (int64_t)coverage_map.values().size()));
+        if (fastg) io::FastgWriter(g, workdir / "graph_nocov_ref.fastg").WriteSegmentsAndLinks();
         omnigraph::FlankingCoverage<DeBruijnGraph> flanking_cov(g, 50);
         FillCoverageAndFlankingFromPHM(coverage_map, g, flanking_cov);
+        if (fastg) {
+            io::FastgWriter(g, workdir / "graph_ref.fastg").WriteSegmentsAndLinks();
+            {
+                size_t idx = 1;
+                std::ofstream f(workdir / "unitigs_ref.fasta");
+                for (const auto &edge : edges) {
+                    f << std::string(">") << io::MakeContigId(idx++, edge.size(), "EDGE") << std::endl;
+                    io::WriteWrapped(edge.str(), f);
+                }
+            }
+            CK(sgpu_graph_write_fastg(ctx, gg, (workdir / "graph.fastg").c_str()));
+            CK(sgpu_graph_write_unitigs_fasta(ctx, gg, (workdir / "unitigs.fasta").c_str()));
+            const std::string gf = file_text(workdir / "graph.fastg"), uf = file_text(workdir / "unitigs.fasta");
+            if (gf != file_text(workdir / "graph_ref.fastg")) { ERROR("the GPU's FASTG differs from the reference's FastgWriter output"); ++bad; }
+            else INFO("FASTG agrees: " << gf.size() << " bytes");
+            if (uf != file_text(workdir / "unitigs_ref.fasta")) { ERROR("the GPU's unitig FASTA differs from the reference's"); ++bad; }
+            else INFO("Unitig FASTA agrees: " << uf.size() << " bytes");
+        }
         std::ostringstream ref_gfa;
         { gfa::GFAWriter w(g, ref_gfa); w.WriteSegmentsAndLinks(); }
         const std::string version = std::string(version::flavour()) + "-" + version::package();      // what GFAWriter prints (gfa_writer.cpp:115)

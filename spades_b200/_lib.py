@@ -46,6 +46,8 @@ SYMBOLS = [
     "sgpu_dist_edge_index_times", "sgpu_dist_edge_index_free", "sgpu_dist_edge_numbers_host", "sgpu_edge_index_vertex_prefix_host",
     "sgpu_dist_slot_range_host",
     "sgpu_selftest",
+    "sgpu_graph_fastg", "sgpu_graph_write_fastg", "sgpu_graph_unitigs_fasta", "sgpu_graph_write_unitigs_fasta", "sgpu_graph_format_stats",
+    "sgpu_format_coverage",
 ]
 
 
@@ -67,6 +69,11 @@ class SgpuTimes(C.Structure):
                 ("sort_oversize_equal", C.c_uint64), ("result_d2h_bytes", C.c_uint64), ("result_d2h_wait_ms", C.c_float),
                 ("stage_h2d_bytes", C.c_uint64), ("graph_junction_batches", C.c_uint64),
                 ("cov_filter_passes", C.c_uint64), ("cov_filter_table_bytes", C.c_uint64)]
+
+
+class SgpuFormatStats(C.Structure):
+    _fields_ = [("runs", C.c_uint64), ("records", C.c_uint64), ("bytes", C.c_uint64), ("format_ms", C.c_float), ("d2h_ms", C.c_float),
+                ("write_ms", C.c_float), ("vertices_ms", C.c_float), ("sizes_ms", C.c_float)]
 
 
 _lib = None
@@ -148,6 +155,12 @@ def load():
     L.sgpu_graph_unitigs.restype = i32; L.sgpu_graph_unitigs.argtypes = [vp, vp, vp]
     L.sgpu_graph_gfa.restype = i64; L.sgpu_graph_gfa.argtypes = [vp, C.c_char_p, vp, i64]
     L.sgpu_graph_write_gfa.restype = i32; L.sgpu_graph_write_gfa.argtypes = [vp, C.c_char_p, C.c_char_p]
+    L.sgpu_graph_fastg.restype = i64; L.sgpu_graph_fastg.argtypes = [vp, vp, vp, i64]
+    L.sgpu_graph_write_fastg.restype = i32; L.sgpu_graph_write_fastg.argtypes = [vp, vp, C.c_char_p]
+    L.sgpu_graph_unitigs_fasta.restype = i64; L.sgpu_graph_unitigs_fasta.argtypes = [vp, vp, vp, i64]
+    L.sgpu_graph_write_unitigs_fasta.restype = i32; L.sgpu_graph_write_unitigs_fasta.argtypes = [vp, vp, C.c_char_p]
+    L.sgpu_graph_format_stats.restype = i32; L.sgpu_graph_format_stats.argtypes = [vp, C.POINTER(SgpuFormatStats)]
+    L.sgpu_format_coverage.restype = i32; L.sgpu_format_coverage.argtypes = [vp, i32, vp, vp, i64, vp]
     L.sgpu_graph_free.restype = None; L.sgpu_graph_free.argtypes = [vp]
     L.sgpu_edge_index_build.restype = i32; L.sgpu_edge_index_build.argtypes = [vp, vp, i32, i32, pp]
     L.sgpu_edge_index_k.restype = i32; L.sgpu_edge_index_k.argtypes = [vp]

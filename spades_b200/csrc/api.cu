@@ -532,6 +532,58 @@ int sgpu_graph_write_gfa(const sgpu_graph *g, const char *version, const char *p
         SG_CHECK(ok, SGPU_EIO, "short write");
     })
 }
+// FASTG / unitig FASTA: a device graph is formatted on its own context, a host-only graph on the one given
+static bool format_ctx_ok(sgpu_ctx *ctx, const sgpu_graph *g) { return ctx && g && (!g->g->ctx || g->g->ctx == &ctx->c); }
+static int64_t graph_text(sgpu_ctx *ctx, const sgpu_graph *g, bool fastg, char *out, int64_t cap) {
+    if (!ctx) return -1;
+    Ctx *c = &ctx->c;
+    if (!format_ctx_ok(ctx, g) || cap < 0) { c->err = "no graph, a negative capacity, or a device graph given another context"; return -1; }
+    try {
+        SG_CUDA(cudaSetDevice(c->device));
+        uint64_t at = 0;
+        return (int64_t)graph_format(c, g->g, fastg, out ? (uint64_t)cap : 0, [&](const char *p, size_t b) { memcpy(out + at, p, b); at += b; });
+    } catch (const std::exception &e) { c->err = e.what(); return -1; }
+}
+static int graph_text_file(sgpu_ctx *ctx, const sgpu_graph *g, bool fastg, const char *path) {
+    if (!ctx) return SGPU_EINVAL;
+    Ctx *c = &ctx->c;
+    if (!format_ctx_ok(ctx, g) || !path) return fail(c, SGPU_EINVAL, "no graph or path, or a device graph given another context");
+    API_TRY(c, {
+        SG_CUDA(cudaSetDevice(c->device));
+        const int fd = open(path, O_WRONLY | O_CREAT | O_TRUNC, 0644);
+        SG_CHECK(fd >= 0, SGPU_EIO, "cannot open the output file for writing");
+        bool ok = true;
+        try {
+            graph_format(c, g->g, fastg, ~0ull, [&](const char *p, size_t b) {
+                while (b && ok) {
+                    const ssize_t w = write(fd, p, std::min<size_t>(b, (size_t)1 << 30));
+                    if (w <= 0) ok = false;
+                    else { p += w; b -= (size_t)w; }
+                }
+            });
+        } catch (...) { close(fd); throw; }
+        ok = close(fd) == 0 && ok;
+        SG_CHECK(ok, SGPU_EIO, "short write");
+    })
+}
+int64_t sgpu_graph_fastg(sgpu_ctx *ctx, const sgpu_graph *g, char *out, int64_t cap) { return graph_text(ctx, g, true, out, cap); }
+int sgpu_graph_write_fastg(sgpu_ctx *ctx, const sgpu_graph *g, const char *path) { return graph_text_file(ctx, g, true, path); }
+int64_t sgpu_graph_unitigs_fasta(sgpu_ctx *ctx, const sgpu_graph *g, char *out, int64_t cap) { return graph_text(ctx, g, false, out, cap); }
+int sgpu_graph_write_unitigs_fasta(sgpu_ctx *ctx, const sgpu_graph *g, const char *path) { return graph_text_file(ctx, g, false, path); }
+int sgpu_graph_format_stats(const sgpu_graph *g, sgpu_format_stats *out) {
+    if (!g || !out) return SGPU_EINVAL;
+    const FormatStats &f = g->g->fmt;
+    *out = sgpu_format_stats{f.runs, f.records, f.bytes, f.format_ms, f.d2h_ms, f.write_ms, f.vertices_ms, f.sizes_ms};
+    return SGPU_OK;
+}
+int sgpu_format_coverage(sgpu_ctx *ctx, int on_device, const uint32_t *raw, const uint32_t *den, int64_t n, char *out) {
+    if (n < 0 || (n && (!raw || !den || !out)) || (on_device && !ctx)) return SGPU_EINVAL;
+    Ctx *c = ctx ? &ctx->c : nullptr;
+    API_TRY(c, {
+        if (on_device) SG_CUDA(cudaSetDevice(c->device));
+        format_cov(c, on_device != 0, raw, den, n, out);
+    })
+}
 int sgpu_edge_index_build(sgpu_ctx *ctx, const sgpu_graph *g, int K, int num_buckets, sgpu_edge_index **out) {
     if (!ctx || !g || !out) return SGPU_EINVAL;
     *out = nullptr;

@@ -1,11 +1,21 @@
 // graph.h -- condensed de Bruijn graph artefacts (device masks/coverage + host unitigs and link records)
 #pragma once
+#include <functional>
 #include <string>
 #include <vector>
 
+#include "host_par.h"
 #include "sgpu_internal.h"
 
 namespace sg {
+
+// what the last FASTG or unitig FASTA formatting of a graph did: runs of whole records formatted into one device buffer, device
+// milliseconds of the formatting kernels and of the copies to pinned host memory, host milliseconds spent writing the text out, and
+// host milliseconds before the first run: the vertex structure, then the record table, its upload, the size kernel and the scans
+struct FormatStats {
+    uint64_t runs = 0, bytes = 0, records = 0;
+    float format_ms = 0, d2h_ms = 0, write_ms = 0, vertices_ms = 0, sizes_ms = 0;
+};
 
 struct Graph {
     Ctx *ctx = nullptr;
@@ -23,6 +33,7 @@ struct Graph {
     std::vector<uint32_t> raw_cov;                // CoverageIndex raw coverage per edge
     uint64_t tc_stats[3] = {0, 0, 0};             // early tip clipper: removed k-mers, tipped junctions, clipped links
     uint64_t at_stats[4] = {0, 0, 0, 0};          // early A/T clipper: edges collected, links removed, k-mers removed, clipped tips
+    mutable FormatStats fmt;                      // the last FASTG or unitig FASTA written (fastg.cu)
 };
 
 struct GraphOptions {
@@ -120,7 +131,26 @@ void dist_edge_numbers(int world, int rank, int B, const int *owner, const uint6
 __host__ __device__ inline uint64_t dist_slot_lo(uint64_t n, int world, int r) { return n * (uint64_t)r / (uint64_t)world; }
 
 // host_graph.cpp : FastGraphFromSequencesConstructor::ConstructGraph + GFAWriter
+// the vertices the link records form: outgoing edge ids (3 + 2i, +1 for a conjugate) of vertex v in lst[lst_off[2v] .. lst_off[2v+1])
+// and of its conjugate in lst[lst_off[2v+1] .. lst_off[2v+2]), each list sorted by id; end_slot[2i + s] is the list slot of the
+// end vertex of edge i (s = 0) or of its conjugate (s = 1; a self-conjugate edge has s = 0 only, its slot 2i+1 stays ~0), filled
+// only when end_slots is set (the FASTG writer needs it, the GFA writer does not)
+struct GraphVertices {
+    size_t V = 0;
+    std::vector<uint8_t> selfc;
+    std::vector<uint64_t> lst_off;
+    raw_vector<uint64_t> lst;
+    raw_vector<uint64_t> end_slot;
+};
+GraphVertices graph_vertices(const Graph *g, Trace &tr, bool end_slots);
 std::string graph_gfa(const Graph *g, const char *version);
 std::vector<std::string> graph_gfa_chunks(const Graph *g, const char *version);   // the same text in consecutive pieces (built on the host threads)
+
+// fastg.cu : FastgWriter::WriteSegmentsAndLinks (fastg = true) or spades-gbuilder's unitig FASTA, formatted on ctx's device in runs
+// of whole records; each run's text is handed to sink(data, bytes) in order while the next run is formatted. A text larger than
+// `cap` bytes is only measured, not formatted. Returns the text's size.
+uint64_t graph_format(Ctx *ctx, const Graph *g, bool fastg, uint64_t cap, const std::function<void(const char *, size_t)> &sink);
+// std::to_string(raw[i] / den[i]) into out + 32 i, NUL-terminated, by the formatter's code on the host or on ctx's device
+void format_cov(Ctx *ctx, bool on_device, const uint32_t *raw, const uint32_t *den, int64_t n, char *out);
 
 }  // namespace sg

@@ -35,12 +35,12 @@ inline void put_u(std::string &s, uint64_t v) {
 
 }  // namespace
 
-std::vector<std::string> graph_gfa_chunks(const Graph *g, const char *version) {
+GraphVertices graph_vertices(const Graph *g, Trace &tr, bool end_slots) {
     const size_t E = g->edge_len.size();
-    const int K = g->k;
-    Trace tr("sgpu gfa");
+    GraphVertices gv;
+    std::vector<uint8_t> &selfc = gv.selfc;
+    selfc.assign(E ? E : 1, 0);
     raw_vector<Rec> recs(2 * E);
-    std::vector<uint8_t> selfc(E ? E : 1, 0);
     par_chunks(E, host_threads_for(E), [&](int, size_t lo, size_t hi) {
         for (size_t i = lo; i < hi; ++i) {
             const uint64_t e = kMinId + 2 * i;
@@ -89,8 +89,10 @@ std::vector<std::string> graph_gfa_chunks(const Graph *g, const char *version) {
         });
     }
     const size_t V = groups.size();
+    gv.V = V;
     // outgoing edge lists of vertex v (slot 2v) and of its conjugate (slot 2v+1), CSR: a vertex group has at most 8 records
-    std::vector<uint64_t> lst_off(2 * V + 1, 0);
+    std::vector<uint64_t> &lst_off = gv.lst_off;
+    lst_off.assign(2 * V + 1, 0);
     const int TV = host_threads_for(V);
     par_chunks(V, TV, [&](int, size_t lo, size_t hi) {
         for (size_t vn = lo; vn < hi; ++vn) {
@@ -105,7 +107,9 @@ std::vector<std::string> graph_gfa_chunks(const Graph *g, const char *version) {
         }
     });
     for (size_t i = 1; i <= 2 * V; ++i) lst_off[i] += lst_off[i - 1];
-    raw_vector<uint64_t> lst(lst_off[2 * V] + 1);
+    raw_vector<uint64_t> &lst = gv.lst;
+    lst.resize(lst_off[2 * V] + 1);
+    if (end_slots) gv.end_slot.assign(2 * E, ~0ull);
     par_chunks(V, TV, [&](int, size_t lo, size_t hi) {
         for (size_t vn = lo; vn < hi; ++vn) {
             const size_t i = groups[vn];
@@ -120,12 +124,29 @@ std::vector<std::string> graph_gfa_chunks(const Graph *g, const char *version) {
                 const int slot = is_start ? side : (side ^ 1);
                 const uint64_t val = is_start ? e : ce;
                 if (slot) lst[p1++] = val; else lst[p0++] = val;
+                // the end vertex of e is v1 when this record is e's end; when it is e's start, the end of conjugate(e) is conjugate(v1)
+                if (!end_slots) continue;
+                if (!is_start) gv.end_slot[2 * ei] = 2 * vn + side;
+                else gv.end_slot[2 * ei + (selfc[ei] ? 0 : 1)] = 2 * vn + (side ^ 1);
             }
             std::sort(lst.begin() + lst_off[2 * vn], lst.begin() + lst_off[2 * vn + 1]);
             std::sort(lst.begin() + lst_off[2 * vn + 1], lst.begin() + lst_off[2 * vn + 2]);
         }
     });
     tr.mark("vertices + edge lists");
+    return gv;
+}
+
+std::vector<std::string> graph_gfa_chunks(const Graph *g, const char *version) {
+    const size_t E = g->edge_len.size();
+    const int K = g->k;
+    Trace tr("sgpu gfa");
+    const GraphVertices gv = graph_vertices(g, tr, false);
+    const std::vector<uint8_t> &selfc = gv.selfc;
+    const std::vector<uint64_t> &lst_off = gv.lst_off;
+    const raw_vector<uint64_t> &lst = gv.lst;
+    const size_t V = gv.V;
+    const int TV = host_threads_for(V);
     const int TE = host_threads_for(E);
     std::vector<std::string> chunks(1 + (size_t)TE + (size_t)TV);
     chunks[0] = std::string("H\tsp:Z:") + version + "\n";

@@ -508,7 +508,8 @@ class DistributedGraphConstructor:
 
 
 class AssembledGraph:
-    """the union's graph from the ranks' edges (assemble_graph): unitigs(), gfa() and write_gfa() as DeBruijnGraph has them"""
+    """the union's graph from the ranks' edges (assemble_graph): unitigs(), gfa() and write_gfa() as DeBruijnGraph has them; the
+    FASTG and unitig FASTA calls take the Context whose device formats them"""
 
     def __init__(self, ctx_lib, h):
         self.L, self.h = ctx_lib, h
@@ -539,6 +540,27 @@ class AssembledGraph:
     def write_gfa(self, path, version="SPAdes-4.3.0-dev"):
         if self.L.sgpu_graph_write_gfa(self.h, version.encode(), str(path).encode()):
             raise self._err()
+
+    def fastg(self, ctx):
+        """the union's FASTG, formatted on the device of Context ctx (any context: the graph lives on the host)"""
+        from .graph import graph_text
+        return graph_text(ctx, self.h, True)
+
+    def write_fastg(self, ctx, path):
+        from .graph import write_graph_text
+        write_graph_text(ctx, self.h, True, path)
+
+    def unitigs_fasta(self, ctx):
+        from .graph import graph_text
+        return graph_text(ctx, self.h, False)
+
+    def write_unitigs_fasta(self, ctx, path):
+        from .graph import write_graph_text
+        write_graph_text(ctx, self.h, False, path)
+
+    def format_stats(self):
+        from .graph import format_stats
+        return format_stats(self.L, self.h)
 
     def free(self):
         if self.h:

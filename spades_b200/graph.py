@@ -6,12 +6,40 @@
         src/common/assembly_graph/construction/debruijn_graph_constructor.hpp:399-406,506-567
   CoverageHashMapBuilder / PHMCoverageFiller histogram   ph_map/coverage_hash_map_builder.hpp:42-56, stages/construction.cpp:404-418
   gfa::GFAWriter                                            io/graph/gfa_writer.cpp:36-116
+  io::FastgWriter, spades-gbuilder's unitig FASTA           io/graph/fastg_writer.cpp:21-46, projects/spades_tools/gbuilder.cpp:191-200
 """
 import ctypes as C
 
 import numpy as np
 
 from .kmer_index import (Context, DeBruijnKMerKMerSplitter, DeBruijnReadKMerSplitter, KMerDiskCounter, KMerIndexBuilder, SpadesGpuError, _p)
+
+
+def graph_text(ctx, h, fastg):
+    """the FASTG (fastg=True) or unitig FASTA of graph handle h, formatted on ctx's device"""
+    f = ctx.L.sgpu_graph_fastg if fastg else ctx.L.sgpu_graph_unitigs_fasta
+    n = f(ctx.h, h, None, 0)
+    if n >= 0:
+        buf = np.zeros(max(n, 1), np.uint8)
+        n = f(ctx.h, h, _p(buf), n)
+    if n < 0:
+        raise SpadesGpuError(ctx.L.sgpu_last_error(ctx.h).decode())
+    return buf[:n].tobytes().decode()
+
+
+def write_graph_text(ctx, h, fastg, path):
+    f = ctx.L.sgpu_graph_write_fastg if fastg else ctx.L.sgpu_graph_write_unitigs_fasta
+    ctx.check(f(ctx.h, h, str(path).encode()))
+
+
+def format_stats(L, h):
+    """what the last FASTG or unitig FASTA call on graph handle h did: runs (formatting runs of whole records), records, bytes,
+    format_ms and d2h_ms (device), write_ms (host)"""
+    from ._lib import SgpuFormatStats
+    st = SgpuFormatStats()
+    if L.sgpu_graph_format_stats(h, C.byref(st)):
+        raise SpadesGpuError("no graph")
+    return {name: getattr(st, name) for name, _ in SgpuFormatStats._fields_}
 
 
 class DeBruijnGraph:
@@ -74,6 +102,23 @@ class DeBruijnGraph:
 
     def write_gfa(self, path, version="SPAdes-4.3.0-dev"):
         self.ctx.check(self.ctx.L.sgpu_graph_write_gfa(self.h, version.encode(), str(path).encode()))
+
+    def fastg(self):
+        """the graph as io::FastgWriter writes it, built on the GPU"""
+        return graph_text(self.ctx, self.h, True)
+
+    def write_fastg(self, path):
+        write_graph_text(self.ctx, self.h, True, path)
+
+    def unitigs_fasta(self):
+        """the unitigs as spades-gbuilder's default mode writes them (>EDGE_<n>_length_<bases>, 60 bases per line), built on the GPU"""
+        return graph_text(self.ctx, self.h, False)
+
+    def write_unitigs_fasta(self, path):
+        write_graph_text(self.ctx, self.h, False, path)
+
+    def format_stats(self):
+        return format_stats(self.ctx.L, self.h)
 
     def free(self):
         if self.h:
